@@ -1,7 +1,7 @@
 #!/usr/bin/env python
-"""bench.py — benchmarks of the B200 DirectXTex backend on the BASELINE.json configurations.
+"""bench.py — benchmarks of the H100 DirectXTex backend on the BASELINE.json configurations.
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--config c2|c3|c4|c5] [--impl reference] [--batch B]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--config c2|c3|c4|c5] [--impl reference] [--batch B] [--dump-outputs DIR]
 
 Default (= the headline, BASELINE.json `metric`, configs[1]):  Mtexels/s BC7 encode, 4096x4096 RGBA32F -> BC7_UNORM,
 TEX_COMPRESS_DEFAULT.  A step = one pass of the hot path over a batch of B (default 32) 4096^2 images per GPU, so that the
@@ -18,6 +18,8 @@ host-pointer C ABI with pinned host buffers (H2D + D2H inside the timed region),
 measured HBM peak, `cpu_baseline` = the UNMODIFIED reference (oracle/_ref) on the host cores on a bounded sample, `parity` =
 the result of this very run checked against the reference (SURVEY 8(d): parity checks run with every measurement).
 `--impl reference` times the reference's own CPU implementation on a bounded sample per step.
+`--dump-outputs DIR` writes what the last timed step computed as DIR/<name>.npy (float32; a fixed, seeded sample of whole blocks or
+pixels where an output is larger than its share of 64 MB), so that two builds can be compared output for output.
 """
 import argparse
 import ctypes as C
@@ -38,28 +40,13 @@ def peaks():
     try:
         return json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json"))), "measured (MEASURED_PEAKS.json)"
     except Exception:
-        return {"hbm_gbs": 6650.0}, "fallback (B200_PROFILING.md)"
-
-
-def ncu_metric(path, key):
-    """value of `key` from a committed ncu summary under profiles/ (None if absent)"""
-    try:
-        for line in open(os.path.join(ROOT, "profiles", path)):
-            parts = line.split()
-            if parts and parts[0] == key:
-                v = float(parts[-1])
-                if len(parts) >= 3 and parts[1].lower().endswith("byte"):          # ncu scales byte counts: normalise to Mbyte
-                    v *= {"byte": 1e-6, "kbyte": 1e-3, "mbyte": 1.0, "gbyte": 1e3}.get(parts[1].lower(), 1.0)
-                return v
-    except Exception:
-        pass
-    return None
+        return {"hbm_gbs": 3350.0}, "fallback (H100 SXM data sheet)"
 
 
 class ClockSampler:
-    """samples nvidia-smi clocks / throttle reasons during the timed region (B200_PROFILING.md recipe)"""
+    """samples nvidia-smi clocks / throttle reasons / power limit during the timed region (read-only queries)"""
     Q = ("clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,"
-         "clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap")
+         "clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap,power.limit,name")
 
     def __init__(self, index):
         self.rows, self.proc, self.index = [], None, index
@@ -79,7 +66,7 @@ class ClockSampler:
 
     def stop(self):
         if not self.proc:
-            return {"sm_mhz": None, "sm_max_mhz": None, "reasons": ["nvidia-smi unavailable"]}
+            return {"sm_mhz": None, "sm_max_mhz": None, "reasons": ["nvidia-smi unavailable"], "power_limit_w": None, "gpu": None}
         time.sleep(0.15)
         self.proc.terminate()
         try:
@@ -90,8 +77,10 @@ class ClockSampler:
         mx = [float(r[1]) for r in self.rows if len(r) >= 7 and r[1].replace(".", "").isdigit()]
         names = ["hw_slowdown", "hw_thermal_slowdown", "sw_thermal_slowdown", "sw_power_cap"]
         reasons = sorted({names[i] for r in self.rows if len(r) >= 7 for i in range(4) if r[3 + i].lower().startswith("active")})
+        pl = [float(r[7]) for r in self.rows if len(r) >= 9 and r[7].replace(".", "").isdigit()]
+        gpu = [r[8] for r in self.rows if len(r) >= 9]
         return {"sm_mhz": float(np.median(sm)) if sm else None, "sm_max_mhz": max(mx) if mx else None,
-                "reasons": reasons, "samples": len(sm)}
+                "reasons": reasons, "samples": len(sm), "power_limit_w": pl[0] if pl else None, "gpu": gpu[0] if gpu else None}
 
 
 def host_threads():
@@ -134,16 +123,14 @@ class C2:
     W = H = 4096
     SRC, DST = 2, 98
     kernel = "k_compress_bc7_tma"     # batches: the TMA-fed persistent kernel (DXB200_OPT_BC7_FEED = 4, automatic); a single image: k_compress_bc7
-    bound_note = ("BC7 mode/partition search is issue-bound, not HBM-bound (SURVEY 8(d)); DRAM traffic = algorithmic bytes; "
-                  "issue-slot utilisation and warp-instructions per block: profiles/r02_ncu_k_compress_bc7.txt")
-    ncu_file = "r02_ncu_k_compress_bc7_tma.txt"
+    bound_note = "BC7 mode/partition search is issue-bound, not HBM-bound (SURVEY 8(d)); DRAM traffic = algorithmic bytes"
     small_sample = {"side": 64}          # the 1-thread rate of the reference is measured on this smaller sample
 
     def __init__(self, args, world):
         self.B = args.batch or 32
         self.world = world
         if self.B == 1:                    # a single image takes the direct kernel under the automatic feed
-            self.kernel, self.ncu_file = "k_compress_bc7", "r02_ncu_k_compress_bc7.txt"
+            self.kernel = "k_compress_bc7"
 
     def workload(self):
         return ("4096x4096 RGBA32F -> BC7_UNORM, TEX_COMPRESS_DEFAULT (BASELINE.json configs[1]); a step = a batch of %d such images per GPU "
@@ -179,6 +166,9 @@ class C2:
         if hr != 0:
             raise ctx.capi.DxTexError(hr, "dxb200_compress_device")
         return e0, e1, self.d_out[i & 1]
+
+    def outputs(self, ctx):
+        return {"bc7_blocks": self.d_out[ctx.last_step & 1].view(-1, 16)}
 
     def alternates(self, ctx):
         """the same batch through the other feed of the BC7 kernel (dxb200_set_option(DXB200_OPT_BC7_FEED, ..)): ms per step, output equal.
@@ -270,7 +260,6 @@ class C3:
     FMT, DST = 10, 95
     kernel = "k_compress_bc6h"
     bound_note = "BC6H mode/shape search is issue-bound; the CUBIC mip kernels of the same step are reported under `kernels`"
-    ncu_file = "r02_ncu_k_compress_bc6h.txt"
     small_sample = {"side": 64}
 
     def __init__(self, args, world):
@@ -321,6 +310,10 @@ class C3:
             raise ctx.capi.DxTexError(hr, "dxb200_compress_device")
         ctx.extra_events.setdefault("mips_cubic", []).append((m0, m1))
         return e0, e1, self.d_out[i & 1]
+
+    def outputs(self, ctx):
+        return {"mip_chain_rgba16f": self.d_chain.view(ctx.torch.float16).view(-1, 4),
+                "bc6h_blocks": self.d_out[ctx.last_step & 1].view(-1, 16)}
 
     def e2e_setup(self, ctx):
         capi = ctx.capi
@@ -402,7 +395,6 @@ class C4:
     TOTAL = 1024
     kernel = "k_compress_bc15_t<77,28>"
     bound_note = "BC3: one thread per block, sequential fp32 Newton fits mandated by bit-exactness (issue bound); BOX mips HBM-bound"
-    ncu_file = "r02_ncu_c4.txt"
     small_sample = {"count": 1}
 
     def __init__(self, args, world):
@@ -460,6 +452,9 @@ class C4:
             raise ctx.capi.DxTexError(hr, "dxb200_compress_device")
         ctx.extra_events.setdefault("mips_box", []).append((m0, m1))
         return e0, e1, self.d_out[i & 1]
+
+    def outputs(self, ctx):
+        return {"mip_chain_rgba8": self.d_chain.view(-1, 4), "bc3_blocks": self.d_out[ctx.last_step & 1].view(-1, 16)}
 
     def e2e_setup(self, ctx):
         capi = ctx.capi
@@ -532,7 +527,6 @@ class C5:
     W = H = 8192
     kernel = "k_convert_vec<61,41>"
     bound_note = "the R8 -> R32F row kernel is HBM-bound (5 B per texel); the BC4 kernel of the same step is reported under `kernels`"
-    ncu_file = "r02_ncu_k_convert_vec.txt"
     small_sample = {"side": 1024}
 
     def __init__(self, args, world):
@@ -586,6 +580,10 @@ class C5:
         ctx.extra_events.setdefault("bc4", []).append((b0, b1))
         ctx.extra_events.setdefault("convert_r32f_to_r8", []).append((r0, r1))
         return e0, e1, self.d_bc[i & 1]
+
+    def outputs(self, ctx):
+        # the row outputs in runs of 64 pixels
+        return {"bc4_blocks": self.d_bc[ctx.last_step & 1].view(-1, 8), "r32f": self.d_f32.view(-1, 64), "r8_roundtrip": self.d_back.view(-1, 64)}
 
     def e2e_setup(self, ctx):
         capi = ctx.capi
@@ -649,6 +647,24 @@ class C5:
 WORKLOADS = {"c2": C2, "c3": C3, "c4": C4, "c5": C5}
 
 
+DUMP_BYTES = 64 * 10**6        # all files of --dump-outputs together, .npy headers included
+
+
+def dump_outputs(wl, ctx, path):
+    """--dump-outputs: every output of the last timed step as float32 DIR/<name>.npy.  An output larger than its share of DUMP_BYTES is
+    represented by a fixed, seeded sample of its rows (whole blocks / pixels, in their original order): the same rows in every run with the
+    same arguments."""
+    torch = ctx.torch
+    outs = wl.outputs(ctx)
+    os.makedirs(path, exist_ok=True)
+    share = (DUMP_BYTES - 1024 * len(outs)) // len(outs) // 4               # float32 values per file
+    for name, rows in outs.items():
+        if rows.numel() > share:
+            idx = np.sort(np.random.default_rng(0).choice(rows.shape[0], share // rows.shape[1], replace=False))
+            rows = rows[torch.from_numpy(idx).to(rows.device)]
+        np.save(os.path.join(path, name + ".npy"), rows.float().cpu().numpy())
+
+
 # =====================================================================================================================
 def run_reference(args):
     """--impl reference: the reference's own CPU implementation of the path (oracle/_ref = the unmodified sources), all host threads,
@@ -688,6 +704,7 @@ def main():
     ap.add_argument("--config", default="c2", choices=sorted(WORKLOADS))
     ap.add_argument("--batch", type=int, default=0, help="images per GPU per step (c4: images in the whole batch); 0 = the config's default")
     ap.add_argument("--gather", default="nccl", choices=["nccl", "none"], help="end-of-step collection of the packed blocks at N>1")
+    ap.add_argument("--dump-outputs", metavar="DIR", help="write the last timed step's outputs (rank 0) as DIR/<name>.npy")
     args = ap.parse_args()
     if args.impl == "reference":
         return run_reference(args)
@@ -768,6 +785,8 @@ def main():
     e1.record()
     barrier()
     ctx.last_step = args.steps - 1
+    if args.dump_outputs and rank == 0:
+        dump_outputs(wl, ctx, args.dump_outputs)
     launches = capi.launch_count() - launches0
     tma_timed = capi.tma_launch_count() - tma0
     clocks = sampler.stop() if rank == 0 else None
@@ -814,18 +833,12 @@ def main():
         u1, sec1, _ = wl.reference_step(ref, **wl.small_sample)
         ref.L.ref_omp_set_threads(threads)
         parity = wl.parity(ctx, ref)
-        traffic = None
-        rd, wr = ncu_metric(wl.ncu_file, "dram__bytes_read.sum"), ncu_metric(wl.ncu_file, "dram__bytes_write.sum")
-        if rd is not None and wr is not None:
-            traffic = (rd + wr) * 1e6
-        inst = ncu_metric(wl.ncu_file, "smsp__inst_executed.sum")
-        issue = ncu_metric(wl.ncu_file, "smsp__issue_active.avg.pct_of_peak_sustained_active")
         out = {
             "metric": wl.metric, "value": value, "unit": "Mtexels/s",
             "n_gpus": world, "steps": args.steps, "warmup": args.warmup, "ms_per_step": ms_per_step,
             "higher_is_better": True, "scaling": wl.scaling, "vs_baseline": None, "dtype": wl.dtype, "data": "synthetic",
             "config": {"workload": wl.workload(), "name": wl.name,
-                       "l2": "inputs per step are far larger than the 126 MB L2 (no flush needed)",
+                       "l2": "inputs per step are far larger than the 50 MB L2 (no flush needed)",
                        "parallelism": "image-per-GPU x%d" % world, "gather": (args.gather if world > 1 else "none"),
                        "timed_region_s": ms_total * 1e-3},
             "clocks": clocks,
@@ -833,10 +846,7 @@ def main():
                     "ms_per_step": float(te[0]), "api": info["api"], "steps": e2e_steps},
             "gpu_launches": int(launches), "tma_launches": int(tma_timed),
             "roofline": {"bound": "hbm", "achieved": achieved, "peak": pk["hbm_gbs"], "unit": "GB/s", "frac": achieved / pk["hbm_gbs"],
-                         "traffic": traffic, "traffic_source": ("dram__bytes_read.sum + dram__bytes_write.sum of one launch, profiles/" + wl.ncu_file) if traffic else None,
                          "peak_source": pk_kind, "kernel": wl.kernel, "kernel_ms": kern_ms, "algorithmic_bytes": wl.algo_bytes(),
-                         "issue_slot_frac": (issue / 100.0) if issue else None,
-                         "warp_inst_per_block": (inst / (4096 * 4096 / 16)) if (inst and args.config == "c2") else None,
                          "note": wl.bound_note},
             "kernels": dict({wl.kernel: kern_ms}, **extra_ms),
             "alternates": alternates,

@@ -1,4 +1,4 @@
-"""directxtex_b200 — B200 (sm_100a) backend for the DirectXTex hot path.
+"""directxtex_b200 — H100 (sm_90a) backend for the DirectXTex hot path.
 
 The product is ``_lib/libdxtex_b200.so`` (CUDA kernels behind the C ABI declared in
 ``include/dxtex_b200.h``) plus the C++ ``namespace DirectX`` mirror in ``host/``.  This Python

@@ -1,4 +1,4 @@
-"""Build libdxtex_b200.so (CUDA kernels + C ABI) in-tree for sm_100a.
+"""Build libdxtex_b200.so (CUDA kernels + C ABI) in-tree for sm_90a (H100).
 
 nvcc cross-compiles without a GPU.  Numeric contract of the build (DESIGN.md):
   -fmad=false            no multiply-add contraction: the BC1-5 / convert / mip kernels must be
@@ -40,7 +40,7 @@ def needs_build():
 
 def _flags():
     return ["-std=c++17", "-O3", "-lineinfo",
-            "-gencode", "arch=compute_100a,code=sm_100a",
+            "-gencode", "arch=compute_90a,code=sm_90a",
             "-fmad=false",
             "-Xcompiler", "-fPIC,-ffp-contract=off,-fvisibility=hidden",
             "-ccbin", "/usr/bin/g++" if os.path.exists("/usr/bin/g++") else "g++",

@@ -1,8 +1,8 @@
 // dxb_api.cu — the extern "C" boundary of libdxtex_b200.so (see include/dxtex_b200.h) and the host
 // logic behind it: argument validation with the reference's HRESULTs, pitch rules, batching,
-// staging of host images through device memory, kernel launches on sm_100a.
+// staging of host images through device memory, kernel launches on sm_90a.
 //
-// Compiled with: nvcc -gencode arch=compute_100a,code=sm_100a -fmad=false (bit-exact fp32 contract
+// Compiled with: nvcc -gencode arch=compute_90a,code=sm_90a -fmad=false (bit-exact fp32 contract
 // of the BC1-5 / convert / mip kernels) -lineinfo.  There is no host implementation of any codec in
 // this file: if CUDA is unavailable every compute entry point returns E_FAIL.
 #include <cuda_runtime.h>
@@ -46,7 +46,7 @@ struct Lane
 struct Device
 {
     int ordinal = 0;
-    int numSMs = 148;
+    int numSMs = 132;
     int numaNode = -1;
     int gridBC15 = 0, gridBC7 = 0, gridBC6H = 0, gridRow = 0;
     std::mutex mu; std::condition_variable cv;
@@ -782,7 +782,7 @@ int32_t launch_mips(const dxb200_image* chain, size_t items, size_t levels, uint
 // =================================================================================================
 extern "C" {
 
-const char* dxb200_version(void) { return "dxtex_b200 0.1 (sm_100a)"; }
+const char* dxb200_version(void) { return "dxtex_b200 0.1 (sm_90a)"; }
 const char* dxb200_last_error(void) { return t_lastError.c_str(); }
 uint64_t dxb200_launch_count(void) { return g_launches.load(); }
 uint64_t dxb200_tma_launch_count(void) { return g_tma_launches.load(); }

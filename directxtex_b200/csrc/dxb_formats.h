@@ -1,5 +1,5 @@
 // dxb_formats.h — DXGI_FORMAT values (public D3D ABI), per-format conversion flags and sizes
-// for the subset of formats the B200 backend implements.  Plain C/C++, host and device.
+// for the subset of formats this backend implements.  Plain C/C++, host and device.
 // Restates: the conversion-flag table DirectXTexConvert.cpp:2960-3047 (CONVF_* at
 // DirectXTexP.h:355-377) and BitsPerPixel DirectXTexUtil.cpp:594.
 #pragma once

@@ -8,15 +8,11 @@
 #include "dxb_launch.h"
 #include "dxb_bc15.cuh"
 
-// Launch shape per destination format, from measurements on B200 (4096^2 RGBA8 / 8192^2 R8; profiles/r02_prof_driver_timings.txt).
-// The encoders are thousands of instructions of mostly straight-line code per block and instruction fetch is their top stall
-// (ncu `no_instruction` 2.3 - 4 cycles per issue, profiles/r02_ncu_c4.txt), so what helps is more resident warps and warps that run the same
-// code at the same time:
-//   registers  BC3 / BC4 / BC5: 64 (32 warps/SM, spills and all): BC3 0.578 -> 0.509 ms, BC4 0.591 -> 0.510 ms.  BC1 / BC2 keep the 16 pixels of
-//              their Newton fit in registers and lose at 64 (0.364 -> 0.471 ms): compiler's choice (168).
-//   CTA shape  BC3: 512 threads that start every block together (one barrier per block): 0.509 -> 0.471 ms, C4 step 54.5 -> 43.9 ms; ncu:
-//              no_instruction 4.05 -> 0.58 cycles per issue.  256 / 384 / 1024 threads and 85 / 128 registers measured within 2 % of it on C4.
-//              BC1 and BC4 lose with big CTAs.
+// Launch shape per destination format.  The encoders are thousands of instructions of mostly straight-line code per block and
+// instruction fetch is their top stall, so what helps is more resident warps and warps that run the same code at the same time:
+//   registers  BC3 / BC4 / BC5: 64 (32 warps/SM, spills and all).  BC1 / BC2 keep the 16 pixels of their Newton fit in registers and
+//              lose at 64: compiler's choice.
+//   CTA shape  BC3: 512 threads that start every block together (one barrier per block).  BC1 and BC4 lose with big CTAs.
 #ifndef DXB_BC3_THREADS
 #define DXB_BC3_THREADS 512u
 #endif

@@ -81,8 +81,7 @@ int dxb_occupancy_bc7()
 //     takes its pixel from the tile with one 128-bit shared load and converts it exactly like the direct kernel does;
 //   * the 4 KB landing buffer is free again as soon as every warp has taken its pixels (the barrier at the top of the iteration), so
 //     the next tile is requested right there and has the whole encode of the current tile to arrive; with it the CTA needs 75.9 KB of
-//     shared memory, which still leaves 3 CTAs per SM resident (requesting behind the encoder's own first barrier instead, to save
-//     this one, measured slower: 4.57 vs 4.43 ms);
+//     shared memory, which still leaves 3 CTAs per SM resident within the 228 KB of an H100 SM;
 //   * tiles are handed out by an atomic counter (blocks with alpha cost more than opaque ones); the counter is read one tile ahead
 //     of the request, so its round trip is off the critical path too.  T.counter == nullptr: statically strided tiles.
 // Eligibility (dxb_launch_bc7_tma): RGBA32F source, full 4x4 blocks only (partial blocks need CompressBC's {0,0,0,1} replication,
@@ -220,13 +219,9 @@ static bool bc7_tma_attr_set()
 
 // mode: 0 = direct kernel only, 1 = TMA with the atomic tile counter, 2 = TMA with statically strided tiles, 3 = TMA with one CTA per
 // tile, 4 = automatic (default): mode 1 for batches of images, the direct kernel for a single image.  DXB200_BC7_TMA / dxb200_set_option
-// select.  Measured on B200 (profiles/r02_prof_driver_timings.txt, r02_bench_lines.jsonl):
-//   one 4096^2 RGBA32F image:      direct 4.30 ms, mode 1 4.41 ms, mode 2 4.75 ms (tile costs differ: static striding loses to any dynamic
-//                                  hand-out), mode 3 4.33 ms
-//   batch of 32 such images (C2):  direct 141.7 ms, mode 1 140.9 ms (one tensor map serves the whole batch: no per-block job search)
-// The feed is not what bounds the encoder (issue-bound, 1 % of HBM); the persistent loop pays two CTA-wide synchronisations per tile
-// (ncu: barrier stall 0.98 vs 0.53 cycles per issue) and saves the job lookup.  Variants tried and dropped: request behind the
-// encoder's own first barrier 4.57 ms, staggered CTA starts 4.42 ms, landing zone aliased onto dead scratch 4.46 ms.
+// select.  Static striding loses to any dynamic hand-out (tile costs differ); for a batch one tensor map serves every image, so the
+// TMA feed saves the per-block job search.  The feed is not what bounds the encoder (issue-bound); the persistent loop pays two
+// CTA-wide synchronisations per tile and saves the job lookup.
 static std::atomic<int> g_bc7_feed{-1};
 int dxb_bc7_get_feed()
 {

@@ -1,5 +1,5 @@
 // dxb_portable.h — compile-time switch that lets the SAME arithmetic source be built
-//   * by nvcc as __device__ code for sm_100a (the product), and
+//   * by nvcc as __device__ code for sm_90a (the product), and
 //   * by g++ as plain host code for tests/emul (a test-only lock-step emulator used to
 //     debug parity on machines without a GPU; it is never linked into the product library).
 // Under nvcc every DXB_DEV function is __device__-only, so the shipped .so contains no
@@ -133,32 +133,16 @@ DXB_DEV float dxb_ssemin(float a, float b) { return (a < b) ? a : b; }
 // explicit fused multiply-add (identical on host and device by IEEE-754 definition)
 DXB_DEV float dxb_fma(float a, float b, float c) { return fmaf(a, b, c); }
 
-// ---- packed pairs of fp32 (sm_100a FFMA2 / FADD2 / FMUL2: two independent IEEE operations in one issue slot).
-// The BC7 encoder is issue-bound, and most of its arithmetic runs on 4-channel vectors = two pairs; each half is an
-// ordinary round-to-nearest fp32 operation (checked on B200 against the scalar instructions over 2^26 operand pairs incl.
-// denormals), so the host emulator (two scalar operations) stays bit-identical -- with ONE rule: ptxas (12.9) contracts
-// mul.rn.f32x2 feeding add.rn.f32x2 into FFMA2 even with -fmad=false, which it never does for the scalar .rn forms.  A packed
-// product may therefore only flow into a packed add / sub when the product is exact (0/1 masks, small integers); everywhere
-// else the code states the fused operation itself (dxb_fma2) so that host and device agree.
-#if DXB_ON_DEVICE && !defined(DXB_SCALAR_F2)
-typedef float2 dxb_f2;
-DXB_DEV dxb_f2 dxb_mk2(float x, float y) { return make_float2(x, y); }
-DXB_DEV dxb_f2 dxb_fma2(dxb_f2 a, dxb_f2 b, dxb_f2 c) { return __ffma2_rn(a, b, c); }
-DXB_DEV dxb_f2 dxb_add2(dxb_f2 a, dxb_f2 b) { return __fadd2_rn(a, b); }
-DXB_DEV dxb_f2 dxb_mul2(dxb_f2 a, dxb_f2 b) { return __fmul2_rn(a, b); }
-#else
+// ---- pairs of fp32.  The BC7 encoder runs most of its arithmetic on 4-channel vectors = two pairs.  sm_90a has no
+// packed fp32 instructions, so each pair is two scalar round-to-nearest operations on host and device alike, and the
+// host emulator stays bit-identical (-fmad=false keeps ptxas from contracting a product into a following add; where the
+// code wants a fused operation it states it with dxb_fma2).
 struct dxb_f2 { float x, y; };
 DXB_DEV dxb_f2 dxb_mk2(float x, float y) { dxb_f2 r; r.x = x; r.y = y; return r; }
 DXB_DEV dxb_f2 dxb_fma2(dxb_f2 a, dxb_f2 b, dxb_f2 c) { return dxb_mk2(fmaf(a.x, b.x, c.x), fmaf(a.y, b.y, c.y)); }
 DXB_DEV dxb_f2 dxb_add2(dxb_f2 a, dxb_f2 b) { return dxb_mk2(a.x + b.x, a.y + b.y); }
 DXB_DEV dxb_f2 dxb_mul2(dxb_f2 a, dxb_f2 b) { return dxb_mk2(a.x * b.x, a.y * b.y); }
-#endif
 DXB_DEV dxb_f2 dxb_sub2(dxb_f2 a, dxb_f2 b) { return dxb_add2(a, dxb_mk2(-b.x, -b.y)); }
-// the same operations issued as two scalar instructions each (experiments: -DDXB_SCALAR_REGION=<n> in dxb_bc7.cuh)
-DXB_DEV dxb_f2 dxb_fma2s(dxb_f2 a, dxb_f2 b, dxb_f2 c) { return dxb_mk2(fmaf(a.x, b.x, c.x), fmaf(a.y, b.y, c.y)); }
-DXB_DEV dxb_f2 dxb_add2s(dxb_f2 a, dxb_f2 b) { return dxb_mk2(a.x + b.x, a.y + b.y); }
-DXB_DEV dxb_f2 dxb_mul2s(dxb_f2 a, dxb_f2 b) { return dxb_mk2(a.x * b.x, a.y * b.y); }
-DXB_DEV dxb_f2 dxb_sub2s(dxb_f2 a, dxb_f2 b) { return dxb_mk2(a.x - b.x, a.y - b.y); }
 DXB_DEV dxb_f2 dxb_bc2(float v) { return dxb_mk2(v, v); }
 
 // ---- IEEE binary16 <-> binary32 (RNE, denormals kept, overflow -> Inf) ----

@@ -1,5 +1,5 @@
 // dxb_warp.cuh — single-source SPMD helpers: the same block-encoder source runs
-//   * on sm_100a by one warp for TWO 4x4 blocks, one per 16-lane half (lane-private scalars, __shfl_sync exchanges), and
+//   * on sm_90a by one warp for TWO 4x4 blocks, one per 16-lane half (lane-private scalars, __shfl_sync exchanges), and
 //   * in tests/emul as a loop over 32 emulated lanes (lane-private values are arrays of 32).
 // Per-lane variables are declared `T v[DXB_NL]` and accessed as `v[L]`; DXB_NL is 1 on the device.
 #pragma once

@@ -1,4 +1,4 @@
-// DirectXTexB200.h — C++ host-side mirror of the part of the DirectXTex public API that the B200 backend
+// DirectXTexB200.h — C++ host-side mirror of the part of the DirectXTex public API that the H100 backend
 // accelerates.  A program written against the reference's DirectXTex.h for this path
 //     ScratchImage out;  HRESULT hr = DirectX::Compress(img, DXGI_FORMAT_BC7_UNORM, TEX_COMPRESS_DEFAULT, 0.5f, out);
 // compiles against this header unchanged and links libdxtex_b200.so instead of libDirectXTex.  Names, argument

@@ -1,4 +1,4 @@
-/* dxtex_b200.h — C ABI of libdxtex_b200.so, the B200 (sm_100a) backend for the DirectXTex hot path:
+/* dxtex_b200.h — C ABI of libdxtex_b200.so, the H100 (sm_90a) backend for the DirectXTex hot path:
  * DirectX::Compress / Decompress-side block codecs, DirectX::Convert, DirectX::GenerateMipMaps.
  *
  * Every entry point names the reference interface it replaces (paths relative to the reference

@@ -2,7 +2,7 @@
 //
 // Lock-step HOST build of the exact arithmetic sources the CUDA kernels are compiled from
 // (directxtex_b200/csrc/*.cuh with DXB_DEV = plain inline).  It exists so that parity against the
-// oracle can be debugged in this GPU-less container; the GPU tests then check the sm_100a build
+// oracle can be debugged in this GPU-less container; the GPU tests then check the sm_90a build
 // against the oracle AND against this emulator.  The product library never contains, loads or
 // calls any of this: there is no CPU fallback.
 //

@@ -266,9 +266,8 @@ def test_bc6h_contract_per_class_on_device(oracle, emul, kind, fmt):
 
 @pytest.mark.parametrize("kind", ["cutout", "alpha_photo", "gradient", "c2"])
 def test_bc7_device_equals_emulator_512(emul, kind):
-    """16384 blocks per class: the packed-fp32 (FFMA2) code paths must round exactly like the scalar host emulator.  (ptxas
-    contracts a packed multiply feeding a packed add; two such sites differed in 1 of ~15000 blocks until the fused form was
-    written explicitly, dxb_portable.h.)"""
+    """16384 blocks per class: the fp32-pair code paths (dxb_portable.h) must round exactly like the host emulator; a product
+    contracted into a following add would differ in a few blocks."""
     img = synth.content_ldr(kind, 512, 512, tolerance.SEED)
     got = capi.compress(img, 512, 512, 2, 98)
     he, em = emul.compress(img, 512, 512, 2, 98)

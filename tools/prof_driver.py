@@ -1,6 +1,5 @@
 #!/usr/bin/env python
-"""Runs each hot-path kernel a few times on device-resident data so that `ncu` can capture it
-(profiles/README.md lists the exact ncu command lines).  Usage: python tools/prof_driver.py [bc7|bc6h|bc15|bc3|dec|rows|rowscubic|rowslinear|all] [reps]"""
+"""Times each hot-path kernel with CUDA events on device-resident data (two warm-up calls, then `reps` calls).  Usage: python tools/prof_driver.py [bc7|bc6h|bc15|bc3|dec|rows|rowscubic|rowslinear|all] [reps]"""
 import ctypes as C
 import os
 import sys
