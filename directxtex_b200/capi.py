@@ -236,6 +236,28 @@ def premultiply_alpha_images(srcs, sizes, fmt, flags=0):
     return outs
 
 
+def generate_mipmaps_images(srcs, w, h, fmt, filter=0, levels=0):
+    """dxb200_generate_mipmaps of several equally sized host images in one call; one chain (ScratchImage layout) per image."""
+    layout, total = F.mip_chain_layout(fmt, w, h, levels)
+    chains = [np.zeros(total, np.uint8) for _ in srcs]
+    for chain, src in zip(chains, srcs):
+        chain[:layout[0][4]] = np.ascontiguousarray(src).view(np.uint8).reshape(-1)[:layout[0][4]]
+    imgs = images([Image(lw, lh, fmt, row, sl, _np_ptr(c) + off) for c in chains for (off, lw, lh, row, sl) in layout])
+    hr = lib.dxb200_generate_mipmaps(imgs, len(chains), len(layout), filter)
+    if hr != 0:
+        raise DxTexError(hr, "dxb200_generate_mipmaps")
+    return chains
+
+
+def resize_images(srcs, w, h, fmt, width, height, filter=0):
+    """dxb200_resize of several equally sized host images in one call; one tightly packed width x height result per image."""
+    srcs, outs = [np.ascontiguousarray(a) for a in srcs], _outputs([(width, height)] * len(srcs), fmt)
+    hr = lib.dxb200_resize(_tight_images(srcs, [(w, h)] * len(srcs), fmt), len(srcs), filter, _tight_images(outs, [(width, height)] * len(srcs), fmt))
+    if hr != 0:
+        raise DxTexError(hr, "dxb200_resize")
+    return outs
+
+
 def convert(src, w, h, src_fmt, dst_fmt, filter=0, threshold=0.5):
     src = np.ascontiguousarray(src)
     if dst_fmt not in F.BYTES_PER_PIXEL:

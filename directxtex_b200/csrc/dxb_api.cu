@@ -2,6 +2,12 @@
 // logic behind it: argument validation with the reference's HRESULTs, pitch rules, batching,
 // staging of host images through device memory, kernel launches on sm_90a.
 //
+// Every host-pointer call stages through one routine, run_staged: whole items (a band and its output, a mip chain, a resize
+// pair) are grouped into chunks that pipeline H2D -> kernels -> D2H over the NSLOT (stream, buffer) slots of a lane.  Band calls
+// (compress, decompress, convert, premultiply) cut images into ~32 MiB bands and stage 48 MiB per chunk; chain and pair calls
+// (generate_mipmaps, resize, mipmaps_compress) stage 80 MiB per chunk.  ScaleMipMapsAlphaForCoverage stages on its own: it
+// downloads with a 2D copy into the caller's pitch and its bisection synchronises on the host.
+//
 // Compiled with: nvcc -gencode arch=compute_90a,code=sm_90a -fmad=false (bit-exact fp32 contract
 // of the BC1-5 / convert / mip kernels) -lineinfo.  There is no host implementation of any codec in
 // this file: if CUDA is unavailable every compute entry point returns E_FAIL.
@@ -27,8 +33,13 @@
 
 namespace {
 
-constexpr int NSLOT = 3;        // (stream, device buffer pair) slots of one lane: H2D / kernel / D2H of consecutive chunks overlap
+constexpr int NSLOT = 3;        // (stream, device buffer) slots of one lane: H2D / kernel / D2H of consecutive chunks overlap
 constexpr int NLANE = 2;        // host-staged calls that can be in flight on one device at the same time (each owns a lane)
+constexpr size_t BAND_BYTES = size_t(32) << 20;     // source + destination bytes of one band of a band call
+constexpr size_t BAND_CHUNK = size_t(48) << 20;     // slot buffer bytes of one chunk of a band call
+// slot buffer bytes of one chunk of a chain or pair call; 80 MiB keeps eleven 1024^2 RGBA8 -> BC3 chains of mipmaps_compress in a
+// chunk: with 64 MiB (nine) its end-to-end time was about 4 % longer (H100 80GB HBM3 at 400 W, DESIGN.md §4)
+constexpr size_t ITEM_CHUNK = size_t(80) << 20;
 
 std::mutex g_mu;                // guards the device table only; calls on different lanes / devices run concurrently
 std::atomic<uint64_t> g_launches{0}, g_tma_launches{0};
@@ -37,8 +48,7 @@ thread_local std::string t_lastError;
 struct Lane
 {
     cudaStream_t streams[NSLOT] = { nullptr, nullptr, nullptr };
-    void* dIn[NSLOT] = { nullptr, nullptr, nullptr };  size_t dInCap[NSLOT] = { 0, 0, 0 };
-    void* dOut[NSLOT] = { nullptr, nullptr, nullptr }; size_t dOutCap[NSLOT] = { 0, 0, 0 };
+    void* buf[NSLOT] = { nullptr, nullptr, nullptr }; size_t cap[NSLOT] = { 0, 0, 0 };
     bool busy = false;
 };
 
@@ -311,6 +321,37 @@ struct DeviceJobs
     void release() { if (d) { cudaFreeAsync(d, s); d = nullptr; } }
 };
 
+// The job table of one launch: one dxb_job per (src[i], dst[i]) whose work units are 4x4 blocks (`blocks`) or pixels, on the
+// host and, for more than one job, on the device; the device copy is released on the launch's stream with the table.
+struct JobTable
+{
+    std::vector<dxb_job> host; DeviceJobs<dxb_job> dev; uint32_t total = 0;
+    ~JobTable() { dev.release(); }
+    int32_t build(const dxb200_image* src, const dxb200_image* dst, size_t n, bool blocks, cudaStream_t stream)
+    {
+        host.resize(n);
+        uint64_t units = 0;
+        for (size_t i = 0; i < n; ++i)
+        {
+            dxb_job& j = host[i];
+            j.src = src[i].pixels; j.dst = dst[i].pixels; j.srcPitch = src[i].rowPitch; j.dstPitch = dst[i].rowPitch;
+            j.width = (uint32_t)src[i].width; j.height = (uint32_t)src[i].height;
+            j.nbx = blocks ? (j.width + 3) / 4 : 0; j.nby = blocks ? (j.height + 3) / 4 : 0;
+            j.firstUnit = (uint32_t)units; j.pad = 0;
+            units += blocks ? (uint64_t)j.nbx * j.nby : (uint64_t)j.width * j.height;
+            if (units > 0x7FFFFFFFull) return DXB_E_INVALIDARG;                // same 2^31-unit limit as CompressBC_Parallel (:258)
+        }
+        total = (uint32_t)units;
+        return dev.upload(host, stream);
+    }
+};
+
+// CTAs for `units` work units at `perCta` units per CTA: at least one, at most `cap`
+uint32_t grid_for(uint32_t units, uint32_t perCta, uint32_t cap)
+{
+    return std::max(1u, std::min((uint32_t)(((uint64_t)units + perCta - 1) / perCta), cap));
+}
+
 int32_t check_launch(const char* name)
 {
     g_launches.fetch_add(1, std::memory_order_relaxed);
@@ -354,74 +395,123 @@ int32_t plan_compress(const dxb200_image* src, size_t n, uint32_t dstFormat, uin
 // enqueue the kernel for images whose pixels already live on the device
 int32_t launch_compress(const CompressPlan& plan, const dxb200_image* src, const dxb200_image* dst, size_t n, cudaStream_t stream)
 {
-    std::vector<dxb_job> jobs(n);
-    uint64_t total = 0;
-    for (size_t i = 0; i < n; ++i)
-    {
-        dxb_job& j = jobs[i];
-        j.src = src[i].pixels; j.dst = dst[i].pixels;
-        j.srcPitch = src[i].rowPitch; j.dstPitch = dst[i].rowPitch;
-        j.width = (uint32_t)src[i].width; j.height = (uint32_t)src[i].height;
-        j.nbx = (j.width + 3) / 4; j.nby = (j.height + 3) / 4;
-        j.firstUnit = (uint32_t)total; j.pad = 0;
-        total += (uint64_t)j.nbx * j.nby;
-        if (total > 0x7FFFFFFFull) return DXB_E_INVALIDARG;                    // same 2^31-block limit as CompressBC_Parallel (:258)
-    }
-    dxb_compress_params P = plan.P;
-    P.totalUnits = (uint32_t)total; P.njobs = (uint32_t)n;
-    // (a periodic job-table lookup for batches of equal mip chains -- one division and a short scan instead of the binary
-    //  search -- was measured slower on C4: 64.3 vs 60.4 ms; the binary search's loads are warp-uniform and stay in L1)
-    P.periodUnits = 0; P.periodJobs = 0;
-    DeviceJobs<dxb_job> dj;
-    int32_t hr = dj.upload(jobs, stream);
+    JobTable jt;
+    const int32_t hr = jt.build(src, dst, n, true, stream);
     if (hr != DXB_S_OK) return hr;
+    dxb_compress_params P = plan.P;
+    P.totalUnits = jt.total; P.njobs = (uint32_t)n;
+    const Device& d = *t_v.dev;
     if (plan.bc6h)
     {
-        const uint32_t need = (uint32_t)((total + 2 * DXB_BC6H_WARPS - 1) / (2 * DXB_BC6H_WARPS));
-        const uint32_t grid = std::max(1u, std::min<uint32_t>(need, (uint32_t)t_v.dev->gridBC6H * 4u));
-        dxb_launch_bc6h(grid, stream, dj.d, jobs[0], P);
-        hr = check_launch("k_compress_bc6h");
+        dxb_launch_bc6h(grid_for(jt.total, 2 * DXB_BC6H_WARPS, (uint32_t)d.gridBC6H * 4u), stream, jt.dev.d, jt.host.data(), P);
+        return check_launch("k_compress_bc6h");
     }
-    else if (plan.bc7)
+    if (plan.bc7)
     {
-        const uint32_t need = (uint32_t)((total + 2 * DXB_BC7_WARPS - 1) / (2 * DXB_BC7_WARPS));
-        // one CTA per 2 * DXB_BC7_WARPS blocks (no grid-stride cap): block costs differ (alpha blocks run the separate-alpha
-        // tasks), so the hardware CTA scheduler balances better than a static stride
-        const uint32_t grid = std::max(1u, need);
-        // RGBA32F sources of full blocks: persistent kernel fed by TMA tile loads; everything else: the direct kernel
-        if (dxb_launch_bc7_tma((unsigned)t_v.dev->gridBC7, stream, jobs.data(), P)) g_tma_launches.fetch_add(1, std::memory_order_relaxed);
-        else dxb_launch_bc7(grid, stream, dj.d, jobs[0], P);
-        hr = check_launch("k_compress_bc7");
+        // RGBA32F sources of full blocks: persistent kernel fed by TMA tile loads; everything else: the direct kernel with one CTA
+        // per 2 * DXB_BC7_WARPS blocks (no grid-stride cap): block costs differ (alpha blocks run the separate-alpha tasks), so the
+        // hardware CTA scheduler balances better than a static stride
+        if (dxb_launch_bc7_tma((unsigned)d.gridBC7, stream, jt.host.data(), P)) g_tma_launches.fetch_add(1, std::memory_order_relaxed);
+        else dxb_launch_bc7(grid_for(jt.total, 2 * DXB_BC7_WARPS, UINT32_MAX), stream, jt.dev.d, jt.host.data(), P);
+        return check_launch("k_compress_bc7");
     }
-    else
-    {
-        const uint32_t need = (uint32_t)((total + 127) / 128);
-        const uint32_t grid = std::max(1u, std::min<uint32_t>(need, (uint32_t)t_v.dev->gridBC15 * 4u));
-        dxb_launch_bc15(grid, stream, dj.d, jobs[0], P);
-        hr = check_launch("k_compress_bc15");
-    }
-    dj.release();
-    return hr;
+    dxb_launch_bc15(grid_for(jt.total, 128, (uint32_t)d.gridBC15 * 4u), stream, jt.dev.d, jt.host.data(), P);
+    return check_launch("k_compress_bc15");
 }
 
 // ---- host staging -------------------------------------------------------------------------------------
-// Host images are cut into BANDS of whole work rows (4 pixel rows per block row on the BC side) of about 32 MiB, and the
-// bands are pushed through NSLOT (stream, device buffer) slots: H2D -> kernel -> D2H of one band overlaps the other
-// slots' copies and kernels (fully when the caller's memory is pinned, see dxb200_host_alloc).  Band boundaries fall on
-// block rows, so the result is identical to processing the whole image at once.
+// How one image of a staged item travels: its host pixels go up before the launch, its device result comes back after the
+// launch, or its bytes are only reserved in device memory (the levels of a chain that is compressed where it is built).
+enum class Copy : uint8_t { Up, Down, None };
+
+// One array of images of a staged call: item i owns images [i * per, (i + 1) * per) of `host`; image 0 of an item travels as
+// `first`, the others as `rest` (a mip chain uploads level 0 and makes the others).
+struct Plane { const dxb200_image* host; size_t per; Copy first, rest; };
+
+// Stages items [0, n) of the planes through the calling thread's lane.  Whole items are grouped into chunks of at most `budget`
+// bytes of device memory (an item larger than that is a chunk by itself), and chunk c goes through slot c % NSLOT, so the H2D
+// copies, kernels and D2H copies of consecutive chunks overlap (fully when the caller's memory is pinned, see
+// dxb200_host_alloc).  In the slot's buffer the chunk's images lie plane after plane, each on a 256-byte boundary, so equal
+// images of one plane sit at a constant stride (the vector kernels' alignment checks and dxb_launch_bc7_tma rely on both).
+// fn(dev, count, stream) enqueues the kernels: dev[p] is plane p's images of the chunk's `count` items, with device pointers.
+// prog (optional) is told before each chunk's upload the units[] of the items the chunk completes, and stops the call between
+// chunks (E_ABORT).  Every slot is synchronised before returning; the first error wins.
+template <typename Fn>
+int32_t run_staged(const Plane* planes, size_t nplanes, size_t n, size_t budget, Fn fn, Progress* prog = nullptr, const size_t* units = nullptr)
+{
+    auto padded = [](const dxb200_image& im) { return (im.slicePitch + 255) & ~size_t(255); };
+    Lane& L = *t_v.lane;
+    std::vector<std::vector<dxb200_image>> dev(nplanes);
+    size_t i = 0; int slot = 0;
+    int32_t hr = DXB_S_OK;
+    while (i < n && hr == DXB_S_OK)
+    {
+        size_t bytes = 0, k = i;
+        while (k < n)
+        {
+            size_t b = 0;
+            for (size_t p = 0; p < nplanes; ++p)
+                for (size_t m = k * planes[p].per; m < (k + 1) * planes[p].per; ++m) b += padded(planes[p].host[m]);
+            if (k > i && bytes + b > budget) break;
+            bytes += b; ++k;
+        }
+        cudaStream_t st = L.streams[slot];
+        hr = cuda_hr(cudaStreamSynchronize(st), "slot sync"); if (hr) break;
+        if (prog)
+        {
+            size_t add = 0;
+            for (size_t m = i; m < k; ++m) add += units[m];
+            if (!prog->report(add)) { hr = DXB_E_ABORT; break; }
+        }
+        hr = ensure_buffer(&L.buf[slot], &L.cap[slot], bytes); if (hr) break;
+        size_t off = 0;
+        for (size_t p = 0; p < nplanes && hr == DXB_S_OK; ++p)
+        {
+            const Plane& pl = planes[p];
+            const dxb200_image* host = pl.host + i * pl.per;
+            dev[p].assign(host, pl.host + k * pl.per);
+            for (size_t m = 0; m < dev[p].size() && hr == DXB_S_OK; ++m)
+            {
+                dev[p][m].pixels = static_cast<uint8_t*>(L.buf[slot]) + off;
+                off += padded(dev[p][m]);
+                if ((m % pl.per ? pl.rest : pl.first) == Copy::Up)
+                    hr = cuda_hr(cudaMemcpyAsync(dev[p][m].pixels, host[m].pixels, host[m].slicePitch, cudaMemcpyHostToDevice, st), "H2D");
+            }
+        }
+        if (hr) break;
+        hr = fn(dev.data(), k - i, st); if (hr) break;
+        for (size_t p = 0; p < nplanes && hr == DXB_S_OK; ++p)
+        {
+            const Plane& pl = planes[p];
+            const dxb200_image* host = pl.host + i * pl.per;
+            for (size_t m = 0; m < dev[p].size() && hr == DXB_S_OK; ++m)
+                if ((m % pl.per ? pl.rest : pl.first) == Copy::Down)
+                    hr = cuda_hr(cudaMemcpyAsync(host[m].pixels, dev[p][m].pixels, host[m].slicePitch, cudaMemcpyDeviceToHost, st), "D2H");
+        }
+        i = k; slot = (slot + 1) % NSLOT;
+    }
+    for (int s = 0; s < NSLOT; ++s)
+    {
+        const int32_t h2 = cuda_hr(cudaStreamSynchronize(L.streams[s]), "final sync");
+        if (hr == DXB_S_OK) hr = h2;
+    }
+    return hr;
+}
+
+// Band calls cut host images into BANDS of whole work rows (4 pixel rows per block row on the BC side) of about BAND_BYTES.
+// Band boundaries fall on block rows, so the result is identical to processing the whole image at once.
 struct BandSplit { std::vector<dxb200_image> src, dst; std::vector<size_t> units; };      // units = progress units a band completes
 
 // srcRows/dstRows: pixel (or block) rows of the source/destination image consumed/produced per work row
 void split_bands(const dxb200_image* src, const dxb200_image* dst, size_t n, size_t srcRows, size_t dstRows, bool srcIsBC, bool dstIsBC, BandSplit& out)
 {
-    const size_t BAND = size_t(32) << 20;
     for (size_t m = 0; m < n; ++m)
     {
         const size_t srcTotalRows = srcIsBC ? (src[m].height + 3) / 4 : src[m].height;
         const size_t dstTotalRows = dstIsBC ? (dst[m].height + 3) / 4 : dst[m].height;
         const size_t units = std::max<size_t>(1, (srcTotalRows + srcRows - 1) / srcRows);
         const size_t bytesPerUnit = src[m].rowPitch * srcRows + dst[m].rowPitch * dstRows;
-        const size_t per = std::max<size_t>(1, BAND / std::max<size_t>(bytesPerUnit, 1));
+        const size_t per = std::max<size_t>(1, BAND_BYTES / std::max<size_t>(bytesPerUnit, 1));
         for (size_t u0 = 0; u0 < units; u0 += per)
         {
             const size_t u1 = std::min(units, u0 + per);
@@ -440,52 +530,26 @@ void split_bands(const dxb200_image* src, const dxb200_image* dst, size_t n, siz
     }
 }
 
+// A band call once its arguments are validated: bands (split_bands) sharded over the devices by bytes and staged BAND_CHUNK
+// bytes per chunk; launch(src, dst, count, stream) enqueues the kernel on device images.  status (optional) is called as the
+// reference calls it, and with (total, total) at the end.
 template <typename LaunchFn>
-int32_t run_staged(const dxb200_image* src, const dxb200_image* dst, size_t n, LaunchFn fn, Progress* prog = nullptr, const size_t* units = nullptr)
+int32_t run_bands(const dxb200_image* src, const dxb200_image* dst, size_t n, size_t srcRows, size_t dstRows, bool srcIsBC, bool dstIsBC,
+                  dxb200_status_fn status, void* user, LaunchFn launch)
 {
-    const size_t CHUNK = size_t(48) << 20;
-    size_t i = 0; int slot = 0;
-    int32_t hr = DXB_S_OK;
-    while (i < n && hr == DXB_S_OK)
-    {
-        size_t inBytes = 0, outBytes = 0, k = i;
-        while (k < n)
+    BandSplit bands;
+    split_bands(src, dst, n, srcRows, dstRows, srcIsBC, dstIsBC, bands);
+    Progress prog; prog.fn = status; prog.user = user;
+    for (size_t u : bands.units) prog.total += u;
+    int32_t hr = run_sharded(bands.src.size(), [&](size_t i) { return bands.src[i].slicePitch + bands.dst[i].slicePitch; },
+        [&](size_t lo, size_t hi)
         {
-            const size_t a = (src[k].slicePitch + 255) & ~size_t(255), b = (dst[k].slicePitch + 255) & ~size_t(255);
-            if (k > i && (inBytes + a + outBytes + b) > CHUNK) break;
-            inBytes += a; outBytes += b; ++k;
-        }
-        cudaStream_t st = t_v.lane->streams[slot];
-        hr = cuda_hr(cudaStreamSynchronize(st), "slot sync"); if (hr) break;
-        if (prog)
-        {
-            size_t add = 0;
-            for (size_t m = i; m < k; ++m) add += units ? units[m] : 0;
-            if (!prog->report(add)) { hr = DXB_E_ABORT; break; }
-        }
-        hr = ensure_buffer(&t_v.lane->dIn[slot], &t_v.lane->dInCap[slot], inBytes); if (hr) break;
-        hr = ensure_buffer(&t_v.lane->dOut[slot], &t_v.lane->dOutCap[slot], outBytes); if (hr) break;
-        std::vector<dxb200_image> ds(src + i, src + k), dd(dst + i, dst + k);
-        size_t offIn = 0, offOut = 0;
-        for (size_t m = i; m < k && hr == DXB_S_OK; ++m)
-        {
-            ds[m - i].pixels = static_cast<uint8_t*>(t_v.lane->dIn[slot]) + offIn;
-            dd[m - i].pixels = static_cast<uint8_t*>(t_v.lane->dOut[slot]) + offOut;
-            hr = cuda_hr(cudaMemcpyAsync(ds[m - i].pixels, src[m].pixels, src[m].slicePitch, cudaMemcpyHostToDevice, st), "H2D");
-            offIn += (src[m].slicePitch + 255) & ~size_t(255);
-            offOut += (dst[m].slicePitch + 255) & ~size_t(255);
-        }
-        if (hr) break;
-        hr = fn(ds.data(), dd.data(), k - i, st); if (hr) break;
-        for (size_t m = i; m < k && hr == DXB_S_OK; ++m)
-            hr = cuda_hr(cudaMemcpyAsync(dst[m].pixels, dd[m - i].pixels, dst[m].slicePitch, cudaMemcpyDeviceToHost, st), "D2H");
-        i = k; slot = (slot + 1) % NSLOT;
-    }
-    for (int s = 0; s < NSLOT; ++s)
-    {
-        const int32_t h2 = cuda_hr(cudaStreamSynchronize(t_v.lane->streams[s]), "final sync");
-        if (hr == DXB_S_OK) hr = h2;
-    }
+            const Plane planes[2] = { { bands.src.data() + lo, 1, Copy::Up, Copy::Up }, { bands.dst.data() + lo, 1, Copy::Down, Copy::Down } };
+            return run_staged(planes, 2, hi - lo, BAND_CHUNK,
+                [&](const std::vector<dxb200_image>* dev, size_t cnt, cudaStream_t st) { return launch(dev[0].data(), dev[1].data(), cnt, st); },
+                status ? &prog : nullptr, bands.units.data() + lo);
+        });
+    if (hr == DXB_S_OK && status && !status(prog.total, prog.total, user)) hr = DXB_E_ABORT;
     return hr;
 }
 
@@ -519,44 +583,26 @@ int32_t plan_convert(const dxb200_image* src, size_t n, uint32_t dstFormat, uint
 
 int32_t launch_convert(dxb_convert_params P, const dxb200_image* src, const dxb200_image* dst, size_t n, cudaStream_t stream)
 {
-    std::vector<dxb_job> jobs(n);
-    uint64_t total = 0;
-    for (size_t i = 0; i < n; ++i)
-    {
-        dxb_job& j = jobs[i];
-        j.src = src[i].pixels; j.dst = dst[i].pixels; j.srcPitch = src[i].rowPitch; j.dstPitch = dst[i].rowPitch;
-        j.width = (uint32_t)src[i].width; j.height = (uint32_t)src[i].height; j.nbx = j.nby = 0; j.pad = 0;
-        j.firstUnit = (uint32_t)total;
-        total += (uint64_t)j.width * j.height;
-        if (total > 0x7FFFFFFFull) return DXB_E_INVALIDARG;
-    }
-    P.totalUnits = (uint32_t)total; P.njobs = (uint32_t)n;
-    DeviceJobs<dxb_job> dj;
-    int32_t hr = dj.upload(jobs, stream);
+    JobTable jt;
+    int32_t hr = jt.build(src, dst, n, false, stream);
     if (hr != DXB_S_OK) return hr;
+    P.totalUnits = jt.total; P.njobs = (uint32_t)n;
     if (P.flags & DXB_FILTER_DITHER_DIFFUSION)
     {
         // two error rows of (width + 2) pixels per image
         uint32_t maxw = 0;
-        for (const dxb_job& j : jobs) maxw = std::max(maxw, j.width);
+        for (const dxb_job& j : jt.host) maxw = std::max(maxw, j.width);
         const uint32_t errStride = 2u * (maxw + 2u);
         void* dErr = nullptr;
         hr = cuda_hr(cudaMallocAsync(&dErr, (size_t)errStride * n * sizeof(float) * 4, stream), "cudaMallocAsync(errors)");
-        if (hr == DXB_S_OK)
-        {
-            dxb_launch_convert_diffuse(stream, (n > 1) ? dj.d : nullptr, jobs.data(), P, dErr, errStride);
-            hr = check_launch("k_convert_diffuse");
-            cudaFreeAsync(dErr, stream);
-        }
-        dj.release();
+        if (hr != DXB_S_OK) return hr;
+        dxb_launch_convert_diffuse(stream, (n > 1) ? jt.dev.d : nullptr, jt.host.data(), P, dErr, errStride);
+        hr = check_launch("k_convert_diffuse");
+        cudaFreeAsync(dErr, stream);
         return hr;
     }
-    const uint32_t need = (uint32_t)((total + 255) / 256);
-    const uint32_t grid = std::max(1u, std::min<uint32_t>(need, (uint32_t)t_v.dev->gridRow * 8u));
-    dxb_launch_convert(grid, stream, dj.d, jobs.data(), P);
-    hr = check_launch("k_convert");
-    dj.release();
-    return hr;
+    dxb_launch_convert(grid_for(jt.total, 256, (uint32_t)t_v.dev->gridRow * 8u), stream, jt.dev.d, jt.host.data(), P);
+    return check_launch("k_convert");
 }
 
 // ---- PremultiplyAlpha ---------------------------------------------------------------------------
@@ -583,27 +629,12 @@ int32_t plan_pmalpha(const dxb200_image* src, size_t n, uint32_t flags, const dx
 
 int32_t launch_pmalpha(dxb_convert_params P, const dxb200_image* src, const dxb200_image* dst, size_t n, cudaStream_t stream)
 {
-    std::vector<dxb_job> jobs(n);
-    uint64_t total = 0;
-    for (size_t i = 0; i < n; ++i)
-    {
-        dxb_job& j = jobs[i];
-        j.src = src[i].pixels; j.dst = dst[i].pixels; j.srcPitch = src[i].rowPitch; j.dstPitch = dst[i].rowPitch;
-        j.width = (uint32_t)src[i].width; j.height = (uint32_t)src[i].height; j.nbx = j.nby = 0; j.pad = 0;
-        j.firstUnit = (uint32_t)total;
-        total += (uint64_t)j.width * j.height;
-        if (total > 0x7FFFFFFFull) return DXB_E_INVALIDARG;
-    }
-    P.totalUnits = (uint32_t)total; P.njobs = (uint32_t)n;
-    DeviceJobs<dxb_job> dj;
-    int32_t hr = dj.upload(jobs, stream);
+    JobTable jt;
+    const int32_t hr = jt.build(src, dst, n, false, stream);
     if (hr != DXB_S_OK) return hr;
-    const uint32_t need = (uint32_t)((total + 255) / 256);
-    const uint32_t grid = std::max(1u, std::min<uint32_t>(need, (uint32_t)t_v.dev->gridRow * 8u));
-    dxb_launch_pmalpha(grid, stream, dj.d, jobs.data(), P);
-    hr = check_launch("k_pmalpha");
-    dj.release();
-    return hr;
+    P.totalUnits = jt.total; P.njobs = (uint32_t)n;
+    dxb_launch_pmalpha(grid_for(jt.total, 256, (uint32_t)t_v.dev->gridRow * 8u), stream, jt.dev.d, jt.host.data(), P);
+    return check_launch("k_pmalpha");
 }
 
 // ---- GenerateMipMaps ----------------------------------------------------------------------------
@@ -836,8 +867,7 @@ void dxb200_shutdown(void)
             {
                 Lane& L = d->lanes[l];
                 if (L.streams[i]) { cudaStreamSynchronize(L.streams[i]); cudaStreamDestroy(L.streams[i]); L.streams[i] = nullptr; }
-                if (L.dIn[i]) { cudaFree(L.dIn[i]); L.dIn[i] = nullptr; L.dInCap[i] = 0; }
-                if (L.dOut[i]) { cudaFree(L.dOut[i]); L.dOut[i] = nullptr; L.dOutCap[i] = 0; }
+                if (L.buf[i]) { cudaFree(L.buf[i]); L.buf[i] = nullptr; L.cap[i] = 0; }
             }
     }
     g_devs.clear();
@@ -909,20 +939,8 @@ int32_t dxb200_compress_ex(const dxb200_image* src, size_t nimages, uint32_t dst
     CompressPlan plan;
     int32_t hr = plan_compress(src, nimages, dstFormat, flags, threshold, dst, &plan);
     if (hr != DXB_S_OK) return hr;
-    BandSplit bands;
-    split_bands(src, dst, nimages, 4, 1, false, true, bands);
-    Progress prog; prog.fn = status; prog.user = user;
-    for (size_t u : bands.units) prog.total += u;
-    // bands (whole block rows) are independent: contiguous band ranges go to the initialised devices, weighted by their bytes
-    hr = run_sharded(bands.src.size(), [&](size_t i) { return bands.src[i].slicePitch + bands.dst[i].slicePitch; },
-        [&](size_t lo, size_t hi)
-        {
-            return run_staged(bands.src.data() + lo, bands.dst.data() + lo, hi - lo,
-                [&](const dxb200_image* ds, const dxb200_image* dd, size_t cnt, cudaStream_t st) { return launch_compress(plan, ds, dd, cnt, st); },
-                status ? &prog : nullptr, bands.units.data() + lo);
-        });
-    if (hr == DXB_S_OK && status && !status(prog.total, prog.total, user)) hr = DXB_E_ABORT;
-    return hr;
+    return run_bands(src, dst, nimages, 4, 1, false, true, status, user,
+        [&](const dxb200_image* ds, const dxb200_image* dd, size_t cnt, cudaStream_t st) { return launch_compress(plan, ds, dd, cnt, st); });
 }
 
 int32_t dxb200_compress(const dxb200_image* src, size_t nimages, uint32_t dstFormat, uint32_t flags, float threshold,
@@ -954,27 +972,12 @@ static int32_t plan_decompress(const dxb200_image* src, size_t n, uint32_t dstFo
 
 static int32_t launch_decompress(dxb_compress_params P, const dxb200_image* src, const dxb200_image* dst, size_t n, cudaStream_t stream)
 {
-    std::vector<dxb_job> jobs(n);
-    uint64_t total = 0;
-    for (size_t i = 0; i < n; ++i)
-    {
-        dxb_job& j = jobs[i];
-        j.src = src[i].pixels; j.dst = dst[i].pixels; j.srcPitch = src[i].rowPitch; j.dstPitch = dst[i].rowPitch;
-        j.width = (uint32_t)src[i].width; j.height = (uint32_t)src[i].height;
-        j.nbx = (j.width + 3) / 4; j.nby = (j.height + 3) / 4; j.pad = 0;
-        j.firstUnit = (uint32_t)total; total += (uint64_t)j.nbx * j.nby;
-        if (total > 0x7FFFFFFFull) return DXB_E_INVALIDARG;
-    }
-    P.totalUnits = (uint32_t)total; P.njobs = (uint32_t)n;
-    DeviceJobs<dxb_job> dj;
-    int32_t hr = dj.upload(jobs, stream);
+    JobTable jt;
+    const int32_t hr = jt.build(src, dst, n, true, stream);
     if (hr != DXB_S_OK) return hr;
-    const uint32_t need = (uint32_t)((total + 127) / 128);
-    const uint32_t grid = std::max(1u, std::min<uint32_t>(need, (uint32_t)t_v.dev->gridBC15 * 8u));
-    dxb_launch_decompress(grid, stream, dj.d, jobs[0], P);
-    hr = check_launch("k_decompress");
-    dj.release();
-    return hr;
+    P.totalUnits = jt.total; P.njobs = (uint32_t)n;
+    dxb_launch_decompress(grid_for(jt.total, 128, (uint32_t)t_v.dev->gridBC15 * 8u), stream, jt.dev.d, jt.host.data(), P);
+    return check_launch("k_decompress");
 }
 
 int32_t dxb200_decompress_device(const dxb200_image* src, size_t nimages, uint32_t dstFormat, const dxb200_image* dst, void* stream)
@@ -993,14 +996,8 @@ int32_t dxb200_decompress(const dxb200_image* src, size_t nimages, uint32_t dstF
     dxb_compress_params P;
     int32_t hr = plan_decompress(src, nimages, dstFormat, dst, &P);
     if (hr != DXB_S_OK) return hr;
-    BandSplit bands;
-    split_bands(src, dst, nimages, 1, 4, true, false, bands);
-    return run_sharded(bands.src.size(), [&](size_t i) { return bands.src[i].slicePitch + bands.dst[i].slicePitch; },
-        [&](size_t lo, size_t hi)
-        {
-            return run_staged(bands.src.data() + lo, bands.dst.data() + lo, hi - lo,
-                [&](const dxb200_image* ds, const dxb200_image* dd, size_t cnt, cudaStream_t st) { return launch_decompress(P, ds, dd, cnt, st); });
-        });
+    return run_bands(src, dst, nimages, 1, 4, true, false, nullptr, nullptr,
+        [&](const dxb200_image* ds, const dxb200_image* dd, size_t cnt, cudaStream_t st) { return launch_decompress(P, ds, dd, cnt, st); });
 }
 
 // ---- Convert ------------------------------------------------------------------------------------
@@ -1024,23 +1021,12 @@ int32_t dxb200_convert_ex(const dxb200_image* src, size_t nimages, uint32_t dstF
     int32_t hr = plan_convert(src, nimages, dstFormat, filter, dst, &P);
     if (hr != DXB_S_OK) return hr;
     P.threshold = threshold;
-    BandSplit bands;
     // bands start on multiples of 4 rows so that the 4x4 ordered-dither matrix keeps its phase
     // (error diffusion carries state from row to row: whole images only)
     size_t rowsPerUnit = (P.flags & DXB_FILTER_DITHER) ? 4 : 1;
     if (P.flags & DXB_FILTER_DITHER_DIFFUSION) for (size_t i = 0; i < nimages; ++i) rowsPerUnit = std::max(rowsPerUnit, src[i].height);
-    split_bands(src, dst, nimages, rowsPerUnit, rowsPerUnit, false, false, bands);
-    Progress prog; prog.fn = status; prog.user = user;
-    for (size_t u : bands.units) prog.total += u;
-    hr = run_sharded(bands.src.size(), [&](size_t i) { return bands.src[i].slicePitch + bands.dst[i].slicePitch; },
-        [&](size_t lo, size_t hi)
-        {
-            return run_staged(bands.src.data() + lo, bands.dst.data() + lo, hi - lo,
-                [&](const dxb200_image* ds, const dxb200_image* dd, size_t cnt, cudaStream_t st) { return launch_convert(P, ds, dd, cnt, st); },
-                status ? &prog : nullptr, bands.units.data() + lo);
-        });
-    if (hr == DXB_S_OK && status && !status(prog.total, prog.total, user)) hr = DXB_E_ABORT;
-    return hr;
+    return run_bands(src, dst, nimages, rowsPerUnit, rowsPerUnit, false, false, status, user,
+        [&](const dxb200_image* ds, const dxb200_image* dd, size_t cnt, cudaStream_t st) { return launch_convert(P, ds, dd, cnt, st); });
 }
 
 int32_t dxb200_convert(const dxb200_image* src, size_t nimages, uint32_t dstFormat, uint32_t filter, float threshold, const dxb200_image* dst)
@@ -1060,45 +1046,6 @@ int32_t dxb200_generate_mipmaps_device(const dxb200_image* chain, size_t items, 
     return launch_mips(chain, items, levels, filter, mode, static_cast<cudaStream_t>(stream));
 }
 
-// host chains of items [lo, hi): level 0 up, kernels, levels 1.. down; whole items per chunk, on the calling thread's lane
-static int32_t mips_host_range(const dxb200_image* chain, size_t lo, size_t hi, size_t levels, uint32_t filter, uint32_t mode)
-{
-    const size_t CHUNK = size_t(1) << 30;
-    int32_t hr = DXB_S_OK;
-    size_t it = lo;
-    cudaStream_t st = t_v.lane->streams[0];
-    while (it < hi && hr == DXB_S_OK)
-    {
-        size_t bytes = 0, k = it;
-        while (k < hi)
-        {
-            size_t b = 0;
-            for (size_t l = 0; l < levels; ++l) b += (chain[k * levels + l].slicePitch + 255) & ~size_t(255);
-            if (k > it && bytes + b > CHUNK) break;
-            bytes += b; ++k;
-        }
-        hr = ensure_buffer(&t_v.lane->dIn[0], &t_v.lane->dInCap[0], bytes); if (hr) break;
-        std::vector<dxb200_image> dev(chain + it * levels, chain + k * levels);
-        size_t off = 0;
-        for (size_t m = 0; m < dev.size() && hr == DXB_S_OK; ++m)
-        {
-            dev[m].pixels = static_cast<uint8_t*>(t_v.lane->dIn[0]) + off;
-            off += (dev[m].slicePitch + 255) & ~size_t(255);
-            if ((m % levels) == 0)
-                hr = cuda_hr(cudaMemcpyAsync(dev[m].pixels, chain[it * levels + m].pixels, dev[m].slicePitch, cudaMemcpyHostToDevice, st), "H2D");
-        }
-        if (hr) break;
-        hr = launch_mips(dev.data(), k - it, levels, filter, mode, st); if (hr) break;
-        for (size_t m = 0; m < dev.size() && hr == DXB_S_OK; ++m)
-            if ((m % levels) != 0)
-                hr = cuda_hr(cudaMemcpyAsync(chain[it * levels + m].pixels, dev[m].pixels, dev[m].slicePitch, cudaMemcpyDeviceToHost, st), "D2H");
-        if (hr) break;
-        hr = cuda_hr(cudaStreamSynchronize(st), "mips sync");
-        it = k;
-    }
-    return hr;
-}
-
 int32_t dxb200_generate_mipmaps(const dxb200_image* chain, size_t items, size_t levels, uint32_t filter)
 {
     uint32_t mode = 0;
@@ -1106,7 +1053,12 @@ int32_t dxb200_generate_mipmaps(const dxb200_image* chain, size_t items, size_t 
     if (hr != DXB_S_OK) return hr;
     // image-per-GPU sharding: contiguous item ranges per device; a single item's chain stays on one device (SURVEY 8(e))
     return run_sharded(items, [&](size_t i) { return chain[i * levels].slicePitch; },
-        [&](size_t lo, size_t hi) { return mips_host_range(chain, lo, hi, levels, filter, mode); });
+        [&](size_t lo, size_t hi)
+        {
+            const Plane chains = { chain + lo * levels, levels, Copy::Up, Copy::Down };
+            return run_staged(&chains, 1, hi - lo, ITEM_CHUNK,
+                [&](const std::vector<dxb200_image>* dev, size_t cnt, cudaStream_t st) { return launch_mips(dev[0].data(), cnt, levels, filter, mode, st); });
+        });
 }
 
 // ---- GenerateMipMaps + Compress in one call: the mip chain never leaves HBM --------------------------------------------
@@ -1133,7 +1085,7 @@ int32_t dxb200_mipmaps_compress(const dxb200_image* base, size_t items, size_t l
             c.width = w; c.height = h; c.format = base[i].format;
             const int32_t hp = compute_pitch(c.format, w, h, &c.rowPitch, &c.slicePitch);
             if (hp != DXB_S_OK) return hp;
-            c.pixels = const_cast<uint8_t*>(base[i].pixels);          // placeholder for validation; replaced by device addresses per chunk
+            c.pixels = const_cast<uint8_t*>(base[i].pixels);          // level 0's upload source; the other levels only need it for validation
             if (h > 1) h >>= 1;
             if (w > 1) w >>= 1;
         }
@@ -1145,53 +1097,17 @@ int32_t dxb200_mipmaps_compress(const dxb200_image* base, size_t items, size_t l
     CompressPlan plan;
     hr = plan_compress(chain.data(), items * levels, dstFormat, flags, threshold, dst, &plan);
     if (hr != DXB_S_OK) return hr;
-    auto range = [&](size_t lo, size_t hi) -> int32_t
-    {
-        const size_t CHUNK = size_t(64) << 20;
-        int32_t h2 = DXB_S_OK;
-        size_t it = lo; int slot = 0;
-        while (it < hi && h2 == DXB_S_OK)
+    return run_sharded(items, [&](size_t i) { return base[i].slicePitch; },
+        [&](size_t lo, size_t hi)
         {
-            size_t inBytes = 0, outBytes = 0, k = it;
-            while (k < hi)
-            {
-                size_t a = 0, b = 0;
-                for (size_t l = 0; l < levels; ++l)
+            const Plane planes[2] = { { chain.data() + lo * levels, levels, Copy::Up, Copy::None }, { dst + lo * levels, levels, Copy::Down, Copy::Down } };
+            return run_staged(planes, 2, hi - lo, ITEM_CHUNK,
+                [&](const std::vector<dxb200_image>* dev, size_t cnt, cudaStream_t st)
                 {
-                    a += (chain[k * levels + l].slicePitch + 255) & ~size_t(255);
-                    b += (dst[k * levels + l].slicePitch + 255) & ~size_t(255);
-                }
-                if (k > it && inBytes + a > CHUNK) break;
-                inBytes += a; outBytes += b; ++k;
-            }
-            cudaStream_t st = t_v.lane->streams[slot];
-            h2 = cuda_hr(cudaStreamSynchronize(st), "slot sync"); if (h2) break;
-            h2 = ensure_buffer(&t_v.lane->dIn[slot], &t_v.lane->dInCap[slot], inBytes); if (h2) break;
-            h2 = ensure_buffer(&t_v.lane->dOut[slot], &t_v.lane->dOutCap[slot], outBytes); if (h2) break;
-            std::vector<dxb200_image> dc(chain.begin() + it * levels, chain.begin() + k * levels), dd(dst + it * levels, dst + k * levels);
-            size_t offIn = 0, offOut = 0;
-            for (size_t m = 0; m < dc.size() && h2 == DXB_S_OK; ++m)
-            {
-                dc[m].pixels = static_cast<uint8_t*>(t_v.lane->dIn[slot]) + offIn;  offIn += (dc[m].slicePitch + 255) & ~size_t(255);
-                dd[m].pixels = static_cast<uint8_t*>(t_v.lane->dOut[slot]) + offOut; offOut += (dd[m].slicePitch + 255) & ~size_t(255);
-                if ((m % levels) == 0)
-                    h2 = cuda_hr(cudaMemcpyAsync(dc[m].pixels, base[it + m / levels].pixels, dc[m].slicePitch, cudaMemcpyHostToDevice, st), "H2D");
-            }
-            if (h2) break;
-            h2 = launch_mips(dc.data(), k - it, levels, filter, mode, st); if (h2) break;
-            h2 = launch_compress(plan, dc.data(), dd.data(), dc.size(), st); if (h2) break;
-            for (size_t m = 0; m < dd.size() && h2 == DXB_S_OK; ++m)
-                h2 = cuda_hr(cudaMemcpyAsync(dst[it * levels + m].pixels, dd[m].pixels, dd[m].slicePitch, cudaMemcpyDeviceToHost, st), "D2H");
-            it = k; slot = (slot + 1) % NSLOT;
-        }
-        for (int sl = 0; sl < NSLOT; ++sl)
-        {
-            const int32_t h3 = cuda_hr(cudaStreamSynchronize(t_v.lane->streams[sl]), "final sync");
-            if (h2 == DXB_S_OK) h2 = h3;
-        }
-        return h2;
-    };
-    return run_sharded(items, [&](size_t i) { return base[i].slicePitch; }, range);
+                    const int32_t h2 = launch_mips(dev[0].data(), cnt, levels, filter, mode, st);
+                    return h2 != DXB_S_OK ? h2 : launch_compress(plan, dev[0].data(), dev[1].data(), cnt * levels, st);
+                });
+        });
 }
 
 int32_t dxb200_premultiply_alpha_device(const dxb200_image* src, size_t nimages, uint32_t flags, const dxb200_image* dst, void* stream)
@@ -1210,14 +1126,8 @@ int32_t dxb200_premultiply_alpha(const dxb200_image* src, size_t nimages, uint32
     dxb_convert_params P;
     int32_t hr = plan_pmalpha(src, nimages, flags, dst, &P);
     if (hr != DXB_S_OK) return hr;
-    BandSplit bands;
-    split_bands(src, dst, nimages, 1, 1, false, false, bands);
-    return run_sharded(bands.src.size(), [&](size_t i) { return bands.src[i].slicePitch + bands.dst[i].slicePitch; },
-        [&](size_t lo, size_t hi)
-        {
-            return run_staged(bands.src.data() + lo, bands.dst.data() + lo, hi - lo,
-                [&](const dxb200_image* ds, const dxb200_image* dd, size_t cnt, cudaStream_t st) { return launch_pmalpha(P, ds, dd, cnt, st); });
-        });
+    return run_bands(src, dst, nimages, 1, 1, false, false, nullptr, nullptr,
+        [&](const dxb200_image* ds, const dxb200_image* dd, size_t cnt, cudaStream_t st) { return launch_pmalpha(P, ds, dd, cnt, st); });
 }
 
 // ---- ScaleMipMapsAlphaForCoverage ----------------------------------------------------------------
@@ -1318,14 +1228,14 @@ int32_t dxb200_scale_mipmaps_alpha_for_coverage(const dxb200_image* src, size_t 
     cudaStream_t st = t_v.lane->streams[0];
     size_t bytes = 0;
     for (size_t l = 0; l < nlevels; ++l) bytes += 2 * ((src[l].slicePitch + 255) & ~size_t(255));
-    hr = ensure_buffer(&t_v.lane->dIn[0], &t_v.lane->dInCap[0], bytes);
+    hr = ensure_buffer(&t_v.lane->buf[0], &t_v.lane->cap[0], bytes);
     if (hr != DXB_S_OK) return hr;
     std::vector<dxb200_image> ds(src, src + nlevels), dd(dst, dst + nlevels);
     size_t off = 0;
     for (size_t l = 0; l < nlevels && hr == DXB_S_OK; ++l)
     {
-        ds[l].pixels = static_cast<uint8_t*>(t_v.lane->dIn[0]) + off; off += (src[l].slicePitch + 255) & ~size_t(255);
-        dd[l].pixels = static_cast<uint8_t*>(t_v.lane->dIn[0]) + off; off += (src[l].slicePitch + 255) & ~size_t(255);
+        ds[l].pixels = static_cast<uint8_t*>(t_v.lane->buf[0]) + off; off += (src[l].slicePitch + 255) & ~size_t(255);
+        dd[l].pixels = static_cast<uint8_t*>(t_v.lane->buf[0]) + off; off += (src[l].slicePitch + 255) & ~size_t(255);
         dd[l].rowPitch = src[l].rowPitch; dd[l].slicePitch = src[l].slicePitch;          // device copy uses the source layout
         hr = cuda_hr(cudaMemcpyAsync(ds[l].pixels, src[l].pixels, src[l].slicePitch, cudaMemcpyHostToDevice, st), "H2D");
     }
@@ -1337,6 +1247,14 @@ int32_t dxb200_scale_mipmaps_alpha_for_coverage(const dxb200_image* src, size_t 
     return hr;
 }
 
+// a resize is a two-"level" chain per item whose second level has an arbitrary size
+static int32_t launch_resize(const dxb200_image* src, const dxb200_image* dst, size_t n, uint32_t filter, uint32_t mode, cudaStream_t stream)
+{
+    std::vector<dxb200_image> pairs(2 * n);
+    for (size_t i = 0; i < n; ++i) { pairs[2 * i] = src[i]; pairs[2 * i + 1] = dst[i]; }
+    return launch_mips(pairs.data(), n, 2, filter, mode, stream);
+}
+
 int32_t dxb200_resize_device(const dxb200_image* src, size_t nimages, uint32_t filter, const dxb200_image* dst, void* stream)
 {
     uint32_t mode = 0;
@@ -1345,47 +1263,7 @@ int32_t dxb200_resize_device(const dxb200_image* src, size_t nimages, uint32_t f
     DevScope scope;
     hr = scope.enter(src[0].pixels);
     if (hr != DXB_S_OK) return hr;
-    // a resize is a two-"level" chain per item whose second level has an arbitrary size
-    std::vector<dxb200_image> pairs(2 * nimages);
-    for (size_t i = 0; i < nimages; ++i) { pairs[2 * i] = src[i]; pairs[2 * i + 1] = dst[i]; }
-    return launch_mips(pairs.data(), nimages, 2, filter, mode, static_cast<cudaStream_t>(stream));
-}
-
-static int32_t resize_host_range(const dxb200_image* src, const dxb200_image* dst, size_t lo, size_t hi, uint32_t filter, uint32_t mode)
-{
-    const size_t CHUNK = size_t(1) << 30;
-    cudaStream_t st = t_v.lane->streams[0];
-    int32_t hr = DXB_S_OK;
-    size_t it = lo;
-    while (it < hi && hr == DXB_S_OK)
-    {
-        size_t bytes = 0, k = it;
-        while (k < hi)
-        {
-            const size_t b = ((src[k].slicePitch + 255) & ~size_t(255)) + ((dst[k].slicePitch + 255) & ~size_t(255));
-            if (k > it && bytes + b > CHUNK) break;
-            bytes += b; ++k;
-        }
-        hr = ensure_buffer(&t_v.lane->dIn[0], &t_v.lane->dInCap[0], bytes); if (hr) break;
-        std::vector<dxb200_image> pairs(2 * (k - it));
-        size_t off = 0;
-        for (size_t i = it; i < k && hr == DXB_S_OK; ++i)
-        {
-            dxb200_image& s = pairs[2 * (i - it)]; dxb200_image& d = pairs[2 * (i - it) + 1];
-            s = src[i]; d = dst[i];
-            s.pixels = static_cast<uint8_t*>(t_v.lane->dIn[0]) + off; off += (s.slicePitch + 255) & ~size_t(255);
-            d.pixels = static_cast<uint8_t*>(t_v.lane->dIn[0]) + off; off += (d.slicePitch + 255) & ~size_t(255);
-            hr = cuda_hr(cudaMemcpyAsync(s.pixels, src[i].pixels, s.slicePitch, cudaMemcpyHostToDevice, st), "H2D");
-        }
-        if (hr) break;
-        hr = launch_mips(pairs.data(), k - it, 2, filter, mode, st); if (hr) break;
-        for (size_t i = it; i < k && hr == DXB_S_OK; ++i)
-            hr = cuda_hr(cudaMemcpyAsync(dst[i].pixels, pairs[2 * (i - it) + 1].pixels, dst[i].slicePitch, cudaMemcpyDeviceToHost, st), "D2H");
-        if (hr) break;
-        hr = cuda_hr(cudaStreamSynchronize(st), "resize sync");
-        it = k;
-    }
-    return hr;
+    return launch_resize(src, dst, nimages, filter, mode, static_cast<cudaStream_t>(stream));
 }
 
 int32_t dxb200_resize(const dxb200_image* src, size_t nimages, uint32_t filter, const dxb200_image* dst)
@@ -1394,7 +1272,12 @@ int32_t dxb200_resize(const dxb200_image* src, size_t nimages, uint32_t filter, 
     int32_t hr = plan_resize(src, nimages, filter, dst, &mode);
     if (hr != DXB_S_OK) return hr;
     return run_sharded(nimages, [&](size_t i) { return src[i].slicePitch + dst[i].slicePitch; },
-        [&](size_t lo, size_t hi) { return resize_host_range(src, dst, lo, hi, filter, mode); });
+        [&](size_t lo, size_t hi)
+        {
+            const Plane planes[2] = { { src + lo, 1, Copy::Up, Copy::Up }, { dst + lo, 1, Copy::Down, Copy::Down } };
+            return run_staged(planes, 2, hi - lo, ITEM_CHUNK,
+                [&](const std::vector<dxb200_image>* dev, size_t cnt, cudaStream_t st) { return launch_resize(dev[0].data(), dev[1].data(), cnt, filter, mode, st); });
+        });
 }
 
 } // extern "C"

@@ -34,7 +34,7 @@ __device__ __forceinline__ void bc15_body(const dxb_job* __restrict__ jobs, cons
         if (SYNC) __syncthreads();
         const uint32_t unit = base + threadIdx.x;
         if (unit >= P.totalUnits) continue;
-        const dxb_job& j = dxb_find_job(jobs, P.njobs, single, unit, P.periodUnits, P.periodJobs);
+        const dxb_job& j = dxb_find_job(jobs, P.njobs, single, unit);
         const uint32_t local = unit - j.firstUnit;
         const uint32_t by = local / j.nbx, bx = local - by * j.nbx;
         dxb_image_desc img; img.pixels = j.src; img.rowPitch = j.srcPitch; img.width = j.width; img.height = j.height; img.format = srcFormat;
@@ -70,7 +70,7 @@ __global__ void __launch_bounds__(dxb_bc15_threads(DF), dxb_bc15_minb(DF)) k_com
     X(80, 61) X(80, 28) X(80, 41) X(80, 2) X(81, 61) X(81, 28) X(81, 41) X(81, 2) \
     X(83, 49) X(83, 28) X(83, 16) X(83, 2) X(84, 49) X(84, 28) X(84, 16) X(84, 2)
 
-void dxb_launch_bc15(unsigned grid, cudaStream_t stream, const dxb_job* jobs, const dxb_job& single, const dxb_compress_params& P)
+void dxb_launch_bc15(unsigned grid, cudaStream_t stream, const dxb_job* jobs, const dxb_job* hostJobs, const dxb_compress_params& P)
 {
     // the _SRGB variants share loader, conversion class and encoder with their UNORM twins; whether an sRGB <-> linear
     // step is needed is already resolved into P.cflags, and the specialised kernels only take the default flag set
@@ -82,11 +82,11 @@ void dxb_launch_bc15(unsigned grid, cudaStream_t stream, const dxb_job* jobs, co
     if (sf == DXB_FMT_B8G8R8A8_UNORM_SRGB) sf = DXB_FMT_B8G8R8A8_UNORM;
     if (P.bcflags == 0 && P.cflags == dxb_bc15_default_cflags(df))
     {
-#define DXB_X(DF, SF) if (df == DF && sf == SF) { k_compress_bc15_t<DF, SF><<<std::max(1u, grid * 128u / dxb_bc15_threads(DF)), dxb_bc15_threads(DF), 0, stream>>>(jobs, single, P); return; }
+#define DXB_X(DF, SF) if (df == DF && sf == SF) { k_compress_bc15_t<DF, SF><<<std::max(1u, grid * 128u / dxb_bc15_threads(DF)), dxb_bc15_threads(DF), 0, stream>>>(jobs, hostJobs[0], P); return; }
         DXB_BC15_PAIRS(DXB_X)
 #undef DXB_X
     }
-    k_compress_bc15<<<grid, 128, 0, stream>>>(jobs, single, P);
+    k_compress_bc15<<<grid, 128, 0, stream>>>(jobs, hostJobs[0], P);
 }
 int dxb_occupancy_bc15()
 {

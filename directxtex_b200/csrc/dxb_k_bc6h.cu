@@ -17,7 +17,7 @@ __global__ void __launch_bounds__(DXB_BC6H_WARPS * 32, DXB_BC6H_MINB) k_compress
         dxb_px ip = dxb_make_px(0.0f, 0.0f, 0.0f, 0.0f);
         if (unit < P.totalUnits)
         {
-            const dxb_job& j = dxb_find_job(jobs, P.njobs, single, unit, P.periodUnits, P.periodJobs);
+            const dxb_job& j = dxb_find_job(jobs, P.njobs, single, unit);
             const uint32_t local = unit - j.firstUnit;
             const uint32_t by = local / j.nbx, bx = local - by * j.nbx;
             // partial-block replication with source map {0,0,0,1} (DirectXTexCompress.cpp:159-187)
@@ -39,9 +39,9 @@ __global__ void __launch_bounds__(DXB_BC6H_WARPS * 32, DXB_BC6H_MINB) k_compress
     }
 }
 
-void dxb_launch_bc6h(unsigned grid, cudaStream_t stream, const dxb_job* jobs, const dxb_job& single, const dxb_compress_params& P)
+void dxb_launch_bc6h(unsigned grid, cudaStream_t stream, const dxb_job* jobs, const dxb_job* hostJobs, const dxb_compress_params& P)
 {
-    k_compress_bc6h<<<grid, DXB_BC6H_WARPS * 32, 0, stream>>>(jobs, single, P);
+    k_compress_bc6h<<<grid, DXB_BC6H_WARPS * 32, 0, stream>>>(jobs, hostJobs[0], P);
 }
 int dxb_occupancy_bc6h()
 {

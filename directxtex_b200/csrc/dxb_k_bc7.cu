@@ -25,7 +25,7 @@ __global__ void __launch_bounds__(DXB_BC7_WARPS * 32, DXB_BC7_MINB) k_compress_b
         dxb_px ldr = dxb_make_px(0.0f, 0.0f, 0.0f, 255.0f);
         if (unit < P.totalUnits)
         {
-            const dxb_job& j = dxb_find_job(jobs, P.njobs, single, unit, P.periodUnits, P.periodJobs);
+            const dxb_job& j = dxb_find_job(jobs, P.njobs, single, unit);
             const uint32_t local = unit - j.firstUnit;
             const uint32_t by = local / j.nbx, bx = local - by * j.nbx;
             // CompressBC's partial-block replication with source map {0,0,0,1} (DirectXTexCompress.cpp:159-187)
@@ -56,12 +56,12 @@ static bool bc7_attr_set()
     return ok;
 }
 
-void dxb_launch_bc7(unsigned grid, cudaStream_t stream, const dxb_job* jobs, const dxb_job& single, const dxb_compress_params& P)
+void dxb_launch_bc7(unsigned grid, cudaStream_t stream, const dxb_job* jobs, const dxb_job* hostJobs, const dxb_compress_params& P)
 {
     bc7_attr_set();
     // the three-subset pass (a non-default flag) lives in its own instantiation
-    if (P.bcflags & DXB_BC_FLAGS_USE_3SUBSETS) k_compress_bc7<true><<<grid, DXB_BC7_WARPS * 32, kBC7Smem, stream>>>(jobs, single, P);
-    else k_compress_bc7<false><<<grid, DXB_BC7_WARPS * 32, kBC7Smem, stream>>>(jobs, single, P);
+    if (P.bcflags & DXB_BC_FLAGS_USE_3SUBSETS) k_compress_bc7<true><<<grid, DXB_BC7_WARPS * 32, kBC7Smem, stream>>>(jobs, hostJobs[0], P);
+    else k_compress_bc7<false><<<grid, DXB_BC7_WARPS * 32, kBC7Smem, stream>>>(jobs, hostJobs[0], P);
 }
 int dxb_occupancy_bc7()
 {

@@ -192,7 +192,7 @@ __global__ void __launch_bounds__(128) k_decompress_t(const dxb_job* __restrict_
 // default targets (DirectXTexCompress.cpp:552-579): BC1/2/3/7 -> RGBA8, BC4 -> R8, BC5 -> R8G8, BC6H -> RGBA32F
 #define DXB_DEC_PAIRS(X) X(71, 28) X(74, 28) X(77, 28) X(98, 28) X(80, 61) X(81, 63) X(83, 49) X(84, 51) X(95, 2) X(96, 2)
 
-void dxb_launch_decompress(unsigned grid, cudaStream_t stream, const dxb_job* jobs, const dxb_job& single, const dxb_compress_params& P)
+void dxb_launch_decompress(unsigned grid, cudaStream_t stream, const dxb_job* jobs, const dxb_job* hostJobs, const dxb_compress_params& P)
 {
     uint32_t sf = P.srcFormat, df = P.dstFormat;
     if (sf == DXB_FMT_BC1_UNORM_SRGB) sf = DXB_FMT_BC1_UNORM;
@@ -203,10 +203,10 @@ void dxb_launch_decompress(unsigned grid, cudaStream_t stream, const dxb_job* jo
 #ifndef DXB_DEC_GENERIC_ONLY
     if (P.cflags == 0)
     {
-#define DXB_X(SF, DF) if (sf == SF && df == DF) { k_decompress_t<SF, DF><<<grid, 128, 0, stream>>>(jobs, single, P); return; }
+#define DXB_X(SF, DF) if (sf == SF && df == DF) { k_decompress_t<SF, DF><<<grid, 128, 0, stream>>>(jobs, hostJobs[0], P); return; }
         DXB_DEC_PAIRS(DXB_X)
 #undef DXB_X
     }
 #endif
-    k_decompress<<<grid, 128, 0, stream>>>(jobs, single, P);
+    k_decompress<<<grid, 128, 0, stream>>>(jobs, hostJobs[0], P);
 }

@@ -22,9 +22,6 @@ struct dxb_compress_params
     uint32_t inF, outF, cflags, bcflags;
     float threshold;
     uint32_t totalUnits, njobs;
-    // batches of equal mip chains (items x levels jobs, item-major): every item has periodJobs jobs covering periodUnits units, so a
-    // unit's job is found from one division and a short forward scan instead of a 14-step binary search of dependent loads
-    uint32_t periodUnits, periodJobs;     // 0 = no such structure
 };
 
 struct dxb_convert_params
@@ -54,16 +51,16 @@ struct dxb_mip_params
 #define DXB_BC6H_MINB 2
 #endif
 
-// launchers: `grid` CTAs on `stream`; jobs == nullptr -> `single` is used
-void dxb_launch_bc15(unsigned grid, cudaStream_t stream, const dxb_job* jobs, const dxb_job& single, const dxb_compress_params& P);
-void dxb_launch_bc7(unsigned grid, cudaStream_t stream, const dxb_job* jobs, const dxb_job& single, const dxb_compress_params& P);
+// launchers: `grid` CTAs on `stream`; hostJobs = the njobs job records on the host, jobs = their device copy, or nullptr when
+// njobs == 1 (the kernel then takes hostJobs[0] by value)
+void dxb_launch_bc15(unsigned grid, cudaStream_t stream, const dxb_job* jobs, const dxb_job* hostJobs, const dxb_compress_params& P);
+void dxb_launch_bc7(unsigned grid, cudaStream_t stream, const dxb_job* jobs, const dxb_job* hostJobs, const dxb_compress_params& P);
 // TMA-fed persistent variant (RGBA32F sources of full 4x4 blocks, equal images at a constant stride); false = not eligible, nothing launched
 bool dxb_launch_bc7_tma(unsigned residentCtas, cudaStream_t stream, const dxb_job* hostJobs, const dxb_compress_params& P);
 int dxb_bc7_get_feed();            // 0 direct kernel, 1-3 TMA-fed variants (dxb_k_bc7.cu)
 void dxb_bc7_set_feed(int mode);
-void dxb_launch_decompress(unsigned grid, cudaStream_t stream, const dxb_job* jobs, const dxb_job& single, const dxb_compress_params& P);
-void dxb_launch_bc6h(unsigned grid, cudaStream_t stream, const dxb_job* jobs, const dxb_job& single, const dxb_compress_params& P);
-// hostJobs = the same records on the host (njobs of them); jobs = device copy or nullptr when njobs == 1
+void dxb_launch_decompress(unsigned grid, cudaStream_t stream, const dxb_job* jobs, const dxb_job* hostJobs, const dxb_compress_params& P);
+void dxb_launch_bc6h(unsigned grid, cudaStream_t stream, const dxb_job* jobs, const dxb_job* hostJobs, const dxb_compress_params& P);
 void dxb_launch_convert(unsigned grid, cudaStream_t stream, const dxb_job* jobs, const dxb_job* hostJobs, const dxb_convert_params& P);
 void dxb_launch_mip(unsigned grid, cudaStream_t stream, const dxb_mip_job* jobs, const dxb_mip_job* hostJobs, const dxb_mip_params& P);
 // tail of a chain: levels [first, first+count) of all items in one launch (jobsDev laid out [level][item]); false = no such kernel
@@ -80,17 +77,9 @@ int dxb_occupancy_bc6h();
 
 #ifdef __CUDACC__
 template <typename J>
-__device__ __forceinline__ const J& dxb_find_job(const J* jobs, uint32_t njobs, const J& single, uint32_t unit, uint32_t periodUnits = 0, uint32_t periodJobs = 0)
+__device__ __forceinline__ const J& dxb_find_job(const J* jobs, uint32_t njobs, const J& single, uint32_t unit)
 {
     if (jobs == nullptr) return single;
-    if (periodUnits != 0u)
-    {
-        const uint32_t item = unit / periodUnits;
-        uint32_t k = item * periodJobs;
-        const uint32_t end = k + periodJobs - 1u;
-        while (k < end && jobs[k + 1u].firstUnit <= unit) ++k;
-        return jobs[k];
-    }
     uint32_t lo = 0, hi = njobs;            // last job with firstUnit <= unit
     while (hi - lo > 1)
     {

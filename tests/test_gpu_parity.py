@@ -162,6 +162,26 @@ def test_mips_vs_oracle(oracle, fl):
         assert hr == 0 and np.array_equal(got, want), (fmt, w, h, hex(fl))
 
 
+@pytest.mark.parametrize("fl", [F.TEX_FILTER_BOX, F.TEX_FILTER_CUBIC])
+def test_mips_array_over_several_chunks(oracle, fl):
+    """four 2048^2 RGBA8 chains in one call (about 85 MiB) are staged in more than one 80 MiB chunk; every chain equals the reference"""
+    rng = np.random.default_rng(53)
+    srcs = [oracle_lib.random_image(28, 2048, 2048, rng) for _ in range(4)]
+    for i, (src, got) in enumerate(zip(srcs, capi.generate_mipmaps_images(srcs, 2048, 2048, 28, fl))):
+        hr, want = oracle.generate_mipmaps(src, 2048, 2048, 28, fl)
+        assert hr == 0 and np.array_equal(got, want), (i, hex(fl))
+
+
+@pytest.mark.parametrize("fl", [0, F.TEX_FILTER_CUBIC])
+def test_resize_array_over_several_chunks(oracle, fl):
+    """five 2048^2 -> 1024^2 RGBA8 pairs in one call (100 MiB) are staged in more than one 80 MiB chunk; every result equals the reference"""
+    rng = np.random.default_rng(59)
+    srcs = [oracle_lib.random_image(28, 2048, 2048, rng) for _ in range(5)]
+    for i, (src, got) in enumerate(zip(srcs, capi.resize_images(srcs, 2048, 2048, 28, 1024, 1024, fl))):
+        hr, want = oracle.resize(src, 2048, 2048, 28, 1024, 1024, fl)
+        assert hr == 0 and np.array_equal(got, want), (i, hex(fl))
+
+
 @pytest.mark.parametrize("fl", [0, F.TEX_FILTER_POINT, F.TEX_FILTER_BOX, F.TEX_FILTER_LINEAR, F.TEX_FILTER_CUBIC, F.TEX_FILTER_TRIANGLE,
                                 F.TEX_FILTER_LINEAR | F.TEX_FILTER_WRAP, F.TEX_FILTER_CUBIC | F.TEX_FILTER_MIRROR])
 def test_resize_vs_oracle(oracle, fl):
@@ -471,7 +491,7 @@ def test_mipmaps_compress_equals_two_calls_and_reference(oracle):
     """dxb200_mipmaps_compress (the chain stays in HBM) == dxb200_generate_mipmaps + dxb200_compress == the reference, bit for bit
     (BASELINE configs[3] shape: RGBA8 -> default-filter chain -> BC3), including a non-power-of-two size (LINEAR default)."""
     rng = np.random.default_rng(41)
-    for (w, h, n) in [(256, 256, 5), (96, 40, 3)]:
+    for (w, h, n) in [(256, 256, 5), (96, 40, 3), (2048, 2048, 4)]:
         srcs = [oracle_lib.random_image(28, w, h, rng) for _ in range(n)]
         outs = capi.mipmaps_compress(srcs, w, h, 28, 77)
         for src, got in zip(srcs, outs):
