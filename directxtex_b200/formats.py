@@ -25,6 +25,7 @@ TEX_COMPRESS_BC7_USE_3SUBSETS = 0x80000
 TEX_COMPRESS_BC7_QUICK = 0x100000
 TEX_COMPRESS_SRGB_IN = 0x1000000
 TEX_COMPRESS_SRGB_OUT = 0x2000000
+TEX_COMPRESS_SRGB = 0x3000000
 TEX_COMPRESS_PARALLEL = 0x10000000
 TEX_THRESHOLD_DEFAULT = 0.5
 

@@ -264,3 +264,198 @@ def convert_refused(dst_fmt, flags):
 
 def involves_srgb(sf, df, flags):
     return sf in SRGB_FORMATS or df in SRGB_FORMATS or bool(flags & F.TEX_FILTER_SRGB)
+
+
+# ---- sRGB inputs on which glibc's and CUDA's powf agree -------------------------------------------------------------------
+SNORM_FORMATS = (13, 31, 37, 51, 58, 63, 81, 84)
+SRGB_BLOCK_FORMATS = (72, 75, 78, 99)
+
+
+def resolve_srgb(flags, in_fmt, out_fmt):
+    """the sRGB bits ConvertScanline runs with (DirectXTexConvert.cpp:3121-3167), restated here independently of
+    dxb_resolve_srgb_convert: an sRGB format adds its side's bit, A8 drops it, and IN together with OUT cancel"""
+    f = flags & F.TEX_FILTER_SRGB
+    srgb = SRGB_FORMATS + SRGB_BLOCK_FORMATS
+    if in_fmt in srgb:
+        f |= F.TEX_FILTER_SRGB_IN
+    elif in_fmt == 65:
+        f &= ~F.TEX_FILTER_SRGB_IN
+    if out_fmt in srgb:
+        f |= F.TEX_FILTER_SRGB_OUT
+    elif out_fmt == 65:
+        f &= ~F.TEX_FILTER_SRGB_OUT
+    if f == F.TEX_FILTER_SRGB:
+        f = 0
+    return f
+
+
+def powf_direction(flags, in_fmt, out_fmt):
+    """TEX_FILTER_SRGB_IN or _OUT when a Convert / Compress / Decompress from in_fmt to out_fmt with these flags runs a pixel
+    through powf, else 0.  sRGB -> linear runs on FLOAT and UNORM inputs, linear -> sRGB on FLOAT and UNORM outputs
+    (dxb_convert_pixel); every supported format is FLOAT, UNORM or SNORM."""
+    f = resolve_srgb(flags, in_fmt, out_fmt)
+    if f & F.TEX_FILTER_SRGB_IN and in_fmt not in SNORM_FORMATS:
+        return F.TEX_FILTER_SRGB_IN
+    if f & F.TEX_FILTER_SRGB_OUT and out_fmt not in SNORM_FORMATS:
+        return F.TEX_FILTER_SRGB_OUT
+    return 0
+
+
+def _fields(fmt):
+    """[(bit offset, bits, kind, decoded channel or None)] of one pixel of `fmt`, or None for R9G9B9E5 (shared exponent: whole
+    pixels).  kind: 'f32', 'f16', 'f11' (an R11G11B10 field) or 'int'.  Every field decodes into one channel alone, which
+    _probe checks on the oracle's decoding."""
+    if fmt in F32_FORMATS:
+        return [(32 * c, 32, "f32", c) for c in range(CHANNELS[fmt])]
+    if fmt in F16_FORMATS:
+        return [(16 * c, 16, "f16", c) for c in range(CHANNELS[fmt])]
+    if fmt == 67:
+        return None
+    bgra = [(0, 8, "int", 2), (8, 8, "int", 1), (16, 8, "int", 0)]
+    fixed = {26: [(0, 11, "f11", 0), (11, 11, "f11", 1), (22, 10, "f11", 2)],
+             24: [(0, 10, "int", 0), (10, 10, "int", 1), (20, 10, "int", 2), (30, 2, "int", 3)],
+             85: [(0, 5, "int", 2), (5, 6, "int", 1), (11, 5, "int", 0)],
+             86: [(0, 5, "int", 2), (5, 5, "int", 1), (10, 5, "int", 0), (15, 1, "int", 3)],
+             115: [(0, 4, "int", 2), (4, 4, "int", 1), (8, 4, "int", 0), (12, 4, "int", 3)],
+             87: bgra + [(24, 8, "int", 3)], 91: bgra + [(24, 8, "int", 3)], 88: bgra + [(24, 8, "int", None)], 93: bgra + [(24, 8, "int", None)],
+             65: [(0, 8, "int", 3)]}
+    if fmt in fixed:
+        return fixed[fmt]
+    size = 16 if fmt in (11, 13, 35, 37, 56, 58) else 8
+    return [(size * c, size, "int", c) for c in range(F.BYTES_PER_PIXEL[fmt] * 8 // size)]
+
+
+def _field_pool(kind, bits, rng):
+    """candidate values of one field: every pattern up to 16 bits (NaN patterns excluded), a seeded pool for fp32"""
+    if kind == "f32":
+        pool = np.concatenate([f32_edges(), rng.random(6144, dtype=np.float32), (rng.random(2048) * 1.4 - 0.2).astype(np.float32)])
+        return np.unique(pool.view(np.uint32))
+    if kind == "f16":
+        return half_patterns().astype(np.uint32)
+    v = np.arange(1 << bits, dtype=np.uint32)
+    if kind == "f11":
+        mb = bits - 5
+        v = v[~(((v >> np.uint32(mb)) == 31) & ((v & np.uint32((1 << mb) - 1)) != 0))]
+    return v
+
+
+def _pack(fmt, fields, cols):
+    """pixels of `fmt` as bytes (n, bpp) from one value column per field"""
+    n, bpp = len(cols[0]), F.BYTES_PER_PIXEL[fmt]
+    out = np.zeros((n, bpp), np.uint8)
+    word = np.zeros(n, np.uint32)
+    for (off, bits, _, _), col in zip(fields, cols):
+        if bits in (8, 16, 32) and off % 8 == 0:
+            out[:, off // 8:(off + bits) // 8] = col.astype("<u%d" % (bits // 8)).view(np.uint8).reshape(n, bits // 8)
+        else:
+            word |= col.astype(np.uint32) << np.uint32(off)
+    if any(not (bits in (8, 16, 32) and off % 8 == 0) for (off, bits, _, _) in fields):
+        out |= word.view(np.uint8).reshape(n, 4)[:, :bpp]
+    return out
+
+
+def _device_convert():
+    """capi.convert when a CUDA device is present, else None"""
+    try:
+        from directxtex_b200 import capi
+        if capi.lib.dxb200_device_count() > 0 and capi.lib.dxb200_init(0) == 0:
+            return capi.convert
+    except Exception:
+        pass
+    return None
+
+
+_SAFE = {}
+SRGB_SAFE_FRACTIONS = {}
+
+
+def _probe(fmt, direction):
+    """(fields, pools, safe masks) of `fmt` for one sRGB direction; cached"""
+    key = (fmt, direction)
+    if key in _SAFE:
+        return _SAFE[key]
+    from tests import oracle_lib
+    oracle = oracle_lib.load_ref()
+    rng = np.random.default_rng(fmt * 7 + direction)
+    fields = _fields(fmt)
+    if fields is None:
+        pools = [packed_patterns(fmt, seed=fmt)]
+        cols = pools
+        n = len(pools[0])
+        pixels = pools[0].astype("<u4").view(np.uint8).reshape(n, 4)
+    else:
+        pools = [_field_pool(kind, bits, rng) for (_, bits, kind, _) in fields]
+        n = max(len(p) for p in pools)
+        cols = [np.resize(p[rng.permutation(len(p))], n) for p in pools]
+        pixels = _pack(fmt, fields, cols)
+    # the value each channel enters the sRGB function with: the pixel as loaded (the oracle's bit-exact Convert to
+    # R32G32B32A32; for an sRGB format with both flags, which cancel its own sRGB -> linear step), and for linear -> sRGB
+    # from an SNORM source after its mapping to UNORM, v * 0.5 + 0.5 unfused
+    if fmt == 2:
+        dec = pixels
+    else:
+        hr, dec = oracle.convert(pixels, n, 1, fmt, 2, F.TEX_FILTER_SRGB if fmt in SRGB_FORMATS else 0)
+        assert hr == 0
+    u = np.ascontiguousarray(dec).view(np.float32).reshape(n, 4).copy()
+    if direction == F.TEX_FILTER_SRGB_OUT and fmt in SNORM_FORMATS:
+        u = (u * np.float32(0.5)).astype(np.float32) + np.float32(0.5)
+    # every distinct value through device and oracle Convert(R32_FLOAT -> R32G32B32A32_FLOAT) with the sRGB flag: the same
+    # dxb_convert_pixel the block encoders run, on the same inputs; a value is safe where both give the same bits
+    ubits = u[:, :3].view(np.uint32)
+    vals = np.unique(ubits)
+    device = _device_convert()
+    if device is None:
+        safe_vals = vals
+    else:
+        m = -(-len(vals) // 256) * 256
+        probe = np.zeros(m, np.uint32)
+        probe[:len(vals)] = vals
+        hr, want = oracle.convert(probe.view(np.float32), 256, m // 256, 41, 2, direction)
+        assert hr == 0
+        got = device(probe.view(np.float32), 256, m // 256, 41, 2, direction)
+        same = got.view(np.uint32).reshape(m, 4)[:, 0] == want.view(np.uint32).reshape(m, 4)[:, 0]
+        safe_vals = vals[same[:len(vals)]]
+    chan_safe = np.isin(ubits, safe_vals)
+    if fields is None:
+        masks = [chan_safe.all(1)]
+        kept, total = int(masks[0].sum()), n
+    else:
+        masks, kept, total = [], 0, 0
+        for (off, bits, kind, ch), pool, col in zip(fields, pools, cols):
+            if ch is None or ch == 3:                           # alpha and X never go through powf
+                masks.append(np.ones(len(pool), bool))
+                continue
+            # the field alone decides its channel (checks the layout of _fields)
+            pairs = np.unique(np.stack([col, ubits[:, ch]], 1), axis=0)
+            assert len(pairs) == len(np.unique(col)), (fmt, off)
+            bad = np.unique(col[~chan_safe[:, ch]])
+            masks.append(~np.isin(pool, bad))
+            kept += int(masks[-1].sum())
+            total += len(pool)
+    frac = kept / total if total else 1.0
+    SRGB_SAFE_FRACTIONS[key] = (kept, total)
+    print("srgb_safe_image: format %d %s: %d of %d values kept (%.1f %%)%s" % (
+        fmt, "SRGB_IN" if direction == F.TEX_FILTER_SRGB_IN else "SRGB_OUT", kept, total, 100.0 * frac, "" if device else " (oracle only)"))
+    assert frac >= 0.25, (fmt, direction, frac)
+    _SAFE[key] = (fields, pools, masks)
+    return _SAFE[key]
+
+
+def srgb_safe_image(fmt, direction, w, h, seed=0):
+    """A w x h source of `fmt` (tightly packed bytes) whose every channel value gives the same bits through CUDA's powf as
+    through glibc's, in the given direction (TEX_FILTER_SRGB_IN: sRGB -> linear on the loaded value; TEX_FILTER_SRGB_OUT:
+    linear -> sRGB after the conversion to UNORM).  A single ulp of difference can change a BC block, so an sRGB compress
+    or convert is compared bit for bit only on such inputs.  The candidates are every pattern of each field up to 16 bits
+    (every code of the 8-, 10- and 16-bit formats, every non-NaN half) and a seeded fp32 pool with the edge list; each
+    field's values are drawn independently from its safe set (R9G9B9E5: whole safe patterns).  Without a CUDA device
+    every value is kept."""
+    fields, pools, masks = _probe(fmt, direction)
+    rng = np.random.default_rng(seed)
+    n = w * h
+    cols = []
+    for pool, mask in zip(pools, masks):
+        keep = pool[mask]
+        cols.append(np.resize(keep[rng.permutation(len(keep))], n))
+    if fields is None:
+        return np.ascontiguousarray(cols[0].astype("<u4").view(np.uint8))
+    return np.ascontiguousarray(_pack(fmt, fields, cols).reshape(-1))
