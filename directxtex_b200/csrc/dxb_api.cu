@@ -709,12 +709,10 @@ int32_t launch_mips(const dxb200_image* chain, size_t items, size_t levels, uint
     dxb_mip_params P; memset(&P, 0, sizeof(P));
     P.format = fmt; P.mode = mode; P.filter = filter;
     P.lflags = dxb_resolve_srgb_linear(filter & DXB_FILTER_SRGB_MASK, fmt);
-    int32_t hr = DXB_S_OK;
     // job records of every level, built once and uploaded with ONE copy (a per-level upload left the GPU idle
     // between the small launches of the tail of the chain)
     std::vector<const dxb200_image*> stale(items, nullptr);
     std::vector<dxb_mip_job> all(items * (levels - 1));
-    std::vector<uint64_t> totals(levels, 0);
     for (size_t l = 1; l < levels; ++l)
     {
         uint64_t total = 0;
@@ -733,78 +731,36 @@ int32_t launch_mips(const dxb200_image* chain, size_t items, size_t levels, uint
                 j.stalePitch = stale[it]->rowPitch;
             }
         }
-        totals[l] = total;
     }
-    dxb_mip_job* dAll = nullptr;
-    // first level whose SOURCE is at most 64x64: from there on one CTA per item finishes the chain in one launch
-    size_t tailStart = levels;
-    for (size_t l = 1; l < levels; ++l)
-        if (chain[l - 1].width <= 64 && chain[l - 1].height <= 64) { tailStart = l; break; }
-    const bool wantTail = (mode == DXB_FILTER_BOX || mode == DXB_FILTER_LINEAR || mode == DXB_FILTER_CUBIC) && (levels - tailStart) >= 2 && items <= 0x7FFFFFFFull;
-    const bool wantFused = (mode == DXB_FILTER_BOX || mode == DXB_FILTER_LINEAR) && levels >= 4;      // LINEAR at 2:1 reads the same 2x2 patches
-    if (items > 1 || wantTail || wantFused)
+    // TRIANGLE's gather lists, X and Y of every level (shared by all items), travel in the same copy after the records
+    std::vector<TriLists> tri(mode == DXB_FILTER_TRIANGLE ? 2 * (levels - 1) : 0);
+    size_t bytes = all.size() * sizeof(dxb_mip_job);
+    for (size_t l = 1; l <= tri.size() / 2; ++l)
     {
-        DXB_CUDA(cudaMallocAsync(reinterpret_cast<void**>(&dAll), all.size() * sizeof(dxb_mip_job), stream));
-        DXB_CUDA(cudaMemcpyAsync(dAll, all.data(), all.size() * sizeof(dxb_mip_job), cudaMemcpyHostToDevice, stream));
+        build_triangle_axis(chain[l - 1].width, chain[l].width, (filter & DXB_FILTER_WRAP_U) != 0, tri[2 * (l - 1)]);
+        build_triangle_axis(chain[l - 1].height, chain[l].height, (filter & DXB_FILTER_WRAP_V) != 0, tri[2 * (l - 1) + 1]);
     }
-    for (size_t l = 1; l < levels && hr == DXB_S_OK; ++l)
+    for (const TriLists& t : tri) bytes += (t.off.size() + t.src.size()) * sizeof(uint32_t) + t.w.size() * sizeof(float);
+    uint8_t* dev = nullptr;
+    std::vector<dxb_tri_axis> axes(tri.size());
+    if (all.size() > 1 || !tri.empty())
     {
-        // three BOX / LINEAR levels per launch while the source is larger than the tail kernel's 64x64 and divides by 8
-        if (wantFused && l + 2 < levels && (chain[l - 1].width > 64 || chain[l - 1].height > 64))
+        DXB_CUDA(cudaMallocAsync(reinterpret_cast<void**>(&dev), bytes, stream));
+        std::vector<uint8_t> host(bytes);
+        size_t at = 0;
+        auto put = [&](const void* p, size_t n) { if (n) memcpy(host.data() + at, p, n); at += n; return dev + at - n; };
+        put(all.data(), all.size() * sizeof(dxb_mip_job));
+        for (size_t i = 0; i < tri.size(); ++i)
         {
-            P.njobs = (uint32_t)items;
-            if (dxb_launch_mip_box3(stream, dAll + (l - 1) * items, all.data() + (l - 1) * items, (uint32_t)items, P))
-            {
-                hr = check_launch("k_mip_box3");
-                l += 2;
-                continue;
-            }
+            axes[i].off = reinterpret_cast<const uint32_t*>(put(tri[i].off.data(), tri[i].off.size() * sizeof(uint32_t)));
+            axes[i].src = reinterpret_cast<const uint32_t*>(put(tri[i].src.data(), tri[i].src.size() * sizeof(uint32_t)));
+            axes[i].w = reinterpret_cast<const float*>(put(tri[i].w.data(), tri[i].w.size() * sizeof(float)));
         }
-        if (wantTail && l >= tailStart)
-        {
-            P.njobs = (uint32_t)items;
-            if (dxb_launch_mip_tail(stream, dAll + (l - 1) * items, (uint32_t)items, (uint32_t)(levels - l), P))
-            {
-                hr = check_launch("k_mip_tail");
-                break;
-            }
-        }
-        if (mode == DXB_FILTER_TRIANGLE)
-        {
-            // gather lists are per level and shared by all items
-            const dxb200_image& s0 = chain[l - 1]; const dxb200_image& d0 = chain[l];
-            TriLists tx, ty;
-            build_triangle_axis(s0.width, d0.width, (filter & DXB_FILTER_WRAP_U) != 0, tx);
-            build_triangle_axis(s0.height, d0.height, (filter & DXB_FILTER_WRAP_V) != 0, ty);
-            const size_t nOff = tx.off.size() + ty.off.size(), nEnt = tx.src.size() + ty.src.size();
-            uint32_t* dU = nullptr; float* dW = nullptr;
-            DXB_CUDA(cudaMallocAsync(reinterpret_cast<void**>(&dU), (nOff + nEnt) * sizeof(uint32_t), stream));
-            DXB_CUDA(cudaMallocAsync(reinterpret_cast<void**>(&dW), nEnt * sizeof(float), stream));
-            std::vector<uint32_t> hu; hu.reserve(nOff + nEnt);
-            hu.insert(hu.end(), tx.off.begin(), tx.off.end()); hu.insert(hu.end(), ty.off.begin(), ty.off.end());
-            hu.insert(hu.end(), tx.src.begin(), tx.src.end()); hu.insert(hu.end(), ty.src.begin(), ty.src.end());
-            std::vector<float> hw; hw.reserve(nEnt);
-            hw.insert(hw.end(), tx.w.begin(), tx.w.end()); hw.insert(hw.end(), ty.w.begin(), ty.w.end());
-            DXB_CUDA(cudaMemcpyAsync(dU, hu.data(), hu.size() * sizeof(uint32_t), cudaMemcpyHostToDevice, stream));
-            DXB_CUDA(cudaMemcpyAsync(dW, hw.data(), hw.size() * sizeof(float), cudaMemcpyHostToDevice, stream));
-            DXB_CUDA(cudaStreamSynchronize(stream));      // host vectors go out of scope below
-            P.triX.off = dU; P.triY.off = dU + tx.off.size();
-            P.triX.src = dU + nOff; P.triY.src = dU + nOff + tx.src.size();
-            P.triX.w = dW; P.triY.w = dW + tx.w.size();
-        }
-        const uint64_t total = totals[l];
-        P.totalUnits = (uint32_t)total; P.njobs = (uint32_t)items;
-        const uint32_t need = (uint32_t)((total + 255) / 256);
-        const uint32_t grid = std::max(1u, std::min<uint32_t>(need, (uint32_t)t_v.dev->gridRow * 8u));
-        dxb_launch_mip(grid, stream, (dAll && items > 1) ? dAll + (l - 1) * items : nullptr, all.data() + (l - 1) * items, P);
-        hr = check_launch("k_mip_level");
-        if (mode == DXB_FILTER_TRIANGLE)
-        {
-            cudaFreeAsync(const_cast<uint32_t*>(P.triX.off), stream);
-            cudaFreeAsync(const_cast<float*>(P.triX.w), stream);
-        }
+        DXB_CUDA(cudaMemcpyAsync(dev, host.data(), bytes, cudaMemcpyHostToDevice, stream));
     }
-    if (dAll) cudaFreeAsync(dAll, stream);
+    const int32_t hr = dxb_launch_mip_chain(stream, reinterpret_cast<const dxb_mip_job*>(dev), all.data(), (uint32_t)items, (uint32_t)levels, P,
+                                            tri.empty() ? nullptr : axes.data(), (unsigned)t_v.dev->gridRow * 8u, check_launch);
+    if (dev) cudaFreeAsync(dev, stream);
     return hr;
 }
 

@@ -2,10 +2,13 @@
 //   k_convert            generic: one thread per pixel, any implemented format pair, heterogeneous batches
 //   k_convert_vec<SF,DF> hot pairs: compile-time formats, 16-byte vector access on the wider side, uniform batches
 //   k_mip_level          generic: one thread per destination pixel, any format / filter
-//   k_mip_tile<FMT,MODE> hot formats x {BOX,LINEAR,CUBIC}: compile-time format and filter, 2D thread tiles,
+//   k_mip_tile<FMT,MODE,SRGB>  hot formats x {BOX,LINEAR,CUBIC}: compile-time format and filter, 2D thread tiles,
 //                        grid.z = array item (all items of a level have the same size), no integer division
-// The arithmetic is the same inline code in all variants (dxb_pixel.cuh / dxb_mips.cuh), so all of them are
-// bit-exact against the oracle; only the memory access pattern differs.
+//   k_mip_sep<FMT,SRGB>  CUBIC levels of a chain: separable, each source row decoded and filtered once per tile
+//   k_mip_tail<FMT,MODE,SRGB>  the levels from 64x64 down: one CTA per item
+//   k_mip_box3<FMT,SRGB,LIN>  three BOX (or 2:1 LINEAR) levels per pass
+// dxb_launch_mip_chain picks the kernel of every level.  The arithmetic is the same inline code in all variants
+// (dxb_pixel.cuh / dxb_mips.cuh), so all of them are bit-exact against the oracle; only the memory access pattern differs.
 #include "dxb_launch.h"
 #include "dxb_pixel.cuh"
 #include "dxb_mips.cuh"
@@ -49,20 +52,25 @@ __global__ void __launch_bounds__(256) k_mip_level(const dxb_mip_job* __restrict
         const dxb_mip_job& j = dxb_find_job(jobs, P.njobs, single, unit);
         const uint32_t local = unit - j.firstUnit;
         const uint32_t y = local / j.dw, x = local - y * j.dw;
-        dxb_px v;
-        switch (P.mode)
-        {
-        case DXB_FILTER_POINT:
-            v = dxb_mip_point(P.format, j, x, y);
-            dxb_store_pixel(P.format, j.dst + (size_t)y * j.dstPitch, x, v);
-            continue;
-        case DXB_FILTER_BOX: v = dxb_mip_box(P.format, j, x, y, P.lflags); break;
-        case DXB_FILTER_LINEAR: v = dxb_mip_linear(P.format, j, x, y, P.filter, P.lflags); break;
-        case DXB_FILTER_CUBIC: v = dxb_mip_cubic(P.format, j, x, y, P.filter, P.lflags); break;
-        default: v = dxb_mip_triangle(P.format, j, x, y, P.lflags, P.triX, P.triY); break;
-        }
-        dxb_store_linear(P.format, j.dst, j.dstPitch, x, y, v, P.lflags);
+        dxb_mip_pixel(P.format, P.mode, j, x, y, P.filter, P.lflags, P.triX, P.triY);
     }
+}
+
+// ------------------------------------------------------------------------------------------------ batch predicates
+// p and pitch are multiples of one vector access of `bytes` bytes (at most 16)
+static bool vec_aligned(const void* p, size_t pitch, uint32_t bytes)
+{
+    const uint32_t v = bytes < 16u ? bytes : 16u;
+    return ((uintptr_t)p % v) == 0 && (pitch % v) == 0;
+}
+static bool same_size(const dxb_job& a, const dxb_job& b) { return a.width == b.width && a.height == b.height; }
+static bool same_size(const dxb_mip_job& a, const dxb_mip_job& b) { return a.sw == b.sw && a.sh == b.sh && a.dw == b.dw && a.dh == b.dh; }
+// every job has the first one's size and there is one per gridDim.z slice: one grid covers the batch
+template <typename J> static bool uniform_batch(const J* jobs, uint32_t n)
+{
+    if (n > 65535u) return false;
+    for (uint32_t i = 1; i < n; ++i) if (!same_size(jobs[i], jobs[0])) return false;
+    return true;
 }
 
 // ------------------------------------------------------------------------------------------------ vector convert
@@ -144,14 +152,9 @@ __global__ void __launch_bounds__(256) k_convert_vec(const dxb_job* __restrict__
 static bool convert_vec_ok(const dxb_job* hostJobs, uint32_t njobs, uint32_t SB, uint32_t DB)
 {
     const uint32_t ppt = 16u / (SB > DB ? SB : DB);
-    const size_t sby = (size_t)SB * ppt, dby = (size_t)DB * ppt;
-    if (njobs > 65535u || hostJobs[0].height > 65535u) return false;
+    if (hostJobs[0].height > 65535u || !uniform_batch(hostJobs, njobs)) return false;
     for (uint32_t i = 0; i < njobs; ++i)
-    {
-        const dxb_job& j = hostJobs[i];
-        if (j.width != hostJobs[0].width || j.height != hostJobs[0].height) return false;
-        if (((uintptr_t)j.src % sby) || ((uintptr_t)j.dst % dby) || (j.srcPitch % sby) || (j.dstPitch % dby)) return false;
-    }
+        if (!vec_aligned(hostJobs[i].src, hostJobs[i].srcPitch, SB * ppt) || !vec_aligned(hostJobs[i].dst, hostJobs[i].dstPitch, DB * ppt)) return false;
     return true;
 }
 
@@ -285,13 +288,6 @@ void dxb_launch_scale_alpha(unsigned grid, cudaStream_t stream, const dxb_job& j
 }
 
 // ------------------------------------------------------------------------------------------------ tiled mips
-template <uint32_t FMT, uint32_t MODE>
-__device__ __forceinline__ dxb_px dxb_mip_eval(const dxb_mip_job& j, uint32_t x, uint32_t y, const dxb_mip_params& P, uint32_t lflags)
-{
-    if (MODE == DXB_FILTER_BOX) return dxb_mip_box(FMT, j, x, y, lflags);
-    if (MODE == DXB_FILTER_LINEAR) return dxb_mip_linear(FMT, j, x, y, P.filter, lflags);
-    return dxb_mip_cubic(FMT, j, x, y, P.filter, lflags);
-}
 // The sRGB <-> linear steps are a COMPILE-TIME property of the specialised kernels (SRGB = both SRGB_IN and SRGB_OUT,
 // the only combination a mip chain produces; anything else takes the generic kernel): with a run-time flag every
 // instantiation carried the inlined powf code (26.5 k SASS instructions for the fused BOX kernel) and stalled on
@@ -300,8 +296,7 @@ __device__ __forceinline__ dxb_px dxb_mip_eval(const dxb_mip_job& j, uint32_t x,
 
 #define DXB_CUBIC_KY 4u       // output rows per thread of the CUBIC tile kernel
 // grid = (ceil(dw/32), ceil(dh/8), items) (CUBIC: ceil(dh / (8 * DXB_CUBIC_KY))); jobs[z] describes item z (all items share the level's size).
-// VEC: source rows are aligned for one vector load of two adjacent pixels (BOX only).
-template <uint32_t FMT, uint32_t MODE, bool VEC, bool SRGB>
+template <uint32_t FMT, uint32_t MODE, bool SRGB>
 __global__ void __launch_bounds__(256) k_mip_tile(const dxb_mip_job* __restrict__ jobs, dxb_mip_job single, dxb_mip_params P)
 {
     const dxb_mip_job& j = (jobs == nullptr) ? single : jobs[blockIdx.z];
@@ -353,12 +348,13 @@ __global__ void __launch_bounds__(256) k_mip_tile(const dxb_mip_job* __restrict_
     }
     const uint32_t x = blockIdx.x * 32u + threadIdx.x, y = blockIdx.y * 8u + threadIdx.y;
     if (x >= j.dw || y >= j.dh) return;
-    dxb_px v;
+    if (MODE != DXB_FILTER_BOX) { dxb_mip_pixel(FMT, MODE, j, x, y, P.filter, LF, P.triX, P.triY); return; }
+    // BOX: the vector and the scalar path share one store (a second copy of the inlined sRGB store costs ~260 instructions).
+    // Alignment is decided per item (uniform within the CTA: blockIdx.z selects the item).
     constexpr int B = (int)dxb_bytes_per_pixel(FMT);
+    dxb_px v;
     constexpr uintptr_t VA = (B * 2 <= 16) ? B * 2 : 16;
-    // VEC = every item is aligned; otherwise decide per item (uniform within the CTA: blockIdx.z selects the item)
-    const bool vecOK = VEC || ((((uintptr_t)j.src % VA) == 0) && ((j.srcPitch % VA) == 0));
-    if (MODE == DXB_FILTER_BOX && vecOK && j.sw > 1 && j.sh > 1)
+    if ((((uintptr_t)j.src % VA) == 0) && ((j.srcPitch % VA) == 0) && j.sw > 1 && j.sh > 1)
     {
         // two horizontally adjacent source pixels per row in one vector load: ((p00 + p10) + p01) + p11) * 0.25
         constexpr int VB = (B * 2 <= 16) ? B * 2 : 16;
@@ -378,7 +374,7 @@ __global__ void __launch_bounds__(256) k_mip_tile(const dxb_mip_job* __restrict_
         v = dxb_px_add(v, p11);
         v = dxb_px_scale(v, 0.25f);
     }
-    else v = dxb_mip_eval<FMT, MODE>(j, x, y, P, LF);
+    else v = dxb_mip_box(FMT, j, x, y, LF);
     dxb_store_linear(FMT, j.dst, j.dstPitch, x, y, v, LF);
 }
 
@@ -395,62 +391,42 @@ template <int N> __device__ __forceinline__ void dxb_copy_vec(uint8_t* dst, cons
     }
 }
 
-// ------------------------------------------------------------------------------------------------ separable LINEAR / CUBIC
+// ------------------------------------------------------------------------------------------------ separable CUBIC
 // One CTA (8 warps) = a 32 x 16 tile of destination pixels.  The reference filters every source row horizontally and then
-// combines 2 (LINEAR) or 4 (CUBIC) of those rows vertically (DirectXTexMipmaps.cpp:1087-1197, 1204-1388); k_mip_tile redoes the
-// horizontal pass for every destination pixel and decodes ~10 source pixels per output.  Here
+// combines 4 of those rows vertically (DirectXTexMipmaps.cpp:1204-1388); k_mip_tile redoes the horizontal pass for every
+// destination pixel and decodes ~10 source pixels per output.  Here
 //   stage A  a warp takes one source row of the tile at a time: its lanes decode the row's pixels ONCE into the warp's
 //            shared row buffer (load + format decode + sRGB linearisation),
 //   stage B  lane x filters that row horizontally for destination column x (same operands, same operation order as
-//            dxb_mip_linear / dxb_mip_cubic) into the shared H[row][x],
+//            dxb_mip_cubic) into the shared H[row][x],
 //   stage C  after one barrier every thread combines the H rows of its two destination pixels vertically and stores them.
 // Per destination pixel of a 2:1 level that is 4.4 pixel decodes, 2.1 horizontal and 1 vertical filter evaluations instead
 // of 10 / 2.5 / 1.  Source coordinates are kept UNBOUNDED inside the tile (consecutive slots of the row buffer / of H) and
-// bounded (clamp / wrap / mirror, filters.h:64-104, 123-207) only when the pixel is fetched, so every addressing mode of
+// bounded (clamp / wrap / mirror, filters.h:123-207) only when the pixel is fetched, so every addressing mode of
 // the reference takes the same path.  Requires source extent <= 3 x destination extent (every level of a mip chain).
 #define DXB_SEP_TW 32
 #define DXB_SEP_TH 16
 #define DXB_SEP_MAXC (DXB_SEP_TW * 3 + 4)
 #define DXB_SEP_MAXR (DXB_SEP_TH * 3 + 4)
 
-// unbounded tap base and weight of destination coordinate u: LINEAR taps base, base + 1 (weights w, 1 - w);
-// CUBIC taps base - 1 .. base + 2 (fraction w)
-template <uint32_t MODE>
+// unbounded tap base and fraction of destination coordinate u: taps base - 1 .. base + 2
 __device__ __forceinline__ void dxb_sep_entry(uint32_t source, uint32_t dest, uint32_t u, int32_t* base, float* w)
 {
     const float scale = (float)source / (float)dest;
     const float t = ((float)u + 0.5f) * scale;
-    if (MODE == DXB_FILTER_LINEAR)
-    {
-        const float srcB = t + 0.5f;
-        const int64_t isrcB = (int64_t)srcB;
-        const float wsum = 1.0f + (float)isrcB;
-        *w = wsum - srcB; *base = (int32_t)(isrcB - 1);
-    }
-    else
-    {
-        const float srcB = t - 0.5f;
-        const int64_t isrcB = (int64_t)srcB;              // always inside [0, source - 1]: dxb_cubic_entry's bounduvw is the identity on it
-        *w = srcB - (float)isrcB; *base = (int32_t)isrcB;
-    }
+    const float srcB = t - 0.5f;
+    const int64_t isrcB = (int64_t)srcB;              // always inside [0, source - 1]: dxb_cubic_entry's bounduvw is the identity on it
+    *w = srcB - (float)isrcB; *base = (int32_t)isrcB;
 }
-template <uint32_t MODE>
 __device__ __forceinline__ uint32_t dxb_sep_bound(int32_t i, uint32_t source, bool wrap, bool mirror)
 {
-    if (MODE == DXB_FILTER_LINEAR)
-    {
-        if (i < 0) return wrap ? source - 1u : 0u;                               // CreateLinearFilter (filters.h:86-97)
-        if ((uint32_t)i >= source) return wrap ? 0u : source - 1u;
-        return (uint32_t)i;
-    }
     return (uint32_t)dxb_bounduvw((int64_t)i, (int64_t)source - 1, wrap, mirror);
 }
 
-template <uint32_t FMT, uint32_t MODE, bool SRGB>
+template <uint32_t FMT, bool SRGB>
 __global__ void __launch_bounds__(256) k_mip_sep(const dxb_mip_job* __restrict__ jobs, dxb_mip_job single, dxb_mip_params P)
 {
     constexpr uint32_t LF = DXB_LF(SRGB);
-    constexpr int TAPS = (MODE == DXB_FILTER_CUBIC) ? 4 : 2, LEAD = (MODE == DXB_FILTER_CUBIC) ? 1 : 0;
     const dxb_mip_job& j = (jobs == nullptr) ? single : jobs[blockIdx.z];
     __shared__ float4 H[DXB_SEP_MAXR][DXB_SEP_TW];
     __shared__ float4 rowbuf[8][DXB_SEP_MAXC];
@@ -459,26 +435,26 @@ __global__ void __launch_bounds__(256) k_mip_sep(const dxb_mip_job* __restrict__
     const uint32_t tid = threadIdx.y * 32u + threadIdx.x, warp = threadIdx.y, lane = threadIdx.x;
     const uint32_t ox = blockIdx.x * DXB_SEP_TW, oy = blockIdx.y * DXB_SEP_TH;
     const uint32_t tw = min((uint32_t)DXB_SEP_TW, j.dw - ox), th = min((uint32_t)DXB_SEP_TH, j.dh - oy);
-    if (tid < DXB_SEP_TW) { int32_t b; float w; dxb_sep_entry<MODE>(j.sw, j.dw, ox + min(tid, tw - 1u), &b, &w); colBase[tid] = b; colW[tid] = w; }
-    else if (tid < DXB_SEP_TW + DXB_SEP_TH) { const uint32_t r = tid - DXB_SEP_TW; int32_t b; float w; dxb_sep_entry<MODE>(j.sh, j.dh, oy + min(r, th - 1u), &b, &w); rowBase[r] = b; rowW[r] = w; }
+    if (tid < DXB_SEP_TW) { int32_t b; float w; dxb_sep_entry(j.sw, j.dw, ox + min(tid, tw - 1u), &b, &w); colBase[tid] = b; colW[tid] = w; }
+    else if (tid < DXB_SEP_TW + DXB_SEP_TH) { const uint32_t r = tid - DXB_SEP_TW; int32_t b; float w; dxb_sep_entry(j.sh, j.dh, oy + min(r, th - 1u), &b, &w); rowBase[r] = b; rowW[r] = w; }
     __syncthreads();
     const bool wrapU = (P.filter & DXB_FILTER_WRAP_U) != 0, mirU = (P.filter & DXB_FILTER_MIRROR_U) != 0;
     const bool wrapV = (P.filter & DXB_FILTER_WRAP_V) != 0, mirV = (P.filter & DXB_FILTER_MIRROR_V) != 0;
-    const int32_t c0 = colBase[0] - LEAD, ncols = colBase[tw - 1u] + (TAPS - 1 - LEAD) - c0 + 1;
-    const int32_t r0 = rowBase[0] - LEAD, nrows = rowBase[th - 1u] + (TAPS - 1 - LEAD) - r0 + 1;
-    const int32_t myc = colBase[lane] - LEAD - c0;
+    const int32_t c0 = colBase[0] - 1, ncols = colBase[tw - 1u] + 2 - c0 + 1;
+    const int32_t r0 = rowBase[0] - 1, nrows = rowBase[th - 1u] + 2 - r0 + 1;
+    const int32_t myc = colBase[lane] - 1 - c0;
     const float myw = colW[lane];
     // the bounded source column of every row-buffer slot this lane fills is the same for all rows: computed once
     constexpr int SPL = (DXB_SEP_MAXC + 31) / 32;
     uint32_t mycol[SPL];
     #pragma unroll
-    for (int k = 0; k < SPL; ++k) mycol[k] = dxb_sep_bound<MODE>(c0 + (int32_t)lane + 32 * k, j.sw, wrapU, mirU);
+    for (int k = 0; k < SPL; ++k) mycol[k] = dxb_sep_bound(c0 + (int32_t)lane + 32 * k, j.sw, wrapU, mirU);
     // software pipeline: the raw pixels of this warp's NEXT source row are in flight while the current row is decoded and filtered
     constexpr int B = (int)dxb_bytes_per_pixel(FMT);
     __align__(16) uint8_t raw[SPL][B];
     auto fetch = [&](int32_t r)
     {
-        const uint8_t* srow = j.src + (size_t)dxb_sep_bound<MODE>(r0 + r, j.sh, wrapV, mirV) * j.srcPitch;
+        const uint8_t* srow = j.src + (size_t)dxb_sep_bound(r0 + r, j.sh, wrapV, mirV) * j.srcPitch;
         #pragma unroll
         for (int k = 0; k < SPL; ++k)
             if ((int32_t)lane + 32 * k < ncols) dxb_copy_vec<B>(raw[k], srow + (size_t)mycol[k] * B, false);
@@ -498,12 +474,10 @@ __global__ void __launch_bounds__(256) k_mip_sep(const dxb_mip_job* __restrict__
         __syncwarp();
         if (lane < tw)
         {
-            dxb_px q[TAPS];
+            dxb_px q[4];
             #pragma unroll
-            for (int k = 0; k < TAPS; ++k) { const float4 f = rowbuf[warp][myc + k]; q[k] = dxb_make_px(f.x, f.y, f.z, f.w); }
-            dxb_px h;
-            if (MODE == DXB_FILTER_CUBIC) h = dxb_cubic4(myw, q[0], q[1], q[2], q[3]);
-            else h = dxb_px_add(dxb_px_scale(q[0], myw), dxb_px_scale(q[1], 1.0f - myw));
+            for (int k = 0; k < 4; ++k) { const float4 f = rowbuf[warp][myc + k]; q[k] = dxb_make_px(f.x, f.y, f.z, f.w); }
+            const dxb_px h = dxb_cubic4(myw, q[0], q[1], q[2], q[3]);
             H[r][lane] = make_float4(h.x, h.y, h.z, h.w);
         }
         __syncwarp();
@@ -515,15 +489,12 @@ __global__ void __launch_bounds__(256) k_mip_sep(const dxb_mip_job* __restrict__
     {
         const uint32_t y = warp + 8u * k;
         if (y >= th) break;
-        const int32_t rr = rowBase[y] - LEAD - r0;
+        const int32_t rr = rowBase[y] - 1 - r0;
         const float wy = rowW[y];
-        dxb_px c[TAPS];
+        dxb_px c[4];
         #pragma unroll
-        for (int t = 0; t < TAPS; ++t) { const float4 f = H[rr + t][lane]; c[t] = dxb_make_px(f.x, f.y, f.z, f.w); }
-        dxb_px v;
-        if (MODE == DXB_FILTER_CUBIC) v = dxb_cubic4(wy, c[0], c[1], c[2], c[3]);
-        else v = dxb_px_add(dxb_px_scale(c[0], wy), dxb_px_scale(c[1], 1.0f - wy));
-        dxb_store_linear(FMT, j.dst, j.dstPitch, ox + lane, oy + y, v, LF);
+        for (int t = 0; t < 4; ++t) { const float4 f = H[rr + t][lane]; c[t] = dxb_make_px(f.x, f.y, f.z, f.w); }
+        dxb_store_linear(FMT, j.dst, j.dstPitch, ox + lane, oy + y, dxb_cubic4(wy, c[0], c[1], c[2], c[3]), LF);
     }
 }
 
@@ -540,75 +511,11 @@ __global__ void __launch_bounds__(256) k_mip_tail(const dxb_mip_job* __restrict_
         for (uint32_t i = threadIdx.x; i < n; i += blockDim.x)
         {
             const uint32_t y = i / j.dw, x = i - y * j.dw;
-            const dxb_px v = dxb_mip_eval<FMT, MODE>(j, x, y, P, DXB_LF(SRGB));
-            dxb_store_linear(FMT, j.dst, j.dstPitch, x, y, v, DXB_LF(SRGB));
+            dxb_mip_pixel(FMT, MODE, j, x, y, P.filter, DXB_LF(SRGB), P.triX, P.triY);
         }
         __threadfence_block();
         __syncthreads();
     }
-}
-
-#define DXB_MIP_FORMATS(X, MODE) X(28, MODE) X(29, MODE) X(10, MODE) X(2, MODE) X(61, MODE) X(41, MODE) X(87, MODE)
-
-static bool mip_uniform(const dxb_mip_job* hostJobs, uint32_t njobs, uint32_t bpp, bool* vec)
-{
-    if (njobs > 65535u) return false;
-    *vec = true;
-    const uint32_t va = (2 * bpp <= 16) ? 2 * bpp : 16;
-    for (uint32_t i = 0; i < njobs; ++i)
-    {
-        const dxb_mip_job& j = hostJobs[i];
-        if (j.dw != hostJobs[0].dw || j.dh != hostJobs[0].dh || j.sw != hostJobs[0].sw || j.sh != hostJobs[0].sh) return false;
-        if (((uintptr_t)j.src % va) || (j.srcPitch % va)) *vec = false;
-    }
-    return true;
-}
-
-void dxb_launch_mip(unsigned grid, cudaStream_t stream, const dxb_mip_job* jobs, const dxb_mip_job* hostJobs, const dxb_mip_params& P)
-{
-    bool vec = false;
-    const bool srgb = (P.lflags == (DXB_FILTER_SRGB_IN | DXB_FILTER_SRGB_OUT));
-    if ((srgb || P.lflags == 0) && mip_uniform(hostJobs, P.njobs, dxb_bytes_per_pixel(P.format), &vec) &&
-        (P.mode == DXB_FILTER_BOX || P.mode == DXB_FILTER_LINEAR || P.mode == DXB_FILTER_CUBIC))
-    {
-        const dim3 blk(32, 8, 1);
-        // LINEAR / CUBIC of a chain level (source <= 3 x destination per axis): separable shared-memory kernel
-        // (LINEAR at 2:1 has no tap shared between neighbouring outputs: the plain tile kernel is faster there, 0.24 vs 0.43 ms per 64 x 1024^2 chain)
-        bool pixAligned = true;                     // k_mip_sep fetches whole pixels with one vector load each
-        {
-            const uint32_t bpp = dxb_bytes_per_pixel(P.format), va = bpp >= 16 ? 16 : bpp;
-            for (uint32_t i = 0; i < P.njobs; ++i) if (((uintptr_t)hostJobs[i].src % va) || (hostJobs[i].srcPitch % va)) pixAligned = false;
-        }
-        if (P.mode == DXB_FILTER_CUBIC && pixAligned && hostJobs[0].sw <= 3u * hostJobs[0].dw && hostJobs[0].sh <= 3u * hostJobs[0].dh)
-        {
-            const dim3 gs((hostJobs[0].dw + DXB_SEP_TW - 1) / DXB_SEP_TW, (hostJobs[0].dh + DXB_SEP_TH - 1) / DXB_SEP_TH, P.njobs);
-            if (gs.y <= 65535u)
-            {
-#define DXB_X(FMT, MODE) if (P.format == FMT && P.mode == MODE) { \
-                    if (srgb) k_mip_sep<FMT, MODE, true><<<gs, blk, 0, stream>>>(jobs, hostJobs[0], P); \
-                    else k_mip_sep<FMT, MODE, false><<<gs, blk, 0, stream>>>(jobs, hostJobs[0], P); \
-                    return; }
-                DXB_MIP_FORMATS(DXB_X, DXB_FILTER_CUBIC)
-#undef DXB_X
-            }
-        }
-        const uint32_t rowsPerCta = (P.mode == DXB_FILTER_CUBIC) ? 8u * DXB_CUBIC_KY : 8u;
-        const dim3 g((hostJobs[0].dw + 31) / 32, (hostJobs[0].dh + rowsPerCta - 1) / rowsPerCta, P.njobs);
-        if (g.y <= 65535u)
-        {
-#define DXB_X(FMT, MODE) if (P.format == FMT && P.mode == MODE) { \
-                if (vec && srgb) k_mip_tile<FMT, MODE, true, true><<<g, blk, 0, stream>>>(jobs, hostJobs[0], P); \
-                else if (vec) k_mip_tile<FMT, MODE, true, false><<<g, blk, 0, stream>>>(jobs, hostJobs[0], P); \
-                else if (srgb) k_mip_tile<FMT, MODE, false, true><<<g, blk, 0, stream>>>(jobs, hostJobs[0], P); \
-                else k_mip_tile<FMT, MODE, false, false><<<g, blk, 0, stream>>>(jobs, hostJobs[0], P); \
-                return; }
-            DXB_MIP_FORMATS(DXB_X, DXB_FILTER_BOX)
-            DXB_MIP_FORMATS(DXB_X, DXB_FILTER_LINEAR)
-            DXB_MIP_FORMATS(DXB_X, DXB_FILTER_CUBIC)
-#undef DXB_X
-        }
-    }
-    k_mip_level<<<grid, 256, 0, stream>>>(jobs, hostJobs[0], P);
 }
 
 // ------------------------------------------------------------------------------------------------ fused BOX levels
@@ -687,47 +594,131 @@ __global__ void __launch_bounds__(256) k_mip_box3(const dxb_mip_job* __restrict_
     dxb_copy_vec<B>(jC.dst + (size_t)ty * jC.dstPitch + (size_t)tx * B, pc, false);
 }
 
-// hostJobs: [3][items] records of levels l, l+1, l+2.  Returns false when the fused kernel does not apply.
-bool dxb_launch_mip_box3(cudaStream_t stream, const dxb_mip_job* jobsDev, const dxb_mip_job* hostJobs, uint32_t items, const dxb_mip_params& P)
+// ------------------------------------------------------------------------------------------------ chain launcher
+#define DXB_MIP_FORMATS(X, MODE) X(28, MODE) X(29, MODE) X(10, MODE) X(2, MODE) X(61, MODE) X(41, MODE) X(87, MODE)
+
+// hj: [3][items] records of levels l, l+1, l+2.  Returns false when the fused kernel does not apply (nothing launched).
+static bool launch_box3(cudaStream_t stream, const dxb_mip_job* jobs, const dxb_mip_job* hj, uint32_t items, const dxb_mip_params& P, bool srgb)
 {
-    if ((P.mode != DXB_FILTER_BOX && P.mode != DXB_FILTER_LINEAR) || items == 0 || items > 65535u || jobsDev == nullptr) return false;
-    const bool lin = (P.mode == DXB_FILTER_LINEAR);
-    const bool srgb = (P.lflags == (DXB_FILTER_SRGB_IN | DXB_FILTER_SRGB_OUT));
-    if (!srgb && P.lflags != 0) return false;
     const uint32_t B = dxb_bytes_per_pixel(P.format);
-    const dxb_mip_job& a0 = hostJobs[0];
-    if (B == 0 || (a0.sw & 7u) || (a0.sh & 7u) || a0.sw < 8u || a0.sh < 8u) return false;
-    auto al = [](const void* p, size_t pitch, uint32_t bytes) { const uint32_t v = bytes >= 16 ? 16 : bytes; return ((uintptr_t)p % v) == 0 && (pitch % v) == 0; };
+    const dxb_mip_job& a0 = hj[0];
+    if ((a0.sw & 7u) || (a0.sh & 7u) || a0.sw < 8u || a0.sh < 8u || !uniform_batch(hj, items)) return false;
     for (uint32_t i = 0; i < items; ++i)
     {
-        const dxb_mip_job& a = hostJobs[i]; const dxb_mip_job& b = hostJobs[items + i]; const dxb_mip_job& c = hostJobs[2 * (size_t)items + i];
-        if (a.sw != a0.sw || a.sh != a0.sh || a.dw != a.sw / 2 || a.dh != a.sh / 2 || b.dw != a.sw / 4 || b.dh != a.sh / 4 || c.dw != a.sw / 8 || c.dh != a.sh / 8) return false;
+        const dxb_mip_job& a = hj[i]; const dxb_mip_job& b = hj[items + i]; const dxb_mip_job& c = hj[2 * (size_t)items + i];
+        if (a.dw != a.sw / 2 || a.dh != a.sh / 2 || b.dw != a.sw / 4 || b.dh != a.sh / 4 || c.dw != a.sw / 8 || c.dh != a.sh / 8) return false;
         if (b.src != a.dst || c.src != b.dst || b.srcPitch != a.dstPitch || c.srcPitch != b.dstPitch) return false;
-        if (!al(a.src, a.srcPitch, 8 * B) || !al(a.dst, a.dstPitch, 4 * B) || !al(b.dst, b.dstPitch, 2 * B) || !al(c.dst, c.dstPitch, B)) return false;
+        if (!vec_aligned(a.src, a.srcPitch, 8 * B) || !vec_aligned(a.dst, a.dstPitch, 4 * B) || !vec_aligned(b.dst, b.dstPitch, 2 * B) ||
+            !vec_aligned(c.dst, c.dstPitch, B)) return false;
     }
     const dim3 blk(32, 8, 1);
     const dim3 g((a0.sw / 8 + 31) / 32, (a0.sh / 8 + 7) / 8, items);
     if (g.y > 65535u) return false;
+    const bool lin = (P.mode == DXB_FILTER_LINEAR);
 #define DXB_X(FMT, MODE) if (P.format == FMT) { \
-        if (lin) { if (srgb) k_mip_box3<FMT, true, true><<<g, blk, 0, stream>>>(jobsDev, items, P); else k_mip_box3<FMT, false, true><<<g, blk, 0, stream>>>(jobsDev, items, P); } \
-        else { if (srgb) k_mip_box3<FMT, true, false><<<g, blk, 0, stream>>>(jobsDev, items, P); else k_mip_box3<FMT, false, false><<<g, blk, 0, stream>>>(jobsDev, items, P); } \
+        if (lin) { if (srgb) k_mip_box3<FMT, true, true><<<g, blk, 0, stream>>>(jobs, items, P); else k_mip_box3<FMT, false, true><<<g, blk, 0, stream>>>(jobs, items, P); } \
+        else { if (srgb) k_mip_box3<FMT, true, false><<<g, blk, 0, stream>>>(jobs, items, P); else k_mip_box3<FMT, false, false><<<g, blk, 0, stream>>>(jobs, items, P); } \
         return true; }
     DXB_MIP_FORMATS(DXB_X, 0)
 #undef DXB_X
     return false;
 }
 
-// levels [first, first+count) of every item in ONE launch; returns false when the format/filter has no tail kernel
-bool dxb_launch_mip_tail(cudaStream_t stream, const dxb_mip_job* jobsDev, uint32_t items, uint32_t count, const dxb_mip_params& P)
+// levels l .. l + count - 1 of every item in one launch; jobs: their [level][item] records
+static void launch_tail(cudaStream_t stream, const dxb_mip_job* jobs, uint32_t items, uint32_t count, const dxb_mip_params& P, bool srgb)
 {
-    const bool srgb = (P.lflags == (DXB_FILTER_SRGB_IN | DXB_FILTER_SRGB_OUT));
-    if (!srgb && P.lflags != 0) return false;
 #define DXB_X(FMT, MODE) if (P.format == FMT && P.mode == MODE) { \
-        if (srgb) k_mip_tail<FMT, MODE, true><<<items, 256, 0, stream>>>(jobsDev, items, count, P); else k_mip_tail<FMT, MODE, false><<<items, 256, 0, stream>>>(jobsDev, items, count, P); \
-        return true; }
+        if (srgb) k_mip_tail<FMT, MODE, true><<<items, 256, 0, stream>>>(jobs, items, count, P); else k_mip_tail<FMT, MODE, false><<<items, 256, 0, stream>>>(jobs, items, count, P); \
+        return; }
     DXB_MIP_FORMATS(DXB_X, DXB_FILTER_BOX)
     DXB_MIP_FORMATS(DXB_X, DXB_FILTER_LINEAR)
     DXB_MIP_FORMATS(DXB_X, DXB_FILTER_CUBIC)
 #undef DXB_X
-    return false;
 }
+
+// one level: hj = its records, jobs = their device copy (nullptr for a single item).  Returns the launched kernel's name.
+static const char* launch_level(cudaStream_t stream, const dxb_mip_job* jobs, const dxb_mip_job* hj, const dxb_mip_params& P, bool special, bool srgb,
+                                unsigned gridCap)
+{
+    const dxb_mip_job& j0 = hj[0];
+    if (special && uniform_batch(hj, P.njobs))
+    {
+        const dim3 blk(32, 8, 1);
+        // CUBIC of a chain level (source <= 3 x destination per axis): separable shared-memory kernel
+        // (LINEAR at 2:1 has no tap shared between neighbouring outputs: the plain tile kernel is faster there, 0.24 vs 0.43 ms per 64 x 1024^2 chain)
+        bool pixAligned = true;                     // k_mip_sep fetches whole pixels with one vector load each
+        for (uint32_t i = 0; i < P.njobs; ++i) pixAligned = pixAligned && vec_aligned(hj[i].src, hj[i].srcPitch, dxb_bytes_per_pixel(P.format));
+        const dim3 gs((j0.dw + DXB_SEP_TW - 1) / DXB_SEP_TW, (j0.dh + DXB_SEP_TH - 1) / DXB_SEP_TH, P.njobs);
+        if (P.mode == DXB_FILTER_CUBIC && pixAligned && j0.sw <= 3u * j0.dw && j0.sh <= 3u * j0.dh && gs.y <= 65535u)
+        {
+#define DXB_X(FMT, MODE) if (P.format == FMT) { \
+                if (srgb) k_mip_sep<FMT, true><<<gs, blk, 0, stream>>>(jobs, j0, P); else k_mip_sep<FMT, false><<<gs, blk, 0, stream>>>(jobs, j0, P); \
+                return "k_mip_sep"; }
+            DXB_MIP_FORMATS(DXB_X, 0)
+#undef DXB_X
+        }
+        const uint32_t rowsPerCta = (P.mode == DXB_FILTER_CUBIC) ? 8u * DXB_CUBIC_KY : 8u;
+        const dim3 g((j0.dw + 31) / 32, (j0.dh + rowsPerCta - 1) / rowsPerCta, P.njobs);
+        if (g.y <= 65535u)
+        {
+#define DXB_X(FMT, MODE) if (P.format == FMT && P.mode == MODE) { \
+                if (srgb) k_mip_tile<FMT, MODE, true><<<g, blk, 0, stream>>>(jobs, j0, P); else k_mip_tile<FMT, MODE, false><<<g, blk, 0, stream>>>(jobs, j0, P); \
+                return "k_mip_tile"; }
+            DXB_MIP_FORMATS(DXB_X, DXB_FILTER_BOX)
+            DXB_MIP_FORMATS(DXB_X, DXB_FILTER_LINEAR)
+            DXB_MIP_FORMATS(DXB_X, DXB_FILTER_CUBIC)
+#undef DXB_X
+        }
+    }
+    const uint32_t need = (uint32_t)(((uint64_t)P.totalUnits + 255) / 256);
+    k_mip_level<<<need < 1u ? 1u : (need < gridCap ? need : gridCap), 256, 0, stream>>>(jobs, j0, P);
+    return "k_mip_level";
+}
+
+int32_t dxb_launch_mip_chain(cudaStream_t stream, const dxb_mip_job* jobs, const dxb_mip_job* hostJobs, uint32_t items, uint32_t levels,
+                             dxb_mip_params P, const dxb_tri_axis* tri, unsigned gridCap, int32_t (*launched)(const char* kernel))
+{
+    // The specialised kernels take BOX / LINEAR / CUBIC on the hot formats with both sRGB steps or none (the only combinations
+    // a chain produces); anything else runs the generic k_mip_level.
+    const bool srgb = (P.lflags == (DXB_FILTER_SRGB_IN | DXB_FILTER_SRGB_OUT));
+    bool special = false;
+#define DXB_X(FMT, MODE) special = special || P.format == FMT;
+    DXB_MIP_FORMATS(DXB_X, 0)
+#undef DXB_X
+    special = special && (srgb || P.lflags == 0) && (P.mode == DXB_FILTER_BOX || P.mode == DXB_FILTER_LINEAR || P.mode == DXB_FILTER_CUBIC);
+    // first level whose SOURCE is at most 64x64: from there on one CTA per item finishes the chain in one launch
+    uint32_t tailStart = levels;
+    for (uint32_t l = 1; l < levels; ++l)
+        if (hostJobs[(size_t)(l - 1) * items].sw <= 64 && hostJobs[(size_t)(l - 1) * items].sh <= 64) { tailStart = l; break; }
+    const bool tail = special && levels - tailStart >= 2 && items <= 0x7FFFFFFFu;
+    const bool fused = special && P.mode != DXB_FILTER_CUBIC && levels >= 4;       // LINEAR at 2:1 reads the same 2x2 patches as BOX
+    P.njobs = items;
+    for (uint32_t l = 1; l < levels;)
+    {
+        const size_t at = (size_t)(l - 1) * items;
+        const dxb_mip_job* hj = hostJobs + at;
+        int32_t hr;
+        // three levels per launch while the source is larger than the tail kernel's 64x64 and divides by 8
+        if (fused && l + 2 < levels && (hj[0].sw > 64 || hj[0].sh > 64) && launch_box3(stream, jobs + at, hj, items, P, srgb))
+        {
+            hr = launched("k_mip_box3");
+            l += 3;
+        }
+        else if (tail && l >= tailStart)
+        {
+            launch_tail(stream, jobs + at, items, levels - l, P, srgb);
+            return launched("k_mip_tail");
+        }
+        else
+        {
+            const dxb_mip_job& last = hj[items - 1];
+            P.totalUnits = last.firstUnit + last.dw * last.dh;
+            if (tri) { P.triX = tri[2 * (l - 1)]; P.triY = tri[2 * (l - 1) + 1]; }
+            hr = launched(launch_level(stream, items > 1 ? jobs + at : nullptr, hj, P, special, srgb, gridCap));
+            l += 1;
+        }
+        if (hr != DXB_S_OK) return hr;
+    }
+    return DXB_S_OK;
+}
+

@@ -62,14 +62,17 @@ void dxb_bc7_set_feed(int mode);
 void dxb_launch_decompress(unsigned grid, cudaStream_t stream, const dxb_job* jobs, const dxb_job* hostJobs, const dxb_compress_params& P);
 void dxb_launch_bc6h(unsigned grid, cudaStream_t stream, const dxb_job* jobs, const dxb_job* hostJobs, const dxb_compress_params& P);
 void dxb_launch_convert(unsigned grid, cudaStream_t stream, const dxb_job* jobs, const dxb_job* hostJobs, const dxb_convert_params& P);
-void dxb_launch_mip(unsigned grid, cudaStream_t stream, const dxb_mip_job* jobs, const dxb_mip_job* hostJobs, const dxb_mip_params& P);
-// tail of a chain: levels [first, first+count) of all items in one launch (jobsDev laid out [level][item]); false = no such kernel
+// Levels 1 .. levels-1 of `items` chains whose items all have the same sizes (a resize is a chain of two levels), each level
+// from the stored previous one.  hostJobs: the (levels - 1) x items records laid out [level - 1][item]; jobs: their device
+// copy, nullptr only when there is a single record.  P: format, mode, filter and lflags.  tri: TRIANGLE's device gather
+// lists, X and Y of each level (nullptr for other filters).  gridCap: most CTAs of the generic kernel.  launched(kernel)
+// follows every launch; a result other than S_OK stops the chain and is returned.
+int32_t dxb_launch_mip_chain(cudaStream_t stream, const dxb_mip_job* jobs, const dxb_mip_job* hostJobs, uint32_t items, uint32_t levels,
+                             dxb_mip_params P, const dxb_tri_axis* tri, unsigned gridCap, int32_t (*launched)(const char* kernel));
 void dxb_launch_convert_diffuse(cudaStream_t stream, const dxb_job* jobs, const dxb_job* hostJobs, const dxb_convert_params& P, void* errors, uint32_t errStride);
 void dxb_launch_alpha_coverage(unsigned grid, cudaStream_t stream, const dxb_job& j, uint32_t fmt, float scale, float ref, unsigned long long* count);
 void dxb_launch_scale_alpha(unsigned grid, cudaStream_t stream, const dxb_job& j, uint32_t fmt, float scale);
 void dxb_launch_pmalpha(unsigned grid, cudaStream_t stream, const dxb_job* jobs, const dxb_job* hostJobs, const dxb_convert_params& P);
-bool dxb_launch_mip_box3(cudaStream_t stream, const dxb_mip_job* jobsDev, const dxb_mip_job* hostJobs, uint32_t items, const dxb_mip_params& P);
-bool dxb_launch_mip_tail(cudaStream_t stream, const dxb_mip_job* jobsDev, uint32_t items, uint32_t count, const dxb_mip_params& P);
 // resident CTAs per SM of each kernel at its block size
 int dxb_occupancy_bc15();
 int dxb_occupancy_bc7();

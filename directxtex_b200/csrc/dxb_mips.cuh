@@ -189,6 +189,26 @@ DXB_DEV dxb_px dxb_mip_triangle(uint32_t fmt, const dxb_mip_job& j, uint32_t x, 
     return acc;
 }
 
+// ---- one destination pixel of a level in filter `mode`: POINT copies with plain Load / Store, the other filters work in
+// linear space and store through StoreScanlineLinear.  Inlined, so a kernel with a compile-time format and mode keeps only
+// its own filter.  ax / ay: TRIANGLE's gather lists.
+DXB_DEV void dxb_mip_pixel(uint32_t fmt, uint32_t mode, const dxb_mip_job& j, uint32_t x, uint32_t y, uint32_t filter, uint32_t lflags,
+                           const dxb_tri_axis& ax, const dxb_tri_axis& ay)
+{
+    dxb_px v;
+    switch (mode)
+    {
+    case DXB_FILTER_POINT:
+        dxb_store_pixel(fmt, j.dst + (size_t)y * j.dstPitch, x, dxb_mip_point(fmt, j, x, y));
+        return;
+    case DXB_FILTER_BOX: v = dxb_mip_box(fmt, j, x, y, lflags); break;
+    case DXB_FILTER_LINEAR: v = dxb_mip_linear(fmt, j, x, y, filter, lflags); break;
+    case DXB_FILTER_CUBIC: v = dxb_mip_cubic(fmt, j, x, y, filter, lflags); break;
+    default: v = dxb_mip_triangle(fmt, j, x, y, lflags, ax, ay); break;
+    }
+    dxb_store_linear(fmt, j.dst, j.dstPitch, x, y, v, lflags);
+}
+
 // ---------------------------------------------------------------------------------------------
 // ScaleMipMapsAlphaForCoverage helpers (DirectXTexMipmaps.cpp:143-356).
 // Coverage of one 2x2 cell (CalculateAlphaCoverage :213-308): the four alphas, scaled and saturated, go through the 8x8

@@ -130,7 +130,7 @@ int32_t emul_convert(const uint8_t* src, size_t w, size_t h, uint32_t srcFmt, si
 
 } // extern "C"
 
-// ---- mip chain emulation: same per-pixel functions as k_mip_level ---------------------------------
+// ---- mip chain emulation: dxb_mip_pixel, the same function k_mip_level and k_mip_tail run per pixel --------------------
 #include "dxb_mips.cuh"
 #include "dxb_host_tri.h"
 
@@ -167,22 +167,7 @@ extern "C" int32_t emul_generate_mipmaps(uint8_t* chainBase, const size_t* offse
             ay.off = ty.off.data(); ay.src = ty.src.data(); ay.w = ty.w.data();
         }
         for (uint32_t y = 0; y < j.dh; ++y)
-            for (uint32_t x = 0; x < j.dw; ++x)
-            {
-                dxb_px v;
-                switch (mode)
-                {
-                case DXB_FILTER_POINT:
-                    v = dxb_mip_point(fmt, j, x, y);
-                    dxb_store_pixel(fmt, j.dst + (size_t)y * j.dstPitch, x, v);
-                    continue;
-                case DXB_FILTER_BOX: v = dxb_mip_box(fmt, j, x, y, lflags); break;
-                case DXB_FILTER_LINEAR: v = dxb_mip_linear(fmt, j, x, y, filter, lflags); break;
-                case DXB_FILTER_CUBIC: v = dxb_mip_cubic(fmt, j, x, y, filter, lflags); break;
-                default: v = dxb_mip_triangle(fmt, j, x, y, lflags, ax, ay); break;
-                }
-                dxb_store_linear(fmt, j.dst, j.dstPitch, x, y, v, lflags);
-            }
+            for (uint32_t x = 0; x < j.dw; ++x) dxb_mip_pixel(fmt, mode, j, x, y, filter, lflags, ax, ay);
     }
     return DXB_S_OK;
 }

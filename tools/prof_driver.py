@@ -21,6 +21,20 @@ def dev(a):
     return torch.from_numpy(np.ascontiguousarray(a).reshape(-1).view(np.uint8)).cuda()
 
 
+def mip_chains(fmt, w, h, items, base, levels=0):
+    """`items` chains of `levels` levels (0 = full) in one device buffer, level 0 of each a copy of the device bytes `base`;
+    the item stride is padded to 256 bytes so that every item is vector-aligned (as the host-staged path does)"""
+    layout, total = F.mip_chain_layout(fmt, w, h, levels)
+    total = (total + 255) & ~255
+    chain = torch.zeros(total * items, dtype=torch.uint8, device="cuda")
+    imgs = []
+    for it in range(items):
+        chain[it * total: it * total + base.numel()] = base
+        for (off, lw, lh, row, sl) in layout:
+            imgs.append(capi.Image(lw, lh, fmt, row, sl, chain.data_ptr() + it * total + off))
+    return chain, capi.images(imgs), len(layout)
+
+
 def timed(name, fn, units):
     for _ in range(2):
         fn()
@@ -99,20 +113,22 @@ if what in ("rows", "all", "rowscubic", "rowslinear"):
     timed("convert r32f->r8 8192^2", lambda: capi.lib.dxb200_convert_device(f, 1, 61, 0, 0.5, b, st), w * h)
     # C4-like: 64 x (1024^2 RGBA8) box mip chains
     items, w, h = 64, 1024, 1024
-    layout, total = F.mip_chain_layout(28, w, h)
-    total = (total + 255) & ~255          # item stride padded so that every item is vector-aligned (as the host-staged path does)
-    chain = torch.zeros(total * items, dtype=torch.uint8, device="cuda")
-    base = dev(synth.c1_rgba8(w, h))
-    imgs = []
-    for it in range(items):
-        chain[it * total: it * total + w * h * 4] = base
-        for (off, lw, lh, row, sl) in layout:
-            imgs.append(capi.Image(lw, lh, 28, row, sl, chain.data_ptr() + it * total + off))
-    arr = capi.images(imgs)
+    chain, arr, nl = mip_chains(28, w, h, items, dev(synth.c1_rgba8(w, h)))
     for fl, nm in ((F.TEX_FILTER_BOX, "box"), (F.TEX_FILTER_CUBIC, "cubic"), (F.TEX_FILTER_LINEAR, "linear")):
         if what.startswith("rows") and what != "rows" and what != "rows" + nm:
             continue
-        timed("mips %s 64x1024^2 rgba8" % nm, lambda: capi.lib.dxb200_generate_mipmaps_device(arr, items, len(layout), fl, st), items * w * h * 4 // 3)
+        timed("mips %s 64x1024^2 rgba8" % nm, lambda: capi.lib.dxb200_generate_mipmaps_device(arr, items, nl, fl, st), items * w * h * 4 // 3)
+    if what in ("rows", "all"):
+        del chain
+        # k_mip_tile: BOX on its vector path takes both levels of a 3-level chain (the fused kernel needs 4 levels and the
+        # tail kernel a source of at most 64x64) ...
+        chain, arr, nl = mip_chains(28, w, h, items, dev(synth.c1_rgba8(w, h)), levels=3)
+        timed("mips box 3 levels 64x1024^2", lambda: capi.lib.dxb200_generate_mipmaps_device(arr, items, nl, F.TEX_FILTER_BOX, st), items * w * h * 5 // 16)
+        del chain
+        # ... and LINEAR at sizes that are not multiples of 8 (no fused kernel) runs every level above 64x64
+        w, h = 1023, 767
+        chain, arr, nl = mip_chains(28, w, h, items, dev(synth.c1_rgba8(w, h)))
+        timed("mips linear 64x1023x767 rgba8", lambda: capi.lib.dxb200_generate_mipmaps_device(arr, items, nl, F.TEX_FILTER_LINEAR, st), items * w * h * 4 // 3)
     del chain
 
 if what in ("rowshalf", "all"):
@@ -126,14 +142,5 @@ if what in ("rowshalf", "all"):
         timed("convert %d->rgba16f 4096^2" % sf, lambda: capi.lib.dxb200_convert_device(s, 1, 10, 0, 0.5, hh, st), w * h)
         del d_in
     items, w, h = 16, 1024, 1024
-    layout, total = F.mip_chain_layout(10, w, h)
-    total = (total + 255) & ~255
-    chain = torch.zeros(total * items, dtype=torch.uint8, device="cuda")
-    base = dev(synth.c3_rgba16f(w, h))
-    imgs = []
-    for it in range(items):
-        chain[it * total: it * total + w * h * 8] = base
-        for (off, lw, lh, row, sl) in layout:
-            imgs.append(capi.Image(lw, lh, 10, row, sl, chain.data_ptr() + it * total + off))
-    arr = capi.images(imgs)
-    timed("mips box 16x1024^2 rgba16f", lambda: capi.lib.dxb200_generate_mipmaps_device(arr, items, len(layout), F.TEX_FILTER_BOX, st), items * w * h * 4 // 3)
+    chain, arr, nl = mip_chains(10, w, h, items, dev(synth.c3_rgba16f(w, h)))
+    timed("mips box 16x1024^2 rgba16f", lambda: capi.lib.dxb200_generate_mipmaps_device(arr, items, nl, F.TEX_FILTER_BOX, st), items * w * h * 4 // 3)
