@@ -41,9 +41,9 @@ __global__ void __launch_bounds__(DXB_BC7_WARPS * 32, DXB_BC7_MINB) k_compress_b
             out = j.dst + (size_t)by * j.dstPitch + (size_t)bx * 16u;
         }
         S->px[lane] = ldr;
+        if (hl == 0) S->out[lane >> 4] = out;
         __syncwarp();
-        // the encoder takes one output pointer per half; every lane passes its own half's pointer in both slots
-        dxb_bc7_encode_pair<THREE>(S, P.bcflags, out, out);
+        dxb_bc7_encode_pair<THREE>(S, P.bcflags);
         __syncwarp();
     }
 }
@@ -80,7 +80,7 @@ int dxb_occupancy_bc7()
 //   * one `cp.async.bulk.tensor.3d` per tile, issued by thread 0, completion on an mbarrier (complete_tx::bytes); every lane then
 //     takes its pixel from the tile with one 128-bit shared load and converts it exactly like the direct kernel does;
 //   * the 4 KB landing buffer is free again as soon as every warp has taken its pixels (the barrier at the top of the iteration), so
-//     the next tile is requested right there and has the whole encode of the current tile to arrive; with it the CTA needs 75.9 KB of
+//     the next tile is requested right there and has the whole encode of the current tile to arrive; with it the CTA needs 76.0 KB of
 //     shared memory, which still leaves 3 CTAs per SM resident within the 228 KB of an H100 SM;
 //   * tiles are handed out by an atomic counter (blocks with alpha cost more than opaque ones); the counter is read one tile ahead
 //     of the request, so its round trip is off the critical path too.  T.counter == nullptr: statically strided tiles.
@@ -117,7 +117,10 @@ struct dxb_bc7_tma_params
 
 __device__ __forceinline__ uint32_t dxb_smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
 
-template <bool THREE>
+// PLAIN: no sRGB conversion flag (the default, and every BC7_UNORM call without TEX_FILTER_SRGB_*).  ConvertScanline from
+// RGBA32F to BC7_UNORM is then a clamp to [0, 1]: with both formats' conversion flags as compile-time constants dxb_convert_pixel
+// folds to it.  The other flag sets keep the run-time branches.
+template <bool THREE, bool PLAIN>
 __global__ void __launch_bounds__(DXB_BC7_WARPS * 32, DXB_BC7_MINB) k_compress_bc7_tma(const __grid_constant__ CUtensorMap tmap, dxb_bc7_tma_params T, dxb_compress_params P)
 {
     static_assert(DXB_BC7_WARPS == 8, "a tile is 16 blocks = 8 warps x 2");
@@ -175,11 +178,14 @@ __global__ void __launch_bounds__(DXB_BC7_WARPS * 32, DXB_BC7_MINB) k_compress_b
         if (bx < T.nbx)
         {
             const float4 f = tileBuf[(hl >> 2) * 64u + blk * 4u + (hl & 3u)];
-            dxb_px v = dxb_convert_pixel(dxb_make_px(f.x, f.y, f.z, f.w), P.inF, P.outF, P.cflags);
+            const dxb_px v = PLAIN ? dxb_convert_pixel(dxb_make_px(f.x, f.y, f.z, f.w), dxb_convert_flags(DXB_FMT_R32G32B32A32_FLOAT),
+                                                       dxb_convert_flags(DXB_FMT_BC7_UNORM), 0u)
+                                   : dxb_convert_pixel(dxb_make_px(f.x, f.y, f.z, f.w), P.inF, P.outF, P.cflags);
             ldr = dxb_make_px(dxb_bc7_ldr(v.x), dxb_bc7_ldr(v.y), dxb_bc7_ldr(v.z), dxb_bc7_ldr(v.w));
             out = T.dst0 + (size_t)img * T.dstImageStride + (size_t)by * T.dstPitch + (size_t)bx * 16u;
         }
         S->px[lane] = ldr;
+        if (hl == 0) S->out[lane >> 4] = out;
         __syncthreads();                // every warp has taken its pixels (and the tile index): the landing buffer is free
         if (threadIdx.x == 0)
         {
@@ -188,7 +194,7 @@ __global__ void __launch_bounds__(DXB_BC7_WARPS * 32, DXB_BC7_MINB) k_compress_b
             // hand-out for the iteration after the next; its value is not needed before the next request, so the round trip hides
             ahead = (nxt >= T.totalTiles) ? nxt : (T.counter ? gridDim.x + atomicAdd(T.counter, 1u) : nxt + gridDim.x);
         }
-        dxb_bc7_encode_pair<THREE>(S, P.bcflags, out, out);
+        dxb_bc7_encode_pair<THREE>(S, P.bcflags);
         __syncwarp();
     }
 }
@@ -212,8 +218,10 @@ static dxb_encode_tiled_fn encode_tiled()
 static const size_t kBC7TmaSmem = DXB_BC7_TILE_BYTES + 128u + sizeof(dxb_bc7_scratch) * DXB_BC7_WARPS;
 static bool bc7_tma_attr_set()
 {
-    static const bool ok = (cudaFuncSetAttribute(k_compress_bc7_tma<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kBC7TmaSmem) == cudaSuccess) &&
-                           (cudaFuncSetAttribute(k_compress_bc7_tma<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kBC7TmaSmem) == cudaSuccess);
+    static const bool ok = (cudaFuncSetAttribute(k_compress_bc7_tma<false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kBC7TmaSmem) == cudaSuccess) &&
+                           (cudaFuncSetAttribute(k_compress_bc7_tma<false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kBC7TmaSmem) == cudaSuccess) &&
+                           (cudaFuncSetAttribute(k_compress_bc7_tma<true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kBC7TmaSmem) == cudaSuccess) &&
+                           (cudaFuncSetAttribute(k_compress_bc7_tma<true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kBC7TmaSmem) == cudaSuccess);
     return ok;
 }
 
@@ -277,8 +285,14 @@ bool dxb_launch_bc7_tma(unsigned residentCtas, cudaStream_t stream, const dxb_jo
         if (cudaMallocAsync((void**)&T.counter, sizeof(uint32_t), stream) != cudaSuccess) { (void)cudaGetLastError(); return false; }
         cudaMemsetAsync(T.counter, 0, sizeof(uint32_t), stream);
     }
-    if (P.bcflags & DXB_BC_FLAGS_USE_3SUBSETS) k_compress_bc7_tma<true><<<grid, DXB_BC7_WARPS * 32, kBC7TmaSmem, stream>>>(tmap, T, P);
-    else k_compress_bc7_tma<false><<<grid, DXB_BC7_WARPS * 32, kBC7TmaSmem, stream>>>(tmap, T, P);
+    // the source is RGBA32F and the destination BC7_UNORM(_SRGB), so P.inF / P.outF are the PLAIN kernel's constants; only the
+    // resolved sRGB flags can differ
+    const bool plain = (P.cflags == 0u);
+    const bool three = (P.bcflags & DXB_BC_FLAGS_USE_3SUBSETS) != 0u;
+    if (three) { if (plain) k_compress_bc7_tma<true, true><<<grid, DXB_BC7_WARPS * 32, kBC7TmaSmem, stream>>>(tmap, T, P);
+                 else k_compress_bc7_tma<true, false><<<grid, DXB_BC7_WARPS * 32, kBC7TmaSmem, stream>>>(tmap, T, P); }
+    else if (plain) k_compress_bc7_tma<false, true><<<grid, DXB_BC7_WARPS * 32, kBC7TmaSmem, stream>>>(tmap, T, P);
+    else k_compress_bc7_tma<false, false><<<grid, DXB_BC7_WARPS * 32, kBC7TmaSmem, stream>>>(tmap, T, P);
     if (T.counter) cudaFreeAsync(T.counter, stream);
     return true;
 }
