@@ -9,7 +9,7 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.environ.get("DXTEX_B200_LIB") or os.path.join(_HERE, "_lib", "libdxtex_b200.so")     # env override: kernel-variant experiments
 
 SYMBOLS = [
-    "dxb200_version", "dxb200_init", "dxb200_init_devices", "dxb200_initialized_devices", "dxb200_shutdown", "dxb200_device_count", "dxb200_launch_count", "dxb200_tma_launch_count", "dxb200_set_option", "dxb200_get_option", "dxb200_last_error",
+    "dxb200_version", "dxb200_init", "dxb200_init_devices", "dxb200_initialized_devices", "dxb200_shutdown", "dxb200_device_count", "dxb200_launch_count", "dxb200_tma_launch_count", "dxb200_kernel_launch_count", "dxb200_set_option", "dxb200_get_option", "dxb200_last_error",
     "dxb200_host_alloc", "dxb200_host_free", "dxb200_compute_pitch", "dxb200_calculate_mip_levels",
     "dxb200_compress", "dxb200_compress_ex", "dxb200_compress_device", "dxb200_convert_ex", "dxb200_mipmaps_compress", "dxb200_decompress", "dxb200_decompress_device",
     "dxb200_convert", "dxb200_convert_device", "dxb200_generate_mipmaps", "dxb200_generate_mipmaps_device",
@@ -53,6 +53,8 @@ def _load():
     lib.dxb200_last_error.restype = C.c_char_p
     lib.dxb200_launch_count.restype = C.c_uint64
     lib.dxb200_tma_launch_count.restype = C.c_uint64
+    lib.dxb200_kernel_launch_count.restype = C.c_uint64
+    lib.dxb200_kernel_launch_count.argtypes = [C.c_char_p]
     lib.dxb200_set_option.argtypes = [C.c_uint32, C.c_int32]
     lib.dxb200_get_option.argtypes = [C.c_uint32]
     lib.dxb200_host_alloc.restype = C.c_void_p
@@ -108,10 +110,16 @@ def launch_count():
 
 
 OPT_BC7_FEED = 1
+OPT_MIP_KERNELS = 2
 
 
 def tma_launch_count():
     return int(lib.dxb200_tma_launch_count())
+
+
+def kernel_launch_count(kernel):
+    """launches of the kernel family `kernel` (e.g. "k_mip_tile") so far in this process"""
+    return int(lib.dxb200_kernel_launch_count(kernel.encode()))
 
 
 def make_image(ptr, w, h, fmt, row_pitch=0):

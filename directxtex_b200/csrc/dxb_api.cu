@@ -20,6 +20,7 @@
 #include <unistd.h>
 #include <sys/syscall.h>
 #include <vector>
+#include <map>
 #include <string>
 #include <cstring>
 #include <cstdio>
@@ -43,6 +44,9 @@ constexpr size_t ITEM_CHUNK = size_t(80) << 20;
 
 std::mutex g_mu;                // guards the device table only; calls on different lanes / devices run concurrently
 std::atomic<uint64_t> g_launches{0}, g_tma_launches{0};
+std::mutex g_count_mu;                                  // guards g_kernel_launches
+std::map<std::string, uint64_t> g_kernel_launches;      // launches per kernel name (dxb200_kernel_launch_count)
+std::atomic<int32_t> g_mip_kernels{0};                  // DXB200_OPT_MIP_KERNELS
 thread_local std::string t_lastError;
 
 struct Lane
@@ -355,6 +359,10 @@ uint32_t grid_for(uint32_t units, uint32_t perCta, uint32_t cap)
 int32_t check_launch(const char* name)
 {
     g_launches.fetch_add(1, std::memory_order_relaxed);
+    {
+        std::lock_guard<std::mutex> lk(g_count_mu);
+        ++g_kernel_launches[name];
+    }
     return cuda_hr(cudaGetLastError(), name);
 }
 
@@ -759,7 +767,8 @@ int32_t launch_mips(const dxb200_image* chain, size_t items, size_t levels, uint
         DXB_CUDA(cudaMemcpyAsync(dev, host.data(), bytes, cudaMemcpyHostToDevice, stream));
     }
     const int32_t hr = dxb_launch_mip_chain(stream, reinterpret_cast<const dxb_mip_job*>(dev), all.data(), (uint32_t)items, (uint32_t)levels, P,
-                                            tri.empty() ? nullptr : axes.data(), (unsigned)t_v.dev->gridRow * 8u, check_launch);
+                                            tri.empty() ? nullptr : axes.data(), (unsigned)t_v.dev->gridRow * 8u, g_mip_kernels.load() == 1,
+                                            check_launch);
     if (dev) cudaFreeAsync(dev, stream);
     return hr;
 }
@@ -773,12 +782,25 @@ const char* dxb200_version(void) { return "dxtex_b200 0.1 (sm_90a)"; }
 const char* dxb200_last_error(void) { return t_lastError.c_str(); }
 uint64_t dxb200_launch_count(void) { return g_launches.load(); }
 uint64_t dxb200_tma_launch_count(void) { return g_tma_launches.load(); }
+uint64_t dxb200_kernel_launch_count(const char* kernel)
+{
+    if (!kernel) return 0;
+    std::lock_guard<std::mutex> lk(g_count_mu);
+    const auto it = g_kernel_launches.find(kernel);
+    return it == g_kernel_launches.end() ? 0 : it->second;
+}
 int32_t dxb200_set_option(uint32_t option, int32_t value)
 {
     if (option == DXB200_OPT_BC7_FEED) { dxb_bc7_set_feed(value); return DXB_S_OK; }
+    if (option == DXB200_OPT_MIP_KERNELS) { g_mip_kernels.store(value == 1 ? 1 : 0); return DXB_S_OK; }
     return DXB_E_INVALIDARG;
 }
-int32_t dxb200_get_option(uint32_t option) { return (option == DXB200_OPT_BC7_FEED) ? dxb_bc7_get_feed() : -1; }
+int32_t dxb200_get_option(uint32_t option)
+{
+    if (option == DXB200_OPT_BC7_FEED) return dxb_bc7_get_feed();
+    if (option == DXB200_OPT_MIP_KERNELS) return g_mip_kernels.load();
+    return -1;
+}
 
 int32_t dxb200_device_count(void)
 {

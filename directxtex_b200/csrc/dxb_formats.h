@@ -228,6 +228,8 @@ DXB_FMT_FN uint32_t dxb_resolve_srgb_linear(uint32_t flags, uint32_t fmt)
     case DXB_FMT_R32G32_FLOAT: case DXB_FMT_R10G10B10A2_UNORM: case DXB_FMT_R8G8B8A8_UNORM: case DXB_FMT_R16G16_FLOAT:
     case DXB_FMT_R16G16_UNORM: case DXB_FMT_R32_FLOAT: case DXB_FMT_R8G8_UNORM: case DXB_FMT_R16_FLOAT: case DXB_FMT_R16_UNORM:
     case DXB_FMT_R8_UNORM: case DXB_FMT_B8G8R8A8_UNORM: case DXB_FMT_B8G8R8X8_UNORM:
+    case DXB_FMT_R11G11B10_FLOAT: case DXB_FMT_R9G9B9E5_SHAREDEXP: case DXB_FMT_B5G6R5_UNORM: case DXB_FMT_B5G5R5A1_UNORM:
+    case DXB_FMT_B4G4R4A4_UNORM:
         return flags;
     default:
         return flags & ~(uint32_t)(DXB_FILTER_SRGB_IN | DXB_FILTER_SRGB_OUT);

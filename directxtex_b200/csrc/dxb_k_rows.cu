@@ -403,19 +403,28 @@ template <int N> __device__ __forceinline__ void dxb_copy_vec(uint8_t* dst, cons
 // Per destination pixel of a 2:1 level that is 4.4 pixel decodes, 2.1 horizontal and 1 vertical filter evaluations instead
 // of 10 / 2.5 / 1.  Source coordinates are kept UNBOUNDED inside the tile (consecutive slots of the row buffer / of H) and
 // bounded (clamp / wrap / mirror, filters.h:123-207) only when the pixel is fetched, so every addressing mode of
-// the reference takes the same path.  Requires source extent <= 3 x destination extent (every level of a mip chain).
+// the reference takes the same path.  Requires source extent <= 3 x destination extent (every level of a mip chain) and
+// every source and destination extent <= DXB_SEP_MAX_EXTENT.
 #define DXB_SEP_TW 32
 #define DXB_SEP_TH 16
 #define DXB_SEP_MAXC (DXB_SEP_TW * 3 + 4)
 #define DXB_SEP_MAXR (DXB_SEP_TH * 3 + 4)
+// Largest extent k_mip_sep takes.  Its fp32 coordinates srcB = (u + 0.5) * (source / dest) - 0.5 round three times, each within
+// 2^-24 of a value below the source extent, so below 2^22 srcB is within 0.75 of the exact value.  That keeps (a) the tap base
+// inside [0, source - 1], which dxb_cubic_entry clamps before it derives the fraction and dxb_sep_entry does not, and (b) the base
+// span of one tile within 3 (TW - 1) + 2 columns (3 (TH - 1) + 2 rows), so it fits rowbuf / H.  Both fail at larger extents:
+// a same-size CUBIC of 12 582 912 pixels rounds the last base to the width; 537 157 722 -> 179 052 574 needs 132 columns in a
+// tile.  tests/test_cpu_mip_routes.py runs the same statements at this bound.
+#define DXB_SEP_MAX_EXTENT (1u << 22)
 
-// unbounded tap base and fraction of destination coordinate u: taps base - 1 .. base + 2
+// unbounded tap base and fraction of destination coordinate u: taps base - 1 .. base + 2.  dxb_cubic_entry bounds the base tap
+// before it derives the fraction; this does not: the two agree because the base stays inside [0, source - 1] up to DXB_SEP_MAX_EXTENT.
 __device__ __forceinline__ void dxb_sep_entry(uint32_t source, uint32_t dest, uint32_t u, int32_t* base, float* w)
 {
     const float scale = (float)source / (float)dest;
     const float t = ((float)u + 0.5f) * scale;
     const float srcB = t - 0.5f;
-    const int64_t isrcB = (int64_t)srcB;              // always inside [0, source - 1]: dxb_cubic_entry's bounduvw is the identity on it
+    const int64_t isrcB = (int64_t)srcB;
     *w = srcB - (float)isrcB; *base = (int32_t)isrcB;
 }
 __device__ __forceinline__ uint32_t dxb_sep_bound(int32_t i, uint32_t source, bool wrap, bool mirror)
@@ -526,7 +535,8 @@ __global__ void __launch_bounds__(256) k_mip_tail(const dxb_mip_job* __restrict_
 // (5.6 instead of 7.0 bytes moved per source texel-chain, one launch instead of three).
 // jobs: [level][item] records of the three levels; requires source width/height multiples of 8 and vector alignment.
 // LIN: the LINEAR filter at an exact 2:1 ratio.  CreateLinearFilter (filters.h:64-104) gives destination u the taps 2u and 2u + 1 with
-// weights 0.5 / 0.5 (srcB = 2u + 1.5, no edge clamp, WRAP irrelevant), so a destination pixel reads the same 2x2 patch as BOX and only the
+// weights 0.5 / 0.5 (srcB = 2u + 1.5, no edge clamp, WRAP irrelevant) while the source extent is at most 2^23: above it the fp32
+// srcB loses its .5 (width 8388616: u = 4194304 gives 8388610, one tap at weight 1) and launch_box3 declines LIN.  So a destination pixel reads the same 2x2 patch as BOX and only the
 // arithmetic differs: ((a0 w + a1 w) w) + ((b0 w + b1 w) w) in the reference's operation order (dxb_mip_linear, DirectXTexMipmaps.cpp:1087-1197).
 template <uint32_t FMT, bool LIN>
 __device__ __forceinline__ dxb_px dxb_box4(const uint8_t* r0, const uint8_t* r1, int k, uint32_t lflags)
@@ -611,10 +621,11 @@ static bool launch_box3(cudaStream_t stream, const dxb_mip_job* jobs, const dxb_
         if (!vec_aligned(a.src, a.srcPitch, 8 * B) || !vec_aligned(a.dst, a.dstPitch, 4 * B) || !vec_aligned(b.dst, b.dstPitch, 2 * B) ||
             !vec_aligned(c.dst, c.dstPitch, B)) return false;
     }
+    const bool lin = (P.mode == DXB_FILTER_LINEAR);
+    if (lin && (a0.sw > (1u << 23) || a0.sh > (1u << 23))) return false;        // CreateLinearFilter is 2u, 2u + 1 at 0.5 only up to 2^23
     const dim3 blk(32, 8, 1);
     const dim3 g((a0.sw / 8 + 31) / 32, (a0.sh / 8 + 7) / 8, items);
     if (g.y > 65535u) return false;
-    const bool lin = (P.mode == DXB_FILTER_LINEAR);
 #define DXB_X(FMT, MODE) if (P.format == FMT) { \
         if (lin) { if (srgb) k_mip_box3<FMT, true, true><<<g, blk, 0, stream>>>(jobs, items, P); else k_mip_box3<FMT, false, true><<<g, blk, 0, stream>>>(jobs, items, P); } \
         else { if (srgb) k_mip_box3<FMT, true, false><<<g, blk, 0, stream>>>(jobs, items, P); else k_mip_box3<FMT, false, false><<<g, blk, 0, stream>>>(jobs, items, P); } \
@@ -649,7 +660,8 @@ static const char* launch_level(cudaStream_t stream, const dxb_mip_job* jobs, co
         bool pixAligned = true;                     // k_mip_sep fetches whole pixels with one vector load each
         for (uint32_t i = 0; i < P.njobs; ++i) pixAligned = pixAligned && vec_aligned(hj[i].src, hj[i].srcPitch, dxb_bytes_per_pixel(P.format));
         const dim3 gs((j0.dw + DXB_SEP_TW - 1) / DXB_SEP_TW, (j0.dh + DXB_SEP_TH - 1) / DXB_SEP_TH, P.njobs);
-        if (P.mode == DXB_FILTER_CUBIC && pixAligned && j0.sw <= 3u * j0.dw && j0.sh <= 3u * j0.dh && gs.y <= 65535u)
+        const bool sepExtent = j0.sw <= DXB_SEP_MAX_EXTENT && j0.dw <= DXB_SEP_MAX_EXTENT && j0.sh <= DXB_SEP_MAX_EXTENT && j0.dh <= DXB_SEP_MAX_EXTENT;
+        if (P.mode == DXB_FILTER_CUBIC && pixAligned && sepExtent && j0.sw <= 3u * j0.dw && j0.sh <= 3u * j0.dh && gs.y <= 65535u)
         {
 #define DXB_X(FMT, MODE) if (P.format == FMT) { \
                 if (srgb) k_mip_sep<FMT, true><<<gs, blk, 0, stream>>>(jobs, j0, P); else k_mip_sep<FMT, false><<<gs, blk, 0, stream>>>(jobs, j0, P); \
@@ -676,7 +688,8 @@ static const char* launch_level(cudaStream_t stream, const dxb_mip_job* jobs, co
 }
 
 int32_t dxb_launch_mip_chain(cudaStream_t stream, const dxb_mip_job* jobs, const dxb_mip_job* hostJobs, uint32_t items, uint32_t levels,
-                             dxb_mip_params P, const dxb_tri_axis* tri, unsigned gridCap, int32_t (*launched)(const char* kernel))
+                             dxb_mip_params P, const dxb_tri_axis* tri, unsigned gridCap, bool genericOnly,
+                             int32_t (*launched)(const char* kernel))
 {
     // The specialised kernels take BOX / LINEAR / CUBIC on the hot formats with both sRGB steps or none (the only combinations
     // a chain produces); anything else runs the generic k_mip_level.
@@ -685,7 +698,8 @@ int32_t dxb_launch_mip_chain(cudaStream_t stream, const dxb_mip_job* jobs, const
 #define DXB_X(FMT, MODE) special = special || P.format == FMT;
     DXB_MIP_FORMATS(DXB_X, 0)
 #undef DXB_X
-    special = special && (srgb || P.lflags == 0) && (P.mode == DXB_FILTER_BOX || P.mode == DXB_FILTER_LINEAR || P.mode == DXB_FILTER_CUBIC);
+    special = special && !genericOnly && (srgb || P.lflags == 0) &&
+              (P.mode == DXB_FILTER_BOX || P.mode == DXB_FILTER_LINEAR || P.mode == DXB_FILTER_CUBIC);
     // first level whose SOURCE is at most 64x64: from there on one CTA per item finishes the chain in one launch
     uint32_t tailStart = levels;
     for (uint32_t l = 1; l < levels; ++l)

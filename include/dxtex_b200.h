@@ -62,12 +62,19 @@ DXB200_API void     dxb200_shutdown(void);                   /* release cached d
 DXB200_API int32_t  dxb200_device_count(void);
 DXB200_API uint64_t dxb200_launch_count(void);               /* number of kernels this library has launched so far */
 DXB200_API uint64_t dxb200_tma_launch_count(void);           /* ... of which fed by TMA tensor-map tile loads (k_compress_bc7_tma) */
+/* ... of which launched the kernel family `kernel` (e.g. "k_mip_box3", "k_mip_tail", "k_mip_sep", "k_mip_tile", "k_mip_level",
+ * "k_compress_bc7"); 0 for a name that never ran.  Lets a caller or a test see which route a call took. */
+DXB200_API uint64_t dxb200_kernel_launch_count(const char* kernel);
 /* process-wide tuning options (no reference counterpart; results never depend on them).
  *   DXB200_OPT_BC7_FEED  how k_compress_bc7 gets RGBA32F sources made of full blocks: 0 = direct vector loads, one CTA per 16 blocks,
  *                        1 = persistent CTAs fed by TMA tensor-map tile loads with an atomic tile counter, 2 = the same with statically
  *                        strided tiles, 3 = TMA with one CTA per tile, 4 = automatic (default): 1 for batches of images, 0 for a single
- *                        image -- whichever measured faster.  Initial value: environment variable DXB200_BC7_TMA. */
+ *                        image -- whichever measured faster.  Initial value: environment variable DXB200_BC7_TMA.
+ *   DXB200_OPT_MIP_KERNELS  which kernels GenerateMipMaps / Resize levels run on: 0 (default) = the specialised kernels where they apply
+ *                        (k_mip_box3, k_mip_tail, k_mip_sep, k_mip_tile), 1 = every level on the generic k_mip_level, so that the
+ *                        specialised routes can be checked against it; any other value means 0. */
 #define DXB200_OPT_BC7_FEED 1u
+#define DXB200_OPT_MIP_KERNELS 2u
 DXB200_API int32_t  dxb200_set_option(uint32_t option, int32_t value);      /* E_INVALIDARG for an unknown option */
 DXB200_API int32_t  dxb200_get_option(uint32_t option);                     /* -1 for an unknown option */
 DXB200_API const char* dxb200_last_error(void);              /* text of the last CUDA error seen by the calling thread's call */

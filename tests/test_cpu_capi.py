@@ -138,6 +138,19 @@ def test_options_round_trip_and_reject_unknown_ids():
         assert L.dxb200_set_option(capi.OPT_BC7_FEED, -5) == 0 and L.dxb200_get_option(capi.OPT_BC7_FEED) == 4
     finally:
         L.dxb200_set_option(capi.OPT_BC7_FEED, before)
+    # the mip kernel option: 0 (default) = specialised routes, 1 = the generic kernel only, anything else = 0
+    assert L.dxb200_get_option(capi.OPT_MIP_KERNELS) == 0
+    try:
+        for v, want in ((1, 1), (0, 0), (1, 1), (2, 0), (1, 1), (-1, 0), (99, 0)):
+            assert L.dxb200_set_option(capi.OPT_MIP_KERNELS, v) == 0 and L.dxb200_get_option(capi.OPT_MIP_KERNELS) == want, v
+    finally:
+        L.dxb200_set_option(capi.OPT_MIP_KERNELS, 0)
+    assert L.dxb200_get_option(capi.OPT_BC7_FEED) == before             # the two options are independent
     assert F.hr_u32(L.dxb200_set_option(12345, 1)) == 0x80070057
     assert L.dxb200_get_option(12345) == -1
     assert capi.tma_launch_count() >= 0
+    # per-kernel launch counts: a name that never ran (or no name) counts 0
+    assert capi.kernel_launch_count("k_no_such_kernel") == 0
+    assert capi.lib.dxb200_kernel_launch_count(None) == 0
+    if capi.lib.dxb200_device_count() == 0:
+        assert all(capi.kernel_launch_count(k) == 0 for k in ("k_mip_box3", "k_mip_tail", "k_mip_sep", "k_mip_tile", "k_mip_level"))

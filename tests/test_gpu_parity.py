@@ -216,6 +216,22 @@ def test_premultiply_alpha_vs_oracle(oracle, flags):
     assert e.value.hr == F.HRESULT_E_NOT_SUPPORTED
 
 
+@pytest.mark.parametrize("flags", [0x1000000, 0x2000000, 0x3000000, 0x3000002])
+def test_premultiply_alpha_srgb_flags_on_packed_formats(oracle, flags):
+    """LoadScanlineLinear / StoreScanlineLinear honour TEX_PMALPHA_SRGB_IN / _OUT on B5G5R5A1 and B4G4R4A4 too: every colour
+    field within one code of the reference (powf), alpha field identical"""
+    rng = np.random.default_rng(29)
+    for fmt, fields in ((86, ((10, 5), (5, 5), (0, 5), (15, 1))), (115, ((8, 4), (4, 4), (0, 4), (12, 4)))):
+        src = rng.integers(0, 1 << 16, 48 * 16, dtype=np.uint16)
+        hr, want = oracle.premultiply_alpha(src, 48, 16, fmt, flags)
+        got = capi.premultiply_alpha(src, 48, 16, fmt, flags)
+        assert hr == 0
+        g, w = got.view(np.uint16).astype(np.int32), want.view(np.uint16).astype(np.int32)
+        for k, (shift, bits) in enumerate(fields):
+            d = np.abs(((g >> shift) & ((1 << bits) - 1)) - ((w >> shift) & ((1 << bits) - 1))).max()
+            assert d <= (0 if k == 3 else 1), (fmt, hex(flags), k, d)
+
+
 def _alpha_test_image(fmt, w, h, rng):
     yy, xx = np.mgrid[0:h, 0:w]
     a = np.clip(0.5 + 0.4 * np.sin(xx * 0.4) * np.cos(yy * 0.3) + rng.normal(0, 0.12, (h, w)), 0, 1)
