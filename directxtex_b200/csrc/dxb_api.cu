@@ -395,7 +395,7 @@ int32_t plan_compress(const dxb200_image* src, size_t n, uint32_t dstFormat, uin
     P.bcflags = flags & (DXB_BC_FLAGS_DITHER_RGB | DXB_BC_FLAGS_DITHER_A | DXB_BC_FLAGS_UNIFORM |
                          DXB_BC_FLAGS_USE_3SUBSETS | DXB_BC_FLAGS_FORCE_BC7_MODE6);                 // GetBCFlags :26-35
     P.threshold = threshold;
-    plan->bc7 = (dstFormat == DXB_FMT_BC7_UNORM || dstFormat == DXB_FMT_BC7_UNORM_SRGB);
+    plan->bc7 = (dxb_make_linear(dstFormat) == DXB_FMT_BC7_UNORM);
     plan->bc6h = (dstFormat == DXB_FMT_BC6H_UF16 || dstFormat == DXB_FMT_BC6H_SF16);
     return DXB_S_OK;
 }

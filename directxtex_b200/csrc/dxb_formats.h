@@ -188,6 +188,24 @@ DXB_FMT_FN uint32_t dxb_bc_block_bytes(uint32_t fmt)
     }
 }
 
+// The UNORM twin of an sRGB format, every other format itself (MakeLinear, DirectXTexUtil.cpp:1446).  Kernels and launchers
+// select code on the twin: a format and its twin have the same load, store, dither store, BC block codec and conversion flags,
+// so an sRGB step can only come from the resolved flags (TEX_FILTER_SRGB_IN / _OUT) or an SRGB template argument.
+DXB_FMT_FN uint32_t dxb_make_linear(uint32_t fmt)
+{
+    switch (fmt)
+    {
+    case DXB_FMT_R8G8B8A8_UNORM_SRGB: return DXB_FMT_R8G8B8A8_UNORM;
+    case DXB_FMT_B8G8R8A8_UNORM_SRGB: return DXB_FMT_B8G8R8A8_UNORM;
+    case DXB_FMT_B8G8R8X8_UNORM_SRGB: return DXB_FMT_B8G8R8X8_UNORM;
+    case DXB_FMT_BC1_UNORM_SRGB:      return DXB_FMT_BC1_UNORM;
+    case DXB_FMT_BC2_UNORM_SRGB:      return DXB_FMT_BC2_UNORM;
+    case DXB_FMT_BC3_UNORM_SRGB:      return DXB_FMT_BC3_UNORM;
+    case DXB_FMT_BC7_UNORM_SRGB:      return DXB_FMT_BC7_UNORM;
+    default: return fmt;
+    }
+}
+
 DXB_FMT_FN int dxb_is_srgb_format(uint32_t fmt)
 {
     switch (fmt)

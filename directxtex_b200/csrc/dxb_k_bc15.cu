@@ -4,6 +4,7 @@
 //                              "no dithering" are compile-time constants.  The generic kernel carries every format
 //                              loader, the sRGB powf paths and all five encoders with their dither variants: 106 k SASS
 //                              instructions, and it ran at 13 % issue utilisation stalled on instruction fetch.
+//                              No pair names an sRGB format: an sRGB call matches its twins' pair (dxb_make_linear).
 #include <algorithm>
 #include "dxb_launch.h"
 #include "dxb_bc15.cuh"
@@ -72,14 +73,9 @@ __global__ void __launch_bounds__(dxb_bc15_threads(DF), dxb_bc15_minb(DF)) k_com
 
 void dxb_launch_bc15(unsigned grid, cudaStream_t stream, const dxb_job* jobs, const dxb_job* hostJobs, const dxb_compress_params& P)
 {
-    // the _SRGB variants share loader, conversion class and encoder with their UNORM twins; whether an sRGB <-> linear
-    // step is needed is already resolved into P.cflags, and the specialised kernels only take the default flag set
-    uint32_t df = P.dstFormat, sf = P.srcFormat;
-    if (df == DXB_FMT_BC1_UNORM_SRGB) df = DXB_FMT_BC1_UNORM;
-    if (df == DXB_FMT_BC2_UNORM_SRGB) df = DXB_FMT_BC2_UNORM;
-    if (df == DXB_FMT_BC3_UNORM_SRGB) df = DXB_FMT_BC3_UNORM;
-    if (sf == DXB_FMT_R8G8B8A8_UNORM_SRGB) sf = DXB_FMT_R8G8B8A8_UNORM;
-    if (sf == DXB_FMT_B8G8R8A8_UNORM_SRGB) sf = DXB_FMT_B8G8R8A8_UNORM;
+    // sRGB formats run their twins' kernels: an sRGB step is resolved into P.cflags, and the specialised kernels take only
+    // the default flag set
+    const uint32_t df = dxb_make_linear(P.dstFormat), sf = dxb_make_linear(P.srcFormat);
     if (P.bcflags == 0 && P.cflags == dxb_bc15_default_cflags(df))
     {
 #define DXB_X(DF, SF) if (df == DF && sf == SF) { k_compress_bc15_t<DF, SF><<<std::max(1u, grid * 128u / dxb_bc15_threads(DF)), dxb_bc15_threads(DF), 0, stream>>>(jobs, hostJobs[0], P); return; }

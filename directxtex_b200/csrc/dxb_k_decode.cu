@@ -2,7 +2,8 @@
 // decode (dxb_decode.cuh) -> ConvertScanline -> StoreScanline.
 //   k_decompress            generic: any BC source, any implemented target format
 //   k_decompress_t<SF,DF>   the default (source, target) pairs with no sRGB step: compile-time formats (one decoder, one
-//                           store path per kernel) and one vector store per block row
+//                           store path per kernel) and one vector store per block row.  No pair names an sRGB format:
+//                           an sRGB call matches its twins' pair (dxb_make_linear).
 #include "dxb_launch.h"
 #include "dxb_decode.cuh"
 
@@ -194,12 +195,8 @@ __global__ void __launch_bounds__(128) k_decompress_t(const dxb_job* __restrict_
 
 void dxb_launch_decompress(unsigned grid, cudaStream_t stream, const dxb_job* jobs, const dxb_job* hostJobs, const dxb_compress_params& P)
 {
-    uint32_t sf = P.srcFormat, df = P.dstFormat;
-    if (sf == DXB_FMT_BC1_UNORM_SRGB) sf = DXB_FMT_BC1_UNORM;
-    if (sf == DXB_FMT_BC2_UNORM_SRGB) sf = DXB_FMT_BC2_UNORM;
-    if (sf == DXB_FMT_BC3_UNORM_SRGB) sf = DXB_FMT_BC3_UNORM;
-    if (sf == DXB_FMT_BC7_UNORM_SRGB) sf = DXB_FMT_BC7_UNORM;
-    if (df == DXB_FMT_R8G8B8A8_UNORM_SRGB) df = DXB_FMT_R8G8B8A8_UNORM;
+    // sRGB formats run their twins' kernels; the specialised kernels take only calls without an sRGB step (P.cflags == 0)
+    const uint32_t sf = dxb_make_linear(P.srcFormat), df = dxb_make_linear(P.dstFormat);
 #ifndef DXB_DEC_GENERIC_ONLY
     if (P.cflags == 0)
     {

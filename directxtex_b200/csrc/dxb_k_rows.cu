@@ -9,6 +9,8 @@
 //   k_mip_box3<FMT,SRGB,LIN>  three BOX (or 2:1 LINEAR) levels per pass
 // dxb_launch_mip_chain picks the kernel of every level.  The arithmetic is the same inline code in all variants
 // (dxb_pixel.cuh / dxb_mips.cuh), so all of them are bit-exact against the oracle; only the memory access pattern differs.
+// The launchers route on the caller's format but instantiate every specialised kernel on dxb_make_linear(format): an sRGB
+// format runs its UNORM twin's kernel, with its sRGB steps taken from P.flags / P.lflags or the SRGB argument.
 #include "dxb_launch.h"
 #include "dxb_pixel.cuh"
 #include "dxb_mips.cuh"
@@ -145,6 +147,7 @@ __global__ void __launch_bounds__(256) k_convert_vec(const dxb_job* __restrict__
     }
 }
 
+// (29, 28) and (28, 29) both run k_convert_vec<28, 28>: the direction of their sRGB step is in P.flags
 #define DXB_CONVERT_PAIRS(X) \
     X(61, 41) X(41, 61) X(28, 2) X(2, 28) X(10, 2) X(2, 10) X(28, 10) X(10, 28) X(28, 87) X(87, 28) \
     X(61, 28) X(28, 61) X(11, 2) X(2, 11) X(41, 2) X(2, 41) X(29, 2) X(2, 29) X(29, 28) X(28, 29)
@@ -166,7 +169,8 @@ void dxb_launch_convert(unsigned grid, cudaStream_t stream, const dxb_job* jobs,
         const uint32_t ppt = 16u / (SB > DB ? SB : DB);
         const uint32_t chunksPerRow = (hostJobs[0].width + ppt - 1) / ppt;
         const dim3 g((chunksPerRow + 256u * DXB_CONV_UNR - 1) / (256u * DXB_CONV_UNR), hostJobs[0].height, P.njobs);
-#define DXB_X(SF, DF) if (P.srcFormat == SF && P.dstFormat == DF) { k_convert_vec<SF, DF><<<g, 256, 0, stream>>>(jobs, hostJobs[0], P); return; }
+#define DXB_X(SF, DF) if (P.srcFormat == SF && P.dstFormat == DF) { \
+            k_convert_vec<dxb_make_linear(SF), dxb_make_linear(DF)><<<g, 256, 0, stream>>>(jobs, hostJobs[0], P); return; }
         DXB_CONVERT_PAIRS(DXB_X)
 #undef DXB_X
     }
@@ -240,10 +244,10 @@ void dxb_launch_pmalpha(unsigned grid, cudaStream_t stream, const dxb_job* jobs,
         const uint32_t chunksPerRow = (hostJobs[0].width + ppt - 1) / ppt;
         const dim3 g((chunksPerRow + 255u) / 256u, hostJobs[0].height, P.njobs);
 #define DXB_X(FMT) if (P.srcFormat == FMT) { \
-            if (rev && srgb) k_pmalpha_vec<FMT, true, true><<<g, 256, 0, stream>>>(jobs, hostJobs[0], P); \
-            else if (rev) k_pmalpha_vec<FMT, true, false><<<g, 256, 0, stream>>>(jobs, hostJobs[0], P); \
-            else if (srgb) k_pmalpha_vec<FMT, false, true><<<g, 256, 0, stream>>>(jobs, hostJobs[0], P); \
-            else k_pmalpha_vec<FMT, false, false><<<g, 256, 0, stream>>>(jobs, hostJobs[0], P); \
+            if (rev && srgb) k_pmalpha_vec<dxb_make_linear(FMT), true, true><<<g, 256, 0, stream>>>(jobs, hostJobs[0], P); \
+            else if (rev) k_pmalpha_vec<dxb_make_linear(FMT), true, false><<<g, 256, 0, stream>>>(jobs, hostJobs[0], P); \
+            else if (srgb) k_pmalpha_vec<dxb_make_linear(FMT), false, true><<<g, 256, 0, stream>>>(jobs, hostJobs[0], P); \
+            else k_pmalpha_vec<dxb_make_linear(FMT), false, false><<<g, 256, 0, stream>>>(jobs, hostJobs[0], P); \
             return; }
         DXB_X(28) DXB_X(29) DXB_X(87) DXB_X(91) DXB_X(10) DXB_X(2)
 #undef DXB_X
@@ -627,8 +631,10 @@ static bool launch_box3(cudaStream_t stream, const dxb_mip_job* jobs, const dxb_
     const dim3 g((a0.sw / 8 + 31) / 32, (a0.sh / 8 + 7) / 8, items);
     if (g.y > 65535u) return false;
 #define DXB_X(FMT, MODE) if (P.format == FMT) { \
-        if (lin) { if (srgb) k_mip_box3<FMT, true, true><<<g, blk, 0, stream>>>(jobs, items, P); else k_mip_box3<FMT, false, true><<<g, blk, 0, stream>>>(jobs, items, P); } \
-        else { if (srgb) k_mip_box3<FMT, true, false><<<g, blk, 0, stream>>>(jobs, items, P); else k_mip_box3<FMT, false, false><<<g, blk, 0, stream>>>(jobs, items, P); } \
+        if (lin) { if (srgb) k_mip_box3<dxb_make_linear(FMT), true, true><<<g, blk, 0, stream>>>(jobs, items, P); \
+                   else k_mip_box3<dxb_make_linear(FMT), false, true><<<g, blk, 0, stream>>>(jobs, items, P); } \
+        else { if (srgb) k_mip_box3<dxb_make_linear(FMT), true, false><<<g, blk, 0, stream>>>(jobs, items, P); \
+               else k_mip_box3<dxb_make_linear(FMT), false, false><<<g, blk, 0, stream>>>(jobs, items, P); } \
         return true; }
     DXB_MIP_FORMATS(DXB_X, 0)
 #undef DXB_X
@@ -639,7 +645,8 @@ static bool launch_box3(cudaStream_t stream, const dxb_mip_job* jobs, const dxb_
 static void launch_tail(cudaStream_t stream, const dxb_mip_job* jobs, uint32_t items, uint32_t count, const dxb_mip_params& P, bool srgb)
 {
 #define DXB_X(FMT, MODE) if (P.format == FMT && P.mode == MODE) { \
-        if (srgb) k_mip_tail<FMT, MODE, true><<<items, 256, 0, stream>>>(jobs, items, count, P); else k_mip_tail<FMT, MODE, false><<<items, 256, 0, stream>>>(jobs, items, count, P); \
+        if (srgb) k_mip_tail<dxb_make_linear(FMT), MODE, true><<<items, 256, 0, stream>>>(jobs, items, count, P); \
+        else k_mip_tail<dxb_make_linear(FMT), MODE, false><<<items, 256, 0, stream>>>(jobs, items, count, P); \
         return; }
     DXB_MIP_FORMATS(DXB_X, DXB_FILTER_BOX)
     DXB_MIP_FORMATS(DXB_X, DXB_FILTER_LINEAR)
@@ -664,7 +671,8 @@ static const char* launch_level(cudaStream_t stream, const dxb_mip_job* jobs, co
         if (P.mode == DXB_FILTER_CUBIC && pixAligned && sepExtent && j0.sw <= 3u * j0.dw && j0.sh <= 3u * j0.dh && gs.y <= 65535u)
         {
 #define DXB_X(FMT, MODE) if (P.format == FMT) { \
-                if (srgb) k_mip_sep<FMT, true><<<gs, blk, 0, stream>>>(jobs, j0, P); else k_mip_sep<FMT, false><<<gs, blk, 0, stream>>>(jobs, j0, P); \
+                if (srgb) k_mip_sep<dxb_make_linear(FMT), true><<<gs, blk, 0, stream>>>(jobs, j0, P); \
+                else k_mip_sep<dxb_make_linear(FMT), false><<<gs, blk, 0, stream>>>(jobs, j0, P); \
                 return "k_mip_sep"; }
             DXB_MIP_FORMATS(DXB_X, 0)
 #undef DXB_X
@@ -674,7 +682,8 @@ static const char* launch_level(cudaStream_t stream, const dxb_mip_job* jobs, co
         if (g.y <= 65535u)
         {
 #define DXB_X(FMT, MODE) if (P.format == FMT && P.mode == MODE) { \
-                if (srgb) k_mip_tile<FMT, MODE, true><<<g, blk, 0, stream>>>(jobs, j0, P); else k_mip_tile<FMT, MODE, false><<<g, blk, 0, stream>>>(jobs, j0, P); \
+                if (srgb) k_mip_tile<dxb_make_linear(FMT), MODE, true><<<g, blk, 0, stream>>>(jobs, j0, P); \
+                else k_mip_tile<dxb_make_linear(FMT), MODE, false><<<g, blk, 0, stream>>>(jobs, j0, P); \
                 return "k_mip_tile"; }
             DXB_MIP_FORMATS(DXB_X, DXB_FILTER_BOX)
             DXB_MIP_FORMATS(DXB_X, DXB_FILTER_LINEAR)

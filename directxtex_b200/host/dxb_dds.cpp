@@ -116,16 +116,7 @@ int32_t dxb200_dds_encode_header(const dxb200_metadata* md, uint32_t flags, void
     {
         // DDS_FLAGS_FORCE_DX9_LEGACY writes the sRGB formats with their UNORM twins' legacy encodings and BC4U / BC5U as
         // ATI1 / ATI2 (:855-911); without a legacy encoding it fails with HRESULT_E_CANNOT_MAKE (:918-919)
-        uint32_t f = md->format;
-        if (flags & DF_FORCE_DX9)
-        {
-            if (f == DXB_FMT_R8G8B8A8_UNORM_SRGB) f = DXB_FMT_R8G8B8A8_UNORM;
-            else if (f == DXB_FMT_B8G8R8A8_UNORM_SRGB) f = DXB_FMT_B8G8R8A8_UNORM;
-            else if (f == DXB_FMT_B8G8R8X8_UNORM_SRGB) f = DXB_FMT_B8G8R8X8_UNORM;
-            else if (f == DXB_FMT_BC1_UNORM_SRGB) f = DXB_FMT_BC1_UNORM;
-            else if (f == DXB_FMT_BC2_UNORM_SRGB) f = DXB_FMT_BC2_UNORM;
-            else if (f == DXB_FMT_BC3_UNORM_SRGB) f = DXB_FMT_BC3_UNORM;
-        }
+        const uint32_t f = (flags & DF_FORCE_DX9) ? dxb_make_linear(md->format) : md->format;
         for (const Legacy& e : kLegacy)
             if (e.format == f && !e.decodeOnly && (!e.pm || is_pm(*md))) { leg = &e; break; }
         if (leg)

@@ -1,7 +1,8 @@
 """CPU suite for the mip / resize kernel routes (no GPU needed).
 
-- Every specialised mip kernel instantiation that dxb_k_rows.cu compiles (family x hot format x filter mode x sRGB x LIN) is
-  reached by a case of the GPU route table in tests/test_gpu_mip_routes.py, so a new instantiation cannot go untested.
+- Every specialised mip kernel instantiation that dxb_k_rows.cu compiles (family x UNORM twin of a hot format x filter mode x
+  sRGB x LIN) is reached by a case of the GPU route table in tests/test_gpu_mip_routes.py, so a new instantiation cannot go
+  untested and none is compiled that no call selects.
 - k_mip_sep's fp32 tap coordinates, run as the kernel runs them, stay inside the image and inside its shared-memory tile
   buffers up to the extent limit the launcher gives it.
 - The host emulator of the mip arithmetic (the inline code every mip kernel runs) against the oracle under TEX_FILTER_SRGB,
@@ -18,24 +19,21 @@ from tests import oracle_lib, test_gpu_mip_routes as R
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 MODES = {"DXB_FILTER_BOX": R.BOX, "DXB_FILTER_LINEAR": R.LIN, "DXB_FILTER_CUBIC": R.CUB, "0": 0}
-# k_mip_*<29, ..., false>: R8G8B8A8_UNORM_SRGB always resolves to both sRGB steps (LoadScanlineLinear forces them), so the
-# launcher never selects its SRGB = false variants.  They stay compiled because the launcher's format list is shared.
-UNREACHABLE = {("box3", 29, 0, False, False), ("box3", 29, 0, False, True), ("sep", 29, 0, False, False)} | \
-              {(fam, 29, m, False, False) for fam in ("tail", "tile") for m in (R.BOX, R.LIN, R.CUB)}
 
 
 def compiled_instantiations():
-    """(family, format, mode, sRGB, LIN) of every k_mip_box3 / k_mip_tail / k_mip_sep / k_mip_tile template the launcher
-    instantiates, read from the DXB_X dispatch blocks of dxb_k_rows.cu"""
+    """(routed formats, {(family, format, mode, sRGB, LIN)} of every k_mip_box3 / k_mip_tail / k_mip_sep / k_mip_tile template
+    the launcher instantiates), read from the DXB_X dispatch blocks of dxb_k_rows.cu; a template's format is the routed
+    format's UNORM twin where the launcher passes dxb_make_linear(FMT), the routed format itself where it passes FMT"""
     src = open(os.path.join(ROOT, "directxtex_b200", "csrc", "dxb_k_rows.cu")).read()
     fm = re.search(r"#define DXB_MIP_FORMATS\(X, MODE\)((?: X\(\d+, MODE\))+)", src)
     formats = [int(v) for v in re.findall(r"X\((\d+), MODE\)", fm.group(1))]
     out = set()
     for block in re.findall(r"#define DXB_X\(FMT, MODE\)(.*?)#undef DXB_X", src, re.S):
         modes = [MODES[m] for m in re.findall(r"DXB_MIP_FORMATS\(DXB_X, (\w+)\)", block)]
-        for fam, args in re.findall(r"k_mip_(box3|tail|sep|tile)<FMT((?:, \w+)*)>", block):
+        for fam, fmtarg, args in re.findall(r"k_mip_(box3|tail|sep|tile)<(FMT|dxb_make_linear\(FMT\))((?:, \w+)*)>", block):
             args = [a.strip() for a in args.split(",")[1:]]
-            for fmt in formats:
+            for fmt in ({R.TWIN.get(f, f) for f in formats} if fmtarg != "FMT" else formats):
                 for mode in modes:
                     if fam == "box3":                     # <FMT, SRGB, LIN>
                         out.add((fam, fmt, 0, args[0] == "true", args[1] == "true"))
@@ -47,14 +45,13 @@ def compiled_instantiations():
     return formats, out
 
 
-def test_route_table_reaches_every_instantiation():
+def test_route_table_reaches_every_twin_instantiation():
     formats, compiled = compiled_instantiations()
     assert tuple(formats) == R.HOT
-    assert len(compiled) == 126, len(compiled)                 # 7 formats x (box3 4 + tail 6 + sep 2 + tile 6)
+    assert len(compiled) == 108, len(compiled)                 # 6 twins x (box3 4 + tail 6 + sep 2 + tile 6)
     reached = set().union(*(R.instantiations(c) for c in R.CASES))
     assert reached <= compiled, sorted(reached - compiled)
-    assert UNREACHABLE <= compiled and not (UNREACHABLE & reached)
-    missing = compiled - reached - UNREACHABLE
+    missing = compiled - reached
     assert not missing, sorted(missing)
 
 

@@ -2,7 +2,8 @@
 
 dxb_launch_mip_chain (dxb_k_rows.cu) runs every level on one of five kernel families: k_mip_box3 (three BOX or 2:1 LINEAR
 levels per pass), k_mip_tail (the levels from 64x64 down, one CTA per item), k_mip_sep (separable CUBIC), k_mip_tile (2D tiles)
-or the generic k_mip_level.  The specialised families are compiled per hot format, filter and sRGB-ness.  CASES is one table:
+or the generic k_mip_level.  The specialised families are compiled per filter, sRGB-ness and UNORM twin of a hot format (an sRGB
+format runs its twin's kernels).  CASES is one table:
 each case names its format, size, item count, filter flags, memory layout and the families it must launch, and every case runs
 
   - with DXB200_OPT_MIP_KERNELS = 0 (the routing users get): the per-family launch counters must move for exactly those families;
@@ -32,18 +33,21 @@ HOT = (28, 29, 10, 2, 61, 41, 87)                   # DXB_MIP_FORMATS
 FAMILIES = ("k_mip_box3", "k_mip_tail", "k_mip_sep", "k_mip_tile", "k_mip_level")
 
 
-def _srgb_lists():
-    """(formats whose filters honour TEX_FILTER_SRGB_IN / _OUT, sRGB formats that always convert), read from dxb_resolve_srgb_linear
-    in dxb_formats.h: the lists the launcher resolves a call's sRGB steps with"""
+def _format_tables():
+    """(formats whose filters honour TEX_FILTER_SRGB_IN / _OUT, sRGB formats that always convert, {sRGB format: its UNORM twin}),
+    read from dxb_resolve_srgb_linear and dxb_make_linear in dxb_formats.h: the tables the launcher resolves a call's sRGB steps
+    and compiles its specialised kernels with"""
     src = open(os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "directxtex_b200", "csrc", "dxb_formats.h")).read()
     value = {k: int(v) for k, v in re.findall(r"\bDXB_FMT_(\w+) = (\d+)", src)}
     body = re.search(r"dxb_resolve_srgb_linear\(uint32_t flags, uint32_t fmt\)\s*\{(.*?)\n\}", src, re.S).group(1)
     always, keep = re.findall(r"((?:case DXB_FMT_\w+:\s*)+)return flags", body)[:2]
     names = lambda block: {value[n] for n in re.findall(r"case DXB_FMT_(\w+):", block)}
-    return names(keep), names(always)
+    body = re.search(r"dxb_make_linear\(uint32_t fmt\)\s*\{(.*?)\n\}", src, re.S).group(1)
+    twin = {value[a]: value[b] for a, b in re.findall(r"case DXB_FMT_(\w+):\s*return DXB_FMT_(\w+);", body)}
+    return names(keep), names(always), twin
 
 
-SRGB_KEEP, SRGB_ALWAYS = _srgb_lists()
+SRGB_KEEP, SRGB_ALWAYS, TWIN = _format_tables()
 BOX3, TAIL, SEP, TILE, LEVEL = FAMILIES
 
 # layout of device images: item -> (row pitch beyond the tight one, offset of the base from a 256-byte boundary)
@@ -145,17 +149,17 @@ def mode_of(c):
 
 
 def instantiations(c):
-    """(family, format, mode, sRGB, LIN) of every specialised kernel the case launches with option 0; mode is 0 where the
-    template has no mode parameter (k_mip_box3, k_mip_sep)"""
-    srgb, mode = srgb_bits(c.fmt, c.fl) == SRGB, mode_of(c)
+    """(family, format, mode, sRGB, LIN) of every specialised kernel the case launches with option 0; format is the case's
+    UNORM twin (dxb_make_linear), mode is 0 where the template has no mode parameter (k_mip_box3, k_mip_sep)"""
+    fmt, srgb, mode = TWIN.get(c.fmt, c.fmt), srgb_bits(c.fmt, c.fl) == SRGB, mode_of(c)
     out = set()
     for fam in c.fams:
         if fam == BOX3:
-            out.add(("box3", c.fmt, 0, srgb, mode == LIN))
+            out.add(("box3", fmt, 0, srgb, mode == LIN))
         elif fam == SEP:
-            out.add(("sep", c.fmt, 0, srgb, False))
+            out.add(("sep", fmt, 0, srgb, False))
         elif fam in (TILE, TAIL):
-            out.add((fam[len("k_mip_"):], c.fmt, mode, srgb, False))
+            out.add((fam[len("k_mip_"):], fmt, mode, srgb, False))
     return out
 
 
