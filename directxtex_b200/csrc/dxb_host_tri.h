@@ -1,4 +1,4 @@
-// dxb_host_tri.h — HOST-side construction of the triangle-filter weights (shared by dxb_api.cu and tests/emul).
+// dxb_host_tri.h — HOST-side construction of the triangle-filter weights (part of dxb_plan.h's chain records).
 #pragma once
 #include <vector>
 #include <utility>

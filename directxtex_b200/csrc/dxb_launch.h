@@ -1,42 +1,10 @@
-// dxb_launch.h — job/parameter structs shared by the kernels' translation units and the host API, plus the
-// host-callable launchers each kernel TU exports (hidden visibility; not part of the C ABI).
+// dxb_launch.h — the host-callable launchers each kernel TU exports (hidden visibility; not part of the C ABI), on the job and
+// parameter structs of dxb_jobs.h.
 #pragma once
 #include <stdint.h>
 #include <stddef.h>
 #include <cuda_runtime.h>
-#include "dxb_mipjob.h"
-
-struct dxb_job
-{
-    const uint8_t* src; uint8_t* dst;
-    size_t srcPitch, dstPitch;
-    uint32_t width, height;
-    uint32_t nbx, nby;
-    uint32_t firstUnit;
-    uint32_t pad;
-};
-
-struct dxb_compress_params
-{
-    uint32_t srcFormat, dstFormat;
-    uint32_t inF, outF, cflags, bcflags;
-    float threshold;
-    uint32_t totalUnits, njobs;
-};
-
-struct dxb_convert_params
-{
-    uint32_t srcFormat, dstFormat, inF, outF, flags;
-    uint32_t totalUnits, njobs;
-    float threshold;               // alpha threshold of 1-bit alpha destinations (B5G5R5A1)
-};
-
-struct dxb_mip_params
-{
-    uint32_t format, mode /*DXB_FILTER_* mode bits*/, filter, lflags;
-    uint32_t totalUnits, njobs;
-    dxb_tri_axis triX, triY;       // triangle filter only
-};
+#include "dxb_jobs.h"
 
 #ifndef DXB_BC7_WARPS
 #define DXB_BC7_WARPS 8       // warps per CTA of k_compress_bc7 (two blocks per warp, 8.6 KB dynamic shared per warp)

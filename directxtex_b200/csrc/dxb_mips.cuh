@@ -13,7 +13,7 @@
 #pragma once
 #include "dxb_pixel.cuh"
 
-#include "dxb_mipjob.h"
+#include "dxb_jobs.h"
 
 DXB_DEV dxb_px dxb_load_linear(uint32_t fmt, const uint8_t* base, size_t pitch, uint32_t x, uint32_t y, uint32_t lflags)
 {

@@ -6,6 +6,9 @@
 // against the oracle AND against this emulator.  The product library never contains, loads or
 // calls any of this: there is no CPU fallback.
 //
+// Every entry point plans its call with the library's own planners (csrc/dxb_plan.h): argument checks and HRESULTs, flag
+// resolution, the filter mode and a chain's job records.  Only the per-pixel and per-block walk is restated here.
+//
 // Build flags mirror the device build's numeric contract: -ffp-contract=off (== nvcc -fmad=false),
 // IEEE division/sqrt, -mfma only so that explicit fmaf() is one instruction (fmaf is exact either way).
 #include <cstdint>
@@ -17,6 +20,7 @@
 
 #include "dxb_portable.h"
 #include "dxb_formats.h"
+#include "dxb_plan.h"
 #include "dxb_pixel.cuh"
 #include "dxb_block.cuh"
 #include "dxb_bc15.cuh"
@@ -24,6 +28,16 @@
 #include "dxb_bc7.cuh"
 #include "dxb_bc6h.cuh"
 #endif
+
+// The dxb200_image the library's planners see for one w x h image at `pixels` (rowPitch 0: the tight pitch).  An unimplemented
+// format keeps pitches of 0: every planner refuses it before a pitch is read.
+static dxb200_image emul_image(const uint8_t* pixels, size_t w, size_t h, uint32_t fmt, size_t rowPitch)
+{
+    dxb200_image im = { w, h, fmt, 0, 0, const_cast<uint8_t*>(pixels) };
+    (void)compute_pitch(fmt, w, h, &im.rowPitch, &im.slicePitch);
+    if (rowPitch) { im.rowPitch = rowPitch; im.slicePitch = rowPitch * h; }
+    return im;
+}
 
 extern "C" {
 
@@ -36,20 +50,16 @@ void emul_bc7_force_shapes(const int8_t* shapes) { g_force_shapes = shapes; }
 int32_t emul_compress(const uint8_t* src, size_t w, size_t h, uint32_t srcFmt, size_t rowPitch,
                       uint32_t dstFmt, uint32_t flags, float threshold, uint8_t* dst)
 {
-    const uint32_t inF = dxb_convert_flags(srcFmt), outF = dxb_convert_flags(dstFmt);
+    const dxb200_image s = emul_image(src, w, h, srcFmt, rowPitch), d = emul_image(dst, w, h, dstFmt, 0);
+    CompressPlan plan;
+    const int32_t hr = plan_compress(&s, 1, dstFmt, flags, threshold, &d, &plan);
+    if (hr != DXB_S_OK) return hr;
+    const uint32_t inF = plan.P.inF, outF = plan.P.outF, cflags = plan.P.cflags, bcflags = plan.P.bcflags;
     const uint32_t bs = dxb_bc_block_bytes(dstFmt);
-    if (!inF || !outF || !bs || (inF & DXB_CONVF_BC)) return DXB_E_NOT_SUPPORTED;
-    if (rowPitch == 0) rowPitch = w * dxb_bytes_per_pixel(srcFmt);
-    uint32_t cflags = 0;
-    if (dstFmt == DXB_FMT_BC4_UNORM || dstFmt == DXB_FMT_BC4_SNORM) cflags = DXB_FILTER_RGB_COPY_RED;
-    if (dstFmt == DXB_FMT_BC5_UNORM || dstFmt == DXB_FMT_BC5_SNORM) cflags = DXB_FILTER_RGB_COPY_RED | DXB_FILTER_RGB_COPY_GREEN;
-    cflags |= (flags & DXB_FILTER_SRGB_MASK);
-    cflags = dxb_resolve_srgb_convert(cflags, srcFmt, dstFmt);
-    const uint32_t bcflags = flags & (DXB_BC_FLAGS_DITHER_RGB | DXB_BC_FLAGS_DITHER_A | DXB_BC_FLAGS_UNIFORM | DXB_BC_FLAGS_USE_3SUBSETS | DXB_BC_FLAGS_FORCE_BC7_MODE6);
-    dxb_image_desc img; img.pixels = src; img.rowPitch = rowPitch; img.width = (uint32_t)w; img.height = (uint32_t)h; img.format = srcFmt;
+    dxb_image_desc img; img.pixels = src; img.rowPitch = s.rowPitch; img.width = (uint32_t)w; img.height = (uint32_t)h; img.format = srcFmt;
     const uint32_t nbx = (uint32_t)((w + 3) / 4), nby = (uint32_t)((h + 3) / 4);
 #ifdef DXB_EMUL_BC7
-    if (dstFmt == DXB_FMT_BC7_UNORM || dstFmt == DXB_FMT_BC7_UNORM_SRGB)
+    if (plan.bc7)
     {
         // the device kernel encodes two consecutive blocks (raster order) per warp; so does the emulator
         const long total = (long)nbx * (long)nby;
@@ -69,9 +79,7 @@ int32_t emul_compress(const uint8_t* src, size_t w, size_t h, uint32_t srcFmt, s
         }
         return DXB_S_OK;
     }
-#endif
-#ifdef DXB_EMUL_BC7
-    if (dstFmt == DXB_FMT_BC6H_UF16 || dstFmt == DXB_FMT_BC6H_SF16)
+    if (plan.bc6h)
     {
         const long total = (long)nbx * (long)nby;
         #pragma omp parallel for schedule(dynamic, 32)
@@ -96,7 +104,7 @@ int32_t emul_compress(const uint8_t* src, size_t w, size_t h, uint32_t srcFmt, s
             dxb_px px[16];
             dxb_gather_block(img, bx, (uint32_t)by, inF, outF, cflags, px);
             alignas(16) uint8_t blk[16];
-            dxb_encode_block_bc15(dstFmt, px, bcflags, threshold, blk);
+            dxb_encode_block_bc15(dstFmt, px, bcflags, plan.P.threshold, blk);
             memcpy(dst + ((size_t)by * nbx + bx) * bs, blk, bs);
         }
     return DXB_S_OK;
@@ -106,24 +114,24 @@ int32_t emul_compress(const uint8_t* src, size_t w, size_t h, uint32_t srcFmt, s
 int32_t emul_convert(const uint8_t* src, size_t w, size_t h, uint32_t srcFmt, size_t srcPitch,
                      uint32_t dstFmt, size_t dstPitch, uint32_t filter, uint8_t* dst)
 {
-    const uint32_t inF = dxb_convert_flags(srcFmt), outF = dxb_convert_flags(dstFmt);
-    if (!inF || !outF || ((inF | outF) & DXB_CONVF_BC)) return DXB_E_NOT_SUPPORTED;
-    if (srcPitch == 0) srcPitch = w * dxb_bytes_per_pixel(srcFmt);
-    if (dstPitch == 0) dstPitch = w * dxb_bytes_per_pixel(dstFmt);
-    const uint32_t flags = dxb_resolve_srgb_convert(filter, srcFmt, dstFmt);
+    const dxb200_image s = emul_image(src, w, h, srcFmt, srcPitch), d = emul_image(dst, w, h, dstFmt, dstPitch);
+    dxb_convert_params P;
+    const int32_t hr = plan_convert(&s, 1, dstFmt, filter, &d, &P);
+    if (hr != DXB_S_OK) return hr;
+    const uint32_t inF = P.inF, outF = P.outF, flags = P.flags;
     if (flags & DXB_FILTER_DITHER_DIFFUSION)
     {
         std::vector<dxb_px> E(2 * (w + 2));
-        dxb_convert_diffuse_image(srcFmt, dstFmt, inF, outF, flags, src, srcPitch, dst, dstPitch, (uint32_t)w, (uint32_t)h, E.data(), E.data() + w + 2);
+        dxb_convert_diffuse_image(srcFmt, dstFmt, inF, outF, flags, src, s.rowPitch, dst, d.rowPitch, (uint32_t)w, (uint32_t)h, E.data(), E.data() + w + 2);
         return DXB_S_OK;
     }
     for (size_t y = 0; y < h; ++y)
         for (size_t x = 0; x < w; ++x)
         {
-            dxb_px v = dxb_load_pixel(srcFmt, src + y * srcPitch, x);
+            dxb_px v = dxb_load_pixel(srcFmt, src + y * s.rowPitch, x);
             v = dxb_convert_pixel(v, inF, outF, flags);
-            if (flags & DXB_FILTER_DITHER) dxb_store_pixel_dither(dstFmt, dst + y * dstPitch, x, (uint32_t)y, v);
-            else dxb_store_pixel(dstFmt, dst + y * dstPitch, x, v, 0.5f);       // TEX_THRESHOLD_DEFAULT (B5G5R5A1 alpha bit)
+            if (flags & DXB_FILTER_DITHER) dxb_store_pixel_dither(dstFmt, dst + y * d.rowPitch, x, (uint32_t)y, v);
+            else dxb_store_pixel(dstFmt, dst + y * d.rowPitch, x, v, P.threshold);
         }
     return DXB_S_OK;
 }
@@ -132,42 +140,36 @@ int32_t emul_convert(const uint8_t* src, size_t w, size_t h, uint32_t srcFmt, si
 
 // ---- mip chain emulation: dxb_mip_pixel, the same function k_mip_level and k_mip_tail run per pixel --------------------
 #include "dxb_mips.cuh"
-#include "dxb_host_tri.h"
 
-// ScaleMipMapsAlphaForCoverage for one chain held in `src` (ScratchImage layout); result chain in `dst`
-extern "C" int32_t emul_scale_mips_alpha(const uint8_t* src, uint8_t* dst, const size_t* offsets, const size_t* widths, const size_t* heights,
-                                         const size_t* pitches, size_t levels, uint32_t fmt, float ref);
+// the dxb200_image records of one chain held in ScratchImage layout at `base`
+static std::vector<dxb200_image> emul_chain(const uint8_t* base, const size_t* offsets, const size_t* widths, const size_t* heights,
+                                            const size_t* pitches, size_t levels, uint32_t fmt)
+{
+    std::vector<dxb200_image> chain(levels);
+    for (size_t l = 0; l < levels; ++l) chain[l] = emul_image(base + offsets[l], widths[l], heights[l], fmt, pitches[l]);
+    return chain;
+}
 
 extern "C" int32_t emul_generate_mipmaps(uint8_t* chainBase, const size_t* offsets, const size_t* widths, const size_t* heights,
                                          const size_t* pitches, size_t levels, uint32_t fmt, uint32_t filter)
 {
-    if (!dxb_bytes_per_pixel(fmt)) return DXB_E_NOT_SUPPORTED;
-    uint32_t mode = filter & DXB_FILTER_MODE_MASK;
-    auto ispow2 = [](size_t x) { return x && !(x & (x - 1)); };
-    if (!mode) mode = (ispow2(widths[0]) && ispow2(heights[0])) ? DXB_FILTER_BOX : DXB_FILTER_LINEAR;
-    if (mode == DXB_FILTER_BOX && (!ispow2(widths[0]) || !ispow2(heights[0]))) return DXB_E_FAIL;
-    const uint32_t lflags = dxb_resolve_srgb_linear(filter & DXB_FILTER_SRGB_MASK, fmt);
-    const uint8_t* stale = nullptr; size_t stalePitch = 0;
+    const std::vector<dxb200_image> chain = emul_chain(chainBase, offsets, widths, heights, pitches, levels, fmt);
+    uint32_t mode = 0;
+    const int32_t hr = plan_mips(chain.data(), 1, levels, filter, &mode);
+    if (hr != DXB_S_OK) return hr;
+    const MipPlan mp = build_mip_plan(chain.data(), 1, levels, filter, mode);
     for (size_t l = 1; l < levels; ++l)
     {
-        dxb_mip_job j;
-        j.src = chainBase + offsets[l - 1]; j.dst = chainBase + offsets[l];
-        j.srcPitch = pitches[l - 1]; j.dstPitch = pitches[l];
-        j.sw = (uint32_t)widths[l - 1]; j.sh = (uint32_t)heights[l - 1]; j.dw = (uint32_t)widths[l]; j.dh = (uint32_t)heights[l];
-        j.firstUnit = 0;
-        if (j.sh == 2) { stale = j.src + j.srcPitch; stalePitch = j.srcPitch; }
-        j.stale = nullptr; j.stalePitch = 0;
-        if (mode == DXB_FILTER_BOX && j.sh <= 1 && j.sw > 1 && stale) { j.stale = stale; j.stalePitch = stalePitch; }
-        TriLists tx, ty; dxb_tri_axis ax{}, ay{};
-        if (mode == DXB_FILTER_TRIANGLE)
+        const dxb_mip_job& j = mp.jobs[l - 1];
+        dxb_tri_axis ax{}, ay{};
+        if (!mp.tri.empty())
         {
-            build_triangle_axis(j.sw, j.dw, (filter & DXB_FILTER_WRAP_U) != 0, tx);
-            build_triangle_axis(j.sh, j.dh, (filter & DXB_FILTER_WRAP_V) != 0, ty);
-            ax.off = tx.off.data(); ax.src = tx.src.data(); ax.w = tx.w.data();
-            ay.off = ty.off.data(); ay.src = ty.src.data(); ay.w = ty.w.data();
+            const TriLists& tx = mp.tri[2 * (l - 1)]; const TriLists& ty = mp.tri[2 * (l - 1) + 1];
+            ax = { tx.off.data(), tx.src.data(), tx.w.data() };
+            ay = { ty.off.data(), ty.src.data(), ty.w.data() };
         }
         for (uint32_t y = 0; y < j.dh; ++y)
-            for (uint32_t x = 0; x < j.dw; ++x) dxb_mip_pixel(fmt, mode, j, x, y, filter, lflags, ax, ay);
+            for (uint32_t x = 0; x < j.dw; ++x) dxb_mip_pixel(mp.P.format, mp.P.mode, j, x, y, mp.P.filter, mp.P.lflags, ax, ay);
     }
     return DXB_S_OK;
 }
@@ -176,11 +178,12 @@ extern "C" int32_t emul_generate_mipmaps(uint8_t* chainBase, const size_t* offse
 #include "dxb_decode.cuh"
 extern "C" int32_t emul_decompress(const uint8_t* blocks, size_t w, size_t h, uint32_t bcFmt, uint32_t dstFmt, uint8_t* dst)
 {
-    const uint32_t bs = dxb_bc_block_bytes(bcFmt), bpp = dxb_bytes_per_pixel(dstFmt);
-    if (!bs || !bpp) return DXB_E_NOT_SUPPORTED;
-    const uint32_t inF = dxb_convert_flags(bcFmt), outF = dxb_convert_flags(dstFmt);
-    const uint32_t cflags = dxb_resolve_srgb_convert(0, bcFmt, dstFmt);
-    const size_t nbx = (w + 3) / 4, nby = (h + 3) / 4, dpitch = w * bpp;
+    const dxb200_image s = emul_image(blocks, w, h, bcFmt, 0), d = emul_image(dst, w, h, dstFmt, 0);
+    dxb_compress_params P;
+    const int32_t hr = plan_decompress(&s, 1, dstFmt, &d, &P);
+    if (hr != DXB_S_OK) return hr;
+    const uint32_t bs = dxb_bc_block_bytes(bcFmt), inF = P.inF, outF = P.outF, cflags = P.cflags;
+    const size_t nbx = (w + 3) / 4, nby = (h + 3) / 4, dpitch = d.rowPitch;
     for (size_t by = 0; by < nby; ++by)
         for (size_t bx = 0; bx < nbx; ++bx)
         {
@@ -195,40 +198,36 @@ extern "C" int32_t emul_decompress(const uint8_t* blocks, size_t w, size_t h, ui
     return DXB_S_OK;
 }
 
-static float emul_alpha_coverage(const uint8_t* img, size_t w, size_t h, size_t pitch, uint32_t fmt, float ref, float scale)
+static float emul_alpha_coverage(const dxb200_image& im, float ref, float scale)
 {
-    if (w < 2 || h < 2) return 0.0f;
     unsigned long long count = 0;
-    for (size_t y = 0; y + 1 < h; ++y)
-        for (size_t x = 0; x + 1 < w; ++x)
+    for (size_t y = 0; y + 1 < im.height; ++y)
+        for (size_t x = 0; x + 1 < im.width; ++x)
         {
-            const uint8_t* r0 = img + y * pitch; const uint8_t* r1 = r0 + pitch;
-            count += dxb_alpha_coverage_cell(dxb_load_pixel(fmt, r0, x).w, dxb_load_pixel(fmt, r1, x).w,
-                                             dxb_load_pixel(fmt, r0, x + 1).w, dxb_load_pixel(fmt, r1, x + 1).w, scale, ref);
+            const uint8_t* r0 = im.pixels + y * im.rowPitch; const uint8_t* r1 = r0 + im.rowPitch;
+            count += dxb_alpha_coverage_cell(dxb_load_pixel(im.format, r0, x).w, dxb_load_pixel(im.format, r1, x).w,
+                                             dxb_load_pixel(im.format, r0, x + 1).w, dxb_load_pixel(im.format, r1, x + 1).w, scale, ref);
         }
-    const float cscale = static_cast<float>((w - 1) * (h - 1) * 8 * 8);
-    return cscale > 0.0f ? static_cast<float>(count) / cscale : 0.0f;
+    return alpha_coverage_fraction(count, im.width, im.height);
 }
-int32_t emul_scale_mips_alpha(const uint8_t* src, uint8_t* dst, const size_t* offsets, const size_t* widths, const size_t* heights,
-                              const size_t* pitches, size_t levels, uint32_t fmt, float ref)
+
+// ScaleMipMapsAlphaForCoverage for one chain held in `src` (ScratchImage layout); result chain in `dst`
+extern "C" int32_t emul_scale_mips_alpha(const uint8_t* src, uint8_t* dst, const size_t* offsets, const size_t* widths, const size_t* heights,
+                                         const size_t* pitches, size_t levels, uint32_t fmt, float ref)
 {
-    if (!dxb_bytes_per_pixel(fmt)) return DXB_E_NOT_SUPPORTED;
-    const float target = emul_alpha_coverage(src + offsets[0], widths[0], heights[0], pitches[0], fmt, ref, 1.0f);
-    memcpy(dst + offsets[0], src + offsets[0], pitches[0] * heights[0]);
+    const std::vector<dxb200_image> s = emul_chain(src, offsets, widths, heights, pitches, levels, fmt);
+    const std::vector<dxb200_image> d = emul_chain(dst, offsets, widths, heights, pitches, levels, fmt);
+    const int32_t hr = plan_alpha_coverage(s.data(), levels, d.data());
+    if (hr != DXB_S_OK) return hr;
+    const float target = emul_alpha_coverage(s[0], ref, 1.0f);
+    memcpy(d[0].pixels, s[0].pixels, s[0].rowPitch * s[0].height);
     for (size_t l = 1; l < levels; ++l)
     {
-        float lo = 0.0f, hi = 4.0f, scale = 1.0f;
-        for (int it = 0; it < 10; ++it)
-        {
-            const float cov = emul_alpha_coverage(src + offsets[l], widths[l], heights[l], pitches[l], fmt, ref, scale);
-            if (cov < target) lo = scale;
-            else if (cov > target) hi = scale;
-            else break;
-            scale = (lo + hi) * 0.5f;
-        }
-        for (size_t y = 0; y < heights[l]; ++y)
-            for (size_t x = 0; x < widths[l]; ++x)
-                dxb_scale_alpha_pixel(fmt, src + offsets[l] + y * pitches[l], dst + offsets[l] + y * pitches[l], (uint32_t)x, scale);
+        float scale = 1.0f;
+        (void)estimate_alpha_scale(target, [&](float sc, float* cov) { *cov = emul_alpha_coverage(s[l], ref, sc); return DXB_S_OK; }, &scale);
+        for (size_t y = 0; y < s[l].height; ++y)
+            for (size_t x = 0; x < s[l].width; ++x)
+                dxb_scale_alpha_pixel(fmt, s[l].pixels + y * s[l].rowPitch, d[l].pixels + y * d[l].rowPitch, (uint32_t)x, scale);
     }
     return DXB_S_OK;
 }

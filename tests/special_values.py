@@ -258,7 +258,7 @@ def assert_within_one_code(oracle, got, want, w, h, fmt, ctx=""):
 
 
 def convert_refused(dst_fmt, flags):
-    """the pairs the library refuses (dxb_api.cu plan_convert): dithered stores to the 16-bit packed formats"""
+    """the pairs the library refuses (dxb_plan.h plan_convert): dithered stores to the 16-bit packed formats"""
     return bool(flags & (F.TEX_FILTER_DITHER | F.TEX_FILTER_DITHER_DIFFUSION)) and dst_fmt in PACKED16
 
 

@@ -108,6 +108,25 @@ def test_argument_validation_hresults():
     assert F.hr_u32(L.dxb200_resize(s, 1, 0, wrongfmt)) == F.E_INVALIDARG                      # Resize never converts
 
 
+def test_emulator_refuses_what_the_library_refuses(emul):
+    """the host emulator plans its calls with the library's planners, so it answers a call the library refuses with the same HRESULT"""
+    a = np.zeros((8, 8, 4), np.uint8)
+
+    def library_hr(fn, *args):
+        with pytest.raises(capi.DxTexError) as e:
+            fn(*args)
+        return e.value.hr
+    cases = [
+        (emul.convert, capi.convert, (a, 8, 8, 28, 28), F.E_INVALIDARG),                                   # same format
+        (emul.convert, capi.convert, (a, 8, 8, 28, 85, F.TEX_FILTER_DITHER), F.HRESULT_E_NOT_SUPPORTED),   # dithered B5G6R5 store
+        (emul.compress, capi.compress, (a, 8, 8, 71, 77), F.E_INVALIDARG),                                 # BC source
+        (emul.generate_mipmaps, capi.generate_mipmaps, (a, 8, 8, 28, 0x600000), F.HRESULT_E_NOT_SUPPORTED),  # unknown filter mode
+    ]
+    for em, lib, args, want in cases:
+        assert library_hr(lib, *args) == want, args
+        assert em(*args)[0] == want, args
+
+
 def test_compute_entry_points_fail_loudly_without_gpu():
     if capi.lib.dxb200_device_count() > 0:
         pytest.skip("a CUDA device is present")
