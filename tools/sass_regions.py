@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """Static SASS instruction count of one kernel, per encoder stage (runs on the CPU, needs nvdisasm / cuobjdump).
 
-    python tools/sass_regions.py directxtex_b200/_lib/dxb_k_bc7.o k_compress_bc7_tmaILb0ELb1
+    python tools/sass_regions.py directxtex_b200/_lib/dxb_k_bc7.o k_compress_bc7_tmaILb0ELb1 [--pipes]
 
 The object (or cubin) must be built with -lineinfo (directxtex_b200/build.py does), and --src must hold the sources
 it was built from (line numbers).  `nvdisasm -gi` annotates each instruction with its source line followed by the
@@ -11,6 +11,11 @@ opened at `start` when `end` is None).  An instruction counts under the innermos
 region, so an inlined helper that belongs to no region (a fp32-pair wrapper, dxb_rne, dxb_convert_pixel, ...) is
 counted under the stage that calls it.  An instruction without line information takes the region of the one before
 it.  Instruction scheduling mixes neighbouring lines, so the split is good to a few instructions per region.
+
+--pipes splits each region's count by the execution pipe the opcode issues to (PIPES).  An H100 SM sub-partition has 32
+FP32 lanes but 16 lanes for each integer half: a warp instruction on the ALU pipe (logic, shifts, compares, selects,
+min/max, integer adds, byte permutes) or on the FMA-heavy integer pipe (IMAD, IDP, the tensor-core MMAs) occupies its
+pipe for two cycles, so a region whose ALU share is well above 50 % is bound by that pipe rather than by the issue slot.
 """
 import argparse
 import os
@@ -88,6 +93,25 @@ def disassemble(path, kernel):
 
 LINE = re.compile(r'//## File "([^"]+)", line (\d+)')
 INSN = re.compile(r"^\s+/\*[0-9a-f]{4,}\*/\s+(.*?);?\s*$")
+OPCODE = re.compile(r"^(?:@!?U?P[T0-9]+\s+)?([A-Z0-9_]+)")
+
+# opcode (without modifiers) -> pipe class on sm_90; the uniform datapath (U*) and moves fall under "other"
+PIPES = {
+    "FP32": "FFMA FADD FMUL FFMA32I FADD32I FMUL32I FSWZADD HFMA2 HADD2 HMUL2",
+    "FMA-int": "IMAD IMAD32I IDP IMUL HMMA IMMA",
+    "ALU": "LOP3 LOP SHF SHL SHR ISETP SEL FSEL FSETP FSET FMNMX IADD3 IADD VIADD PRMT VABSDIFF4 VABSDIFF VIMNMX VIMNMX3 "
+           "VIADDMNMX IMNMX LEA ISCADD IABS PLOP3 P2R R2P I2FP",
+    "XU": "MUFU F2I I2F F2F FRND FCHK POPC FLO BREV",
+    "MIO": "LDS STS LDG STG LD ST LDC LDL STL SHFL REDUX ATOMS ATOMG ATOM RED LDSM LDGSTS UTMALDG SYNCS MATCH",
+    "control": "BRA BRX BSSY BSYNC EXIT CALL RET BAR WARPSYNC NOP YIELD BPT DEPBAR ENDCOLLECTIVE ELECT FENCE MEMBAR",
+}
+PIPE_OF = {op: pipe for pipe, ops in PIPES.items() for op in ops.split()}
+PIPE_ORDER = list(PIPES) + ["other"]
+
+
+def pipe_of(insn):
+    m = OPCODE.match(insn)
+    return PIPE_OF.get(m.group(1), "other") if m else "other"
 
 
 def count(sass, spans):
@@ -96,7 +120,7 @@ def count(sass, spans):
             if a <= ln <= b:
                 return name
         return None
-    counts, chain, fresh, last = {}, [], False, "(unattributed)"
+    counts, pipes, chain, fresh, last = {}, {}, [], False, "(unattributed)"
     for line in sass.splitlines():
         m = LINE.search(line)
         if m:
@@ -104,13 +128,17 @@ def count(sass, spans):
                 chain, fresh = [], True
             chain.append((m.group(1), int(m.group(2))))
             continue
-        if not INSN.match(line):
+        i = INSN.match(line)
+        if not i:
             continue
         fresh = False
         r = next((x for x in (region(f, ln) for f, ln in chain) if x), None) or last
         last = r
         counts[r] = counts.get(r, 0) + 1
-    return counts
+        per = pipes.setdefault(r, {})
+        p = pipe_of(i.group(1))
+        per[p] = per.get(p, 0) + 1
+    return counts, pipes
 
 
 def main():
@@ -118,14 +146,25 @@ def main():
     ap.add_argument("binary", help="object file or cubin built with -lineinfo")
     ap.add_argument("kernel", help="substring of the kernel's mangled name, e.g. k_compress_bc7_tmaILb0ELb1")
     ap.add_argument("--src", default=CSRC, help="directory of the sources the binary was built from")
+    ap.add_argument("--pipes", action="store_true", help="split each region's count by execution pipe (PIPES)")
     args = ap.parse_args()
     name, sass = disassemble(args.binary, args.kernel)
-    counts = count(sass, region_spans(args.src))
+    counts, pipes = count(sass, region_spans(args.src))
     order = [r[0] for r in REGIONS] + ["(unattributed)"]
     print(name[len(".text."):])
-    for r in sorted(counts, key=order.index):
-        print("%-34s %6d" % (r, counts[r]))
-    print("%-34s %6d" % ("total", sum(counts.values())))
+    if args.pipes:
+        print("%-34s %6s" % ("region", "SASS") + "".join("%9s" % p for p in PIPE_ORDER) + "   ALU share")
+    total = {}
+    for r in sorted(counts, key=order.index) + ["total"]:
+        per = pipes.get(r, total)
+        n = counts.get(r, sum(counts.values()))
+        line = "%-34s %6d" % (r, n)
+        if args.pipes:
+            line += "".join("%9d" % per.get(p, 0) for p in PIPE_ORDER) + "   %5.0f %%" % (100.0 * per.get("ALU", 0) / max(n, 1))
+            if r != "total":
+                for p, v in per.items():
+                    total[p] = total.get(p, 0) + v
+        print(line)
 
 
 if __name__ == "__main__":
