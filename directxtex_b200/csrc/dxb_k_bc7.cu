@@ -5,6 +5,7 @@
 #include <atomic>
 #include "dxb_launch.h"
 #include "dxb_bc7.cuh"
+#include "dxb_udiv.h"
 
 template <bool THREE>
 __global__ void __launch_bounds__(DXB_BC7_WARPS * 32, DXB_BC7_MINB) k_compress_bc7(const dxb_job* __restrict__ jobs, dxb_job single, dxb_compress_params P)
@@ -86,24 +87,7 @@ int dxb_occupancy_bc7()
 //     of the request, so its round trip is off the critical path too.  T.counter == nullptr: statically strided tiles.
 // Eligibility (dxb_launch_bc7_tma): RGBA32F source, full 4x4 blocks only (partial blocks need CompressBC's {0,0,0,1} replication,
 // which a tensor map's zero fill cannot express), 16-byte aligned rows, images of one size at a constant pointer stride.
-// unsigned division by a run-time constant (Granlund / Montgomery round-up form): q = n / d for every 32-bit n
-struct dxb_udiv { uint32_t d, M, sh; };
-static dxb_udiv dxb_udiv_make(uint32_t d)
-{
-    dxb_udiv r; r.d = d; r.M = 0; r.sh = 0;
-    if (d > 1u)
-    {
-        uint32_t l = 0; while ((1ull << l) < d) ++l;                      // ceil(log2 d)
-        r.M = (uint32_t)(((1ull << 32) * ((1ull << l) - d)) / d + 1ull); r.sh = l - 1u;
-    }
-    return r;
-}
-__device__ __forceinline__ uint32_t dxb_udiv_do(uint32_t n, const dxb_udiv& k)
-{
-    if (k.d <= 1u) return n;
-    const uint32_t t = __umulhi(k.M, n);
-    return (t + ((n - t) >> 1)) >> k.sh;
-}
+// The tile index is split into (image, block row, tile column) with dxb_udiv (dxb_udiv.h).
 
 struct dxb_bc7_tma_params
 {

@@ -385,6 +385,62 @@ def _tma_cases(emul, torch, rng):
             assert he == 0 and np.array_equal(out[i], em), (pad, i)
 
 
+_MANY_TILES = {}
+
+
+def _many_tiles_case(emul, flags, df):
+    """a 1000 x 512 RGBA32F image (250 blocks per row: 16 tiles, the last one partial; 2048 tiles) and its emulator blocks, made once
+    per (flags, target) and shared by the feeds"""
+    key = (flags, df)
+    if key not in _MANY_TILES:
+        img = np.random.default_rng(77).random((512, 1000, 4), dtype=np.float32)
+        img[:256, :500, 3] = 1.0
+        he, em = emul.compress(img, 1000, 512, 2, df, flags)
+        assert he == 0
+        _MANY_TILES[key] = (img, em)
+    return _MANY_TILES[key]
+
+
+@pytest.mark.parametrize("df", [98, 99])
+@pytest.mark.parametrize("flags", [0, F.TEX_COMPRESS_BC7_USE_3SUBSETS])
+@pytest.mark.parametrize("feed", [0, 1, 2, 3, 4])
+def test_bc7_every_feed_equals_emulator(emul, feed, flags, df):
+    """Every value of DXB200_OPT_BC7_FEED (0 direct kernel, 1 TMA with the atomic tile counter, 2 TMA with statically strided tiles,
+    3 TMA with one CTA per tile, 4 automatic) with and without the three-subset pass, into BC7_UNORM and BC7_UNORM_SRGB (so each of
+    the four k_compress_bc7_tma instantiations runs under every TMA feed): single images whose width ends in a partial tile or fills
+    whole tiles, and an array at a constant stride, all equal the emulator.  One image has 16 x 128 = 2048 tiles, more than a launch
+    has resident CTAs (132 SMs x at most 3 CTAs of ~76 KB shared memory), so under feeds 1 and 2 every CTA takes further tiles after
+    its first from the counter or the grid stride; a skipped, repeated or misplaced tile leaves blocks that differ from the
+    emulator.  The TMA launch counter moves for single images exactly under feeds 1-3, and for the array under feeds 1-4."""
+    rng = np.random.default_rng(1000 + 10 * feed + df + (flags != 0))
+    old = capi.lib.dxb200_get_option(capi.OPT_BC7_FEED)
+    assert capi.lib.dxb200_set_option(capi.OPT_BC7_FEED, feed) == 0
+    try:
+        for (w, h) in [(72, 20), (64, 8), (328, 12), (1000, 512)]:
+            if w == 1000:
+                img, em = _many_tiles_case(emul, flags, df)
+            else:
+                img = rng.random((h, w, 4), dtype=np.float32)
+                img[: h // 2, :, 3] = 1.0
+                he, em = emul.compress(img, w, h, 2, df, flags)
+                assert he == 0
+            before = capi.tma_launch_count()
+            got = capi.compress(img, w, h, 2, df, flags)
+            moved = capi.tma_launch_count() - before
+            assert np.array_equal(got, em), ("single", w, h)
+            assert (moved > 0) == (feed in (1, 2, 3)), ("single", w, h, moved)
+        imgs = [rng.random((20, 72, 4), dtype=np.float32) for _ in range(3)]
+        before = capi.tma_launch_count()
+        outs = capi.compress_array(imgs, 72, 20, 2, df, flags)
+        moved = capi.tma_launch_count() - before
+        for i, (img, got) in enumerate(zip(imgs, outs)):
+            he, em = emul.compress(img, 72, 20, 2, df, flags)
+            assert he == 0 and np.array_equal(got, em), ("array", i)
+        assert (moved > 0) == (feed != 0), ("array", moved)
+    finally:
+        capi.lib.dxb200_set_option(capi.OPT_BC7_FEED, old)
+
+
 def test_device_api_with_torch_pointers(oracle):
     torch = pytest.importorskip("torch")
     img = synth.c1_rgba8(128, 64, seed=2)
