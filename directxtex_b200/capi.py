@@ -118,7 +118,7 @@ def tma_launch_count():
 
 
 def kernel_launch_count(kernel):
-    """launches of the kernel family `kernel` (e.g. "k_mip_tile") so far in this process"""
+    """launches of the __global__ function `kernel`, named without template arguments (e.g. "k_mip_tile"), so far in this process"""
     return int(lib.dxb200_kernel_launch_count(kernel.encode()))
 
 

@@ -43,7 +43,7 @@ constexpr size_t BAND_CHUNK = size_t(48) << 20;     // slot buffer bytes of one 
 constexpr size_t ITEM_CHUNK = size_t(80) << 20;
 
 std::mutex g_mu;                // guards the device table only; calls on different lanes / devices run concurrently
-std::atomic<uint64_t> g_launches{0}, g_tma_launches{0};
+std::atomic<uint64_t> g_launches{0};
 std::mutex g_count_mu;                                  // guards g_kernel_launches
 std::map<std::string, uint64_t> g_kernel_launches;      // launches per kernel name (dxb200_kernel_launch_count)
 std::atomic<int32_t> g_mip_kernels{0};                  // DXB200_OPT_MIP_KERNELS
@@ -351,20 +351,16 @@ int32_t launch_compress(const CompressPlan& plan, const dxb200_image* src, const
     const Device& d = *t_v.dev;
     if (plan.bc6h)
     {
-        dxb_launch_bc6h(grid_for(jt.total, 2 * DXB_BC6H_WARPS, (uint32_t)d.gridBC6H * 4u), stream, jt.dev.d, jt.host.data(), P);
-        return check_launch("k_compress_bc6h");
+        return check_launch(dxb_launch_bc6h(grid_for(jt.total, 2 * DXB_BC6H_WARPS, (uint32_t)d.gridBC6H * 4u), stream, jt.dev.d, jt.host.data(), P));
     }
     if (plan.bc7)
     {
         // RGBA32F sources of full blocks: persistent kernel fed by TMA tile loads; everything else: the direct kernel with one CTA
         // per 2 * DXB_BC7_WARPS blocks (no grid-stride cap): block costs differ (alpha blocks run the separate-alpha tasks), so the
         // hardware CTA scheduler balances better than a static stride
-        if (dxb_launch_bc7_tma((unsigned)d.gridBC7, stream, jt.host.data(), P)) g_tma_launches.fetch_add(1, std::memory_order_relaxed);
-        else dxb_launch_bc7(grid_for(jt.total, 2 * DXB_BC7_WARPS, UINT32_MAX), stream, jt.dev.d, jt.host.data(), P);
-        return check_launch("k_compress_bc7");
+        return check_launch(dxb_launch_bc7(grid_for(jt.total, 2 * DXB_BC7_WARPS, UINT32_MAX), (unsigned)d.gridBC7, stream, jt.dev.d, jt.host.data(), P));
     }
-    dxb_launch_bc15(grid_for(jt.total, 128, (uint32_t)d.gridBC15 * 4u), stream, jt.dev.d, jt.host.data(), P);
-    return check_launch("k_compress_bc15");
+    return check_launch(dxb_launch_bc15(grid_for(jt.total, 128, (uint32_t)d.gridBC15 * 4u), stream, jt.dev.d, jt.host.data(), P));
 }
 
 // ---- host staging -------------------------------------------------------------------------------------
@@ -380,7 +376,7 @@ struct Plane { const dxb200_image* host; size_t per; Copy first, rest; };
 // bytes of device memory (an item larger than that is a chunk by itself), and chunk c goes through slot c % NSLOT, so the H2D
 // copies, kernels and D2H copies of consecutive chunks overlap (fully when the caller's memory is pinned, see
 // dxb200_host_alloc).  In the slot's buffer the chunk's images lie plane after plane, each on a 256-byte boundary, so equal
-// images of one plane sit at a constant stride (the vector kernels' alignment checks and dxb_launch_bc7_tma rely on both).
+// images of one plane sit at a constant stride (the vector kernels' alignment checks and the BC7 TMA feed rely on both).
 // fn(dev, count, stream) enqueues the kernels: dev[p] is plane p's images of the chunk's `count` items, with device pointers.
 // prog (optional) is told before each chunk's upload the units[] of the items the chunk completes, and stops the call between
 // chunks (E_ABORT).  Every slot is synchronised before returning; the first error wins.
@@ -517,13 +513,11 @@ int32_t launch_convert(dxb_convert_params P, const dxb200_image* src, const dxb2
         void* dErr = nullptr;
         hr = cuda_hr(cudaMallocAsync(&dErr, (size_t)errStride * n * sizeof(float) * 4, stream), "cudaMallocAsync(errors)");
         if (hr != DXB_S_OK) return hr;
-        dxb_launch_convert_diffuse(stream, (n > 1) ? jt.dev.d : nullptr, jt.host.data(), P, dErr, errStride);
-        hr = check_launch("k_convert_diffuse");
+        hr = check_launch(dxb_launch_convert_diffuse(stream, (n > 1) ? jt.dev.d : nullptr, jt.host.data(), P, dErr, errStride));
         cudaFreeAsync(dErr, stream);
         return hr;
     }
-    dxb_launch_convert(grid_for(jt.total, 256, (uint32_t)t_v.dev->gridRow * 8u), stream, jt.dev.d, jt.host.data(), P);
-    return check_launch("k_convert");
+    return check_launch(dxb_launch_convert(grid_for(jt.total, 256, (uint32_t)t_v.dev->gridRow * 8u), stream, jt.dev.d, jt.host.data(), P));
 }
 
 // ---- PremultiplyAlpha ---------------------------------------------------------------------------
@@ -533,8 +527,7 @@ int32_t launch_pmalpha(dxb_convert_params P, const dxb200_image* src, const dxb2
     const int32_t hr = jt.build(src, dst, n, false, stream);
     if (hr != DXB_S_OK) return hr;
     P.totalUnits = jt.total; P.njobs = (uint32_t)n;
-    dxb_launch_pmalpha(grid_for(jt.total, 256, (uint32_t)t_v.dev->gridRow * 8u), stream, jt.dev.d, jt.host.data(), P);
-    return check_launch("k_pmalpha");
+    return check_launch(dxb_launch_pmalpha(grid_for(jt.total, 256, (uint32_t)t_v.dev->gridRow * 8u), stream, jt.dev.d, jt.host.data(), P));
 }
 
 // ---- GenerateMipMaps ----------------------------------------------------------------------------
@@ -580,7 +573,6 @@ extern "C" {
 const char* dxb200_version(void) { return "dxtex_b200 0.1 (sm_90a)"; }
 const char* dxb200_last_error(void) { return t_lastError.c_str(); }
 uint64_t dxb200_launch_count(void) { return g_launches.load(); }
-uint64_t dxb200_tma_launch_count(void) { return g_tma_launches.load(); }
 uint64_t dxb200_kernel_launch_count(const char* kernel)
 {
     if (!kernel) return 0;
@@ -588,6 +580,7 @@ uint64_t dxb200_kernel_launch_count(const char* kernel)
     const auto it = g_kernel_launches.find(kernel);
     return it == g_kernel_launches.end() ? 0 : it->second;
 }
+uint64_t dxb200_tma_launch_count(void) { return dxb200_kernel_launch_count("k_compress_bc7_tma"); }
 int32_t dxb200_set_option(uint32_t option, int32_t value)
 {
     if (option == DXB200_OPT_BC7_FEED) { dxb_bc7_set_feed(value); return DXB_S_OK; }
@@ -733,8 +726,7 @@ static int32_t launch_decompress(dxb_compress_params P, const dxb200_image* src,
     const int32_t hr = jt.build(src, dst, n, true, stream);
     if (hr != DXB_S_OK) return hr;
     P.totalUnits = jt.total; P.njobs = (uint32_t)n;
-    dxb_launch_decompress(grid_for(jt.total, 128, (uint32_t)t_v.dev->gridBC15 * 8u), stream, jt.dev.d, jt.host.data(), P);
-    return check_launch("k_decompress");
+    return check_launch(dxb_launch_decompress(grid_for(jt.total, 128, (uint32_t)t_v.dev->gridBC15 * 8u), stream, jt.dev.d, jt.host.data(), P));
 }
 
 int32_t dxb200_decompress_device(const dxb200_image* src, size_t nimages, uint32_t dstFormat, const dxb200_image* dst, void* stream)
@@ -898,8 +890,7 @@ static int32_t alpha_coverage_device(const dxb200_image& img, float ref, float s
     DXB_CUDA(cudaMemsetAsync(dCount, 0, sizeof(unsigned long long), st));
     const uint64_t cells = (uint64_t)(img.width - 1) * (img.height - 1);
     const uint32_t grid = (uint32_t)std::max<uint64_t>(1, std::min<uint64_t>((cells + 255) / 256, (uint64_t)t_v.dev->gridRow * 8u));
-    dxb_launch_alpha_coverage(grid, st, j, img.format, scale, ref, dCount);
-    int32_t hr = check_launch("k_alpha_coverage");
+    const int32_t hr = check_launch(dxb_launch_alpha_coverage(grid, st, j, img.format, scale, ref, dCount));
     if (hr != DXB_S_OK) return hr;
     unsigned long long hCount = 0;
     DXB_CUDA(cudaMemcpyAsync(&hCount, dCount, sizeof(hCount), cudaMemcpyDeviceToHost, st));
@@ -928,8 +919,7 @@ static int32_t scale_alpha_for_coverage_device(const dxb200_image* src, size_t n
         j.width = (uint32_t)src[l].width; j.height = (uint32_t)src[l].height;
         const uint64_t px = (uint64_t)j.width * j.height;
         const uint32_t grid = (uint32_t)std::max<uint64_t>(1, std::min<uint64_t>((px + 255) / 256, (uint64_t)t_v.dev->gridRow * 8u));
-        dxb_launch_scale_alpha(grid, st, j, src[l].format, scale);
-        hr = check_launch("k_scale_alpha");
+        hr = check_launch(dxb_launch_scale_alpha(grid, st, j, src[l].format, scale));
     }
     cudaFreeAsync(dCount, st);
     return hr;

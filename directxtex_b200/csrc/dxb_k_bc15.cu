@@ -7,6 +7,7 @@
 //                              No pair names an sRGB format: an sRGB call matches its twins' pair (dxb_make_linear).
 #include <algorithm>
 #include "dxb_launch.h"
+#include "dxb_dispatch.h"
 #include "dxb_bc15.cuh"
 
 // Launch shape per destination format.  The encoders are thousands of instructions of mostly straight-line code per block and
@@ -65,24 +66,25 @@ __global__ void __launch_bounds__(dxb_bc15_threads(DF), dxb_bc15_minb(DF)) k_com
     bc15_body<false, DF, SF>(jobs, single, P);
 }
 
-// hot pairs: colour formats x {RGBA8, BGRA8, RGBA16F, RGBA32F}; BC4 x {R8, RGBA8, R32F, RGBA32F}; BC5 x {R8G8, RGBA8, R32G32F, RGBA32F}
-#define DXB_BC15_PAIRS(X) \
-    X(71, 28) X(71, 87) X(71, 10) X(71, 2) X(74, 28) X(74, 87) X(74, 10) X(74, 2) X(77, 28) X(77, 87) X(77, 10) X(77, 2) \
-    X(80, 61) X(80, 28) X(80, 41) X(80, 2) X(81, 61) X(81, 28) X(81, 41) X(81, 2) \
-    X(83, 49) X(83, 28) X(83, 16) X(83, 2) X(84, 49) X(84, 28) X(84, 16) X(84, 2)
-
-void dxb_launch_bc15(unsigned grid, cudaStream_t stream, const dxb_job* jobs, const dxb_job* hostJobs, const dxb_compress_params& P)
+const char* dxb_launch_bc15(unsigned grid, cudaStream_t stream, const dxb_job* jobs, const dxb_job* hostJobs, const dxb_compress_params& P)
 {
     // sRGB formats run their twins' kernels: an sRGB step is resolved into P.cflags, and the specialised kernels take only
     // the default flag set
     const uint32_t df = dxb_make_linear(P.dstFormat), sf = dxb_make_linear(P.srcFormat);
-    if (P.bcflags == 0 && P.cflags == dxb_bc15_default_cflags(df))
+    const auto hot = [&](auto DF, auto SF)
     {
-#define DXB_X(DF, SF) if (df == DF && sf == SF) { k_compress_bc15_t<DF, SF><<<std::max(1u, grid * 128u / dxb_bc15_threads(DF)), dxb_bc15_threads(DF), 0, stream>>>(jobs, hostJobs[0], P); return; }
-        DXB_BC15_PAIRS(DXB_X)
-#undef DXB_X
-    }
+        constexpr uint32_t threads = dxb_bc15_threads(decltype(DF)::value);
+        k_compress_bc15_t<decltype(DF)::value, decltype(SF)::value><<<std::max(1u, grid * 128u / threads), threads, 0, stream>>>(jobs, hostJobs[0], P);
+    };
+    // hot (destination, source) pairs: colour formats x {RGBA8, BGRA8, RGBA16F, RGBA32F}; BC4 x {R8, RGBA8, R32F, RGBA32F};
+    // BC5 x {R8G8, RGBA8, R32G32F, RGBA32F}
+    if (P.bcflags == 0 && P.cflags == dxb_bc15_default_cflags(df) &&
+        dxb_on_pair<71, 28, 71, 87, 71, 10, 71, 2,  74, 28, 74, 87, 74, 10, 74, 2,  77, 28, 77, 87, 77, 10, 77, 2,
+                    80, 61, 80, 28, 80, 41, 80, 2,  81, 61, 81, 28, 81, 41, 81, 2,
+                    83, 49, 83, 28, 83, 16, 83, 2,  84, 49, 84, 28, 84, 16, 84, 2>(df, sf, hot))
+        return "k_compress_bc15_t";
     k_compress_bc15<<<grid, 128, 0, stream>>>(jobs, hostJobs[0], P);
+    return "k_compress_bc15";
 }
 int dxb_occupancy_bc15()
 {

@@ -39,9 +39,10 @@ __global__ void __launch_bounds__(DXB_BC6H_WARPS * 32, DXB_BC6H_MINB) k_compress
     }
 }
 
-void dxb_launch_bc6h(unsigned grid, cudaStream_t stream, const dxb_job* jobs, const dxb_job* hostJobs, const dxb_compress_params& P)
+const char* dxb_launch_bc6h(unsigned grid, cudaStream_t stream, const dxb_job* jobs, const dxb_job* hostJobs, const dxb_compress_params& P)
 {
     k_compress_bc6h<<<grid, DXB_BC6H_WARPS * 32, 0, stream>>>(jobs, hostJobs[0], P);
+    return "k_compress_bc6h";
 }
 int dxb_occupancy_bc6h()
 {

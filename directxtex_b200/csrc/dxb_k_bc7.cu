@@ -4,6 +4,7 @@
 #include <algorithm>
 #include <atomic>
 #include "dxb_launch.h"
+#include "dxb_dispatch.h"
 #include "dxb_bc7.cuh"
 #include "dxb_udiv.h"
 
@@ -49,25 +50,23 @@ __global__ void __launch_bounds__(DXB_BC7_WARPS * 32, DXB_BC7_MINB) k_compress_b
     }
 }
 
-static const size_t kBC7Smem = sizeof(dxb_bc7_scratch) * DXB_BC7_WARPS;
-static bool bc7_attr_set()
+// raises kernel K's dynamic shared memory limit to `bytes` on the first call for K; false when the runtime refused
+template <auto K>
+static bool smem_limit(size_t bytes)
 {
-    static const bool ok = (cudaFuncSetAttribute(k_compress_bc7<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kBC7Smem) == cudaSuccess) &&
-                           (cudaFuncSetAttribute(k_compress_bc7<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kBC7Smem) == cudaSuccess);
+    static const bool ok = cudaFuncSetAttribute(K, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes) == cudaSuccess;
     return ok;
 }
 
-void dxb_launch_bc7(unsigned grid, cudaStream_t stream, const dxb_job* jobs, const dxb_job* hostJobs, const dxb_compress_params& P)
-{
-    bc7_attr_set();
-    // the three-subset pass (a non-default flag) lives in its own instantiation
-    if (P.bcflags & DXB_BC_FLAGS_USE_3SUBSETS) k_compress_bc7<true><<<grid, DXB_BC7_WARPS * 32, kBC7Smem, stream>>>(jobs, hostJobs[0], P);
-    else k_compress_bc7<false><<<grid, DXB_BC7_WARPS * 32, kBC7Smem, stream>>>(jobs, hostJobs[0], P);
-}
+static const size_t kBC7Smem = sizeof(dxb_bc7_scratch) * DXB_BC7_WARPS;
 int dxb_occupancy_bc7()
 {
+    // Both direct instantiations get their limit here, at initialisation.  Under lazy module loading that also loads both, and the
+    // kernels loaded early decide where later ones land in device memory: with only <false> loaded here, C5's BC4 kernel ran 2 %
+    // slower on an H100 with identical SASS.
     int b = 0;
-    if (!bc7_attr_set() || cudaOccupancyMaxActiveBlocksPerMultiprocessor(&b, k_compress_bc7<false>, DXB_BC7_WARPS * 32, kBC7Smem) != cudaSuccess) { (void)cudaGetLastError(); b = 1; }
+    if (!smem_limit<k_compress_bc7<false>>(kBC7Smem) || !smem_limit<k_compress_bc7<true>>(kBC7Smem) ||
+        cudaOccupancyMaxActiveBlocksPerMultiprocessor(&b, k_compress_bc7<false>, DXB_BC7_WARPS * 32, kBC7Smem) != cudaSuccess) { (void)cudaGetLastError(); b = 1; }
     return b > 0 ? b : 1;
 }
 
@@ -85,7 +84,7 @@ int dxb_occupancy_bc7()
 //     shared memory, which still leaves 3 CTAs per SM resident within the 228 KB of an H100 SM;
 //   * tiles are handed out by an atomic counter (blocks with alpha cost more than opaque ones); the counter is read one tile ahead
 //     of the request, so its round trip is off the critical path too.  T.counter == nullptr: statically strided tiles.
-// Eligibility (dxb_launch_bc7_tma): RGBA32F source, full 4x4 blocks only (partial blocks need CompressBC's {0,0,0,1} replication,
+// Eligibility (launch_bc7_tma): RGBA32F source, full 4x4 blocks only (partial blocks need CompressBC's {0,0,0,1} replication,
 // which a tensor map's zero fill cannot express), 16-byte aligned rows, images of one size at a constant pointer stride.
 // The tile index is split into (image, block row, tile column) with dxb_udiv (dxb_udiv.h).
 
@@ -200,14 +199,6 @@ static dxb_encode_tiled_fn encode_tiled()
 }
 
 static const size_t kBC7TmaSmem = DXB_BC7_TILE_BYTES + 128u + sizeof(dxb_bc7_scratch) * DXB_BC7_WARPS;
-static bool bc7_tma_attr_set()
-{
-    static const bool ok = (cudaFuncSetAttribute(k_compress_bc7_tma<false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kBC7TmaSmem) == cudaSuccess) &&
-                           (cudaFuncSetAttribute(k_compress_bc7_tma<false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kBC7TmaSmem) == cudaSuccess) &&
-                           (cudaFuncSetAttribute(k_compress_bc7_tma<true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kBC7TmaSmem) == cudaSuccess) &&
-                           (cudaFuncSetAttribute(k_compress_bc7_tma<true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kBC7TmaSmem) == cudaSuccess);
-    return ok;
-}
 
 // mode: 0 = direct kernel only, 1 = TMA with the atomic tile counter, 2 = TMA with statically strided tiles, 3 = TMA with one CTA per
 // tile, 4 = automatic (default): mode 1 for batches of images, the direct kernel for a single image.  DXB200_BC7_TMA / dxb200_set_option
@@ -224,7 +215,8 @@ int dxb_bc7_get_feed()
 void dxb_bc7_set_feed(int mode) { g_bc7_feed.store((mode < 0 || mode > 4) ? 4 : mode, std::memory_order_relaxed); }
 static int bc7_tma_mode() { return dxb_bc7_get_feed(); }
 
-bool dxb_launch_bc7_tma(unsigned residentCtas, cudaStream_t stream, const dxb_job* hostJobs, const dxb_compress_params& P)
+// the TMA-fed kernel when the feed mode and the batch allow it; false = not eligible, nothing launched
+static bool launch_bc7_tma(unsigned residentCtas, cudaStream_t stream, const dxb_job* hostJobs, const dxb_compress_params& P, bool three)
 {
     int mode = bc7_tma_mode();
     if (mode == 4) mode = (P.njobs > 1u) ? 1 : 0;
@@ -244,7 +236,7 @@ bool dxb_launch_bc7_tma(unsigned residentCtas, cudaStream_t stream, const dxb_jo
         }
     }
     const dxb_encode_tiled_fn enc = encode_tiled();
-    if (!enc || !bc7_tma_attr_set()) return false;
+    if (!enc) return false;
     CUtensorMap tmap;
     const cuuint64_t dims[3] = { (cuuint64_t)j0.width * 4u, j0.height, P.njobs };
     const cuuint64_t strides[2] = { (cuuint64_t)j0.srcPitch, (cuuint64_t)srcStride };
@@ -262,21 +254,35 @@ bool dxb_launch_bc7_tma(unsigned residentCtas, cudaStream_t stream, const dxb_jo
     T.totalTiles = (uint32_t)total;
     // mode 3: one CTA per tile (the hardware CTA scheduler hands the tiles out)
     const unsigned grid = (mode == 3) ? (unsigned)total : (unsigned)std::min<uint64_t>(total, residentCtas ? residentCtas : 1u);
-    T.counter = nullptr;
-    if (mode == 1)
-    {
-        // counts the tiles handed out after the first one of every CTA (its own index); stream-ordered allocation, released after the launch
-        if (cudaMallocAsync((void**)&T.counter, sizeof(uint32_t), stream) != cudaSuccess) { (void)cudaGetLastError(); return false; }
-        cudaMemsetAsync(T.counter, 0, sizeof(uint32_t), stream);
-    }
     // the source is RGBA32F and the destination BC7_UNORM(_SRGB), so P.inF / P.outF are the PLAIN kernel's constants; only the
     // resolved sRGB flags can differ
-    const bool plain = (P.cflags == 0u);
+    return dxb_on_bool(three, [&](auto THREE) { return dxb_on_bool(P.cflags == 0u, [&](auto PLAIN)
+    {
+        constexpr bool T3 = decltype(THREE)::value, PL = decltype(PLAIN)::value;
+        if (!smem_limit<k_compress_bc7_tma<T3, PL>>(kBC7TmaSmem)) return false;
+        T.counter = nullptr;
+        if (mode == 1)
+        {
+            // counts the tiles handed out after the first one of every CTA (its own index); stream-ordered allocation, released after the launch
+            if (cudaMallocAsync((void**)&T.counter, sizeof(uint32_t), stream) != cudaSuccess) { (void)cudaGetLastError(); return false; }
+            cudaMemsetAsync(T.counter, 0, sizeof(uint32_t), stream);
+        }
+        k_compress_bc7_tma<T3, PL><<<grid, DXB_BC7_WARPS * 32, kBC7TmaSmem, stream>>>(tmap, T, P);
+        if (T.counter) cudaFreeAsync(T.counter, stream);
+        return true;
+    }); });
+}
+
+const char* dxb_launch_bc7(unsigned grid, unsigned residentCtas, cudaStream_t stream, const dxb_job* jobs, const dxb_job* hostJobs,
+                           const dxb_compress_params& P)
+{
+    // the three-subset pass (a non-default flag) lives in its own instantiations
     const bool three = (P.bcflags & DXB_BC_FLAGS_USE_3SUBSETS) != 0u;
-    if (three) { if (plain) k_compress_bc7_tma<true, true><<<grid, DXB_BC7_WARPS * 32, kBC7TmaSmem, stream>>>(tmap, T, P);
-                 else k_compress_bc7_tma<true, false><<<grid, DXB_BC7_WARPS * 32, kBC7TmaSmem, stream>>>(tmap, T, P); }
-    else if (plain) k_compress_bc7_tma<false, true><<<grid, DXB_BC7_WARPS * 32, kBC7TmaSmem, stream>>>(tmap, T, P);
-    else k_compress_bc7_tma<false, false><<<grid, DXB_BC7_WARPS * 32, kBC7TmaSmem, stream>>>(tmap, T, P);
-    if (T.counter) cudaFreeAsync(T.counter, stream);
-    return true;
+    if (launch_bc7_tma(residentCtas, stream, hostJobs, P, three)) return "k_compress_bc7_tma";
+    dxb_on_bool(three, [&](auto THREE)
+    {
+        smem_limit<k_compress_bc7<decltype(THREE)::value>>(kBC7Smem);
+        k_compress_bc7<decltype(THREE)::value><<<grid, DXB_BC7_WARPS * 32, kBC7Smem, stream>>>(jobs, hostJobs[0], P);
+    });
+    return "k_compress_bc7";
 }

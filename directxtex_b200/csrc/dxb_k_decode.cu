@@ -5,6 +5,7 @@
 //                           store path per kernel) and one vector store per block row.  No pair names an sRGB format:
 //                           an sRGB call matches its twins' pair (dxb_make_linear).
 #include "dxb_launch.h"
+#include "dxb_dispatch.h"
 #include "dxb_decode.cuh"
 
 // ---- table-driven fast paths -------------------------------------------------------------------------------------------
@@ -190,20 +191,19 @@ __global__ void __launch_bounds__(128) k_decompress_t(const dxb_job* __restrict_
     decode_body<false, SF, DF>(jobs, single, P);
 }
 
-// default targets (DirectXTexCompress.cpp:552-579): BC1/2/3/7 -> RGBA8, BC4 -> R8, BC5 -> R8G8, BC6H -> RGBA32F
-#define DXB_DEC_PAIRS(X) X(71, 28) X(74, 28) X(77, 28) X(98, 28) X(80, 61) X(81, 63) X(83, 49) X(84, 51) X(95, 2) X(96, 2)
-
-void dxb_launch_decompress(unsigned grid, cudaStream_t stream, const dxb_job* jobs, const dxb_job* hostJobs, const dxb_compress_params& P)
+const char* dxb_launch_decompress(unsigned grid, cudaStream_t stream, const dxb_job* jobs, const dxb_job* hostJobs, const dxb_compress_params& P)
 {
     // sRGB formats run their twins' kernels; the specialised kernels take only calls without an sRGB step (P.cflags == 0)
     const uint32_t sf = dxb_make_linear(P.srcFormat), df = dxb_make_linear(P.dstFormat);
 #ifndef DXB_DEC_GENERIC_ONLY
-    if (P.cflags == 0)
+    const auto hot = [&](auto SF, auto DF)
     {
-#define DXB_X(SF, DF) if (sf == SF && df == DF) { k_decompress_t<SF, DF><<<grid, 128, 0, stream>>>(jobs, hostJobs[0], P); return; }
-        DXB_DEC_PAIRS(DXB_X)
-#undef DXB_X
-    }
+        k_decompress_t<decltype(SF)::value, decltype(DF)::value><<<grid, 128, 0, stream>>>(jobs, hostJobs[0], P);
+    };
+    // default targets (DirectXTexCompress.cpp:552-579): BC1/2/3/7 -> RGBA8, BC4 -> R8, BC5 -> R8G8, BC6H -> RGBA32F
+    if (P.cflags == 0 && dxb_on_pair<71, 28, 74, 28, 77, 28, 98, 28, 80, 61, 81, 63, 83, 49, 84, 51, 95, 2, 96, 2>(sf, df, hot))
+        return "k_decompress_t";
 #endif
     k_decompress<<<grid, 128, 0, stream>>>(jobs, hostJobs[0], P);
+    return "k_decompress";
 }

@@ -12,6 +12,7 @@
 // The launchers route on the caller's format but instantiate every specialised kernel on dxb_make_linear(format): an sRGB
 // format runs its UNORM twin's kernel, with its sRGB steps taken from P.flags / P.lflags or the SRGB argument.
 #include "dxb_launch.h"
+#include "dxb_dispatch.h"
 #include "dxb_pixel.cuh"
 #include "dxb_mips.cuh"
 
@@ -41,9 +42,10 @@ __global__ void __launch_bounds__(32) k_convert_diffuse(const dxb_job* __restric
     dxb_convert_diffuse_image(P.srcFormat, P.dstFormat, P.inF, P.outF, P.flags, j.src, j.srcPitch, j.dst, j.dstPitch, j.width, j.height,
                               E, E + (j.width + 2u));
 }
-void dxb_launch_convert_diffuse(cudaStream_t stream, const dxb_job* jobs, const dxb_job* hostJobs, const dxb_convert_params& P, void* errors, uint32_t errStride)
+const char* dxb_launch_convert_diffuse(cudaStream_t stream, const dxb_job* jobs, const dxb_job* hostJobs, const dxb_convert_params& P, void* errors, uint32_t errStride)
 {
     k_convert_diffuse<<<P.njobs, 32, 0, stream>>>(jobs, hostJobs[0], P, static_cast<dxb_px*>(errors), errStride);
+    return "k_convert_diffuse";
 }
 
 __global__ void __launch_bounds__(256) k_mip_level(const dxb_mip_job* __restrict__ jobs, dxb_mip_job single, dxb_mip_params P)
@@ -147,11 +149,6 @@ __global__ void __launch_bounds__(256) k_convert_vec(const dxb_job* __restrict__
     }
 }
 
-// (29, 28) and (28, 29) both run k_convert_vec<28, 28>: the direction of their sRGB step is in P.flags
-#define DXB_CONVERT_PAIRS(X) \
-    X(61, 41) X(41, 61) X(28, 2) X(2, 28) X(10, 2) X(2, 10) X(28, 10) X(10, 28) X(28, 87) X(87, 28) \
-    X(61, 28) X(28, 61) X(11, 2) X(2, 11) X(41, 2) X(2, 41) X(29, 2) X(2, 29) X(29, 28) X(28, 29)
-
 static bool convert_vec_ok(const dxb_job* hostJobs, uint32_t njobs, uint32_t SB, uint32_t DB)
 {
     const uint32_t ppt = 16u / (SB > DB ? SB : DB);
@@ -161,7 +158,7 @@ static bool convert_vec_ok(const dxb_job* hostJobs, uint32_t njobs, uint32_t SB,
     return true;
 }
 
-void dxb_launch_convert(unsigned grid, cudaStream_t stream, const dxb_job* jobs, const dxb_job* hostJobs, const dxb_convert_params& P)
+const char* dxb_launch_convert(unsigned grid, cudaStream_t stream, const dxb_job* jobs, const dxb_job* hostJobs, const dxb_convert_params& P)
 {
     const uint32_t SB = dxb_bytes_per_pixel(P.srcFormat), DB = dxb_bytes_per_pixel(P.dstFormat);
     if (!(P.flags & DXB_FILTER_DITHER) && convert_vec_ok(hostJobs, P.njobs, SB, DB))
@@ -169,12 +166,18 @@ void dxb_launch_convert(unsigned grid, cudaStream_t stream, const dxb_job* jobs,
         const uint32_t ppt = 16u / (SB > DB ? SB : DB);
         const uint32_t chunksPerRow = (hostJobs[0].width + ppt - 1) / ppt;
         const dim3 g((chunksPerRow + 256u * DXB_CONV_UNR - 1) / (256u * DXB_CONV_UNR), hostJobs[0].height, P.njobs);
-#define DXB_X(SF, DF) if (P.srcFormat == SF && P.dstFormat == DF) { \
-            k_convert_vec<dxb_make_linear(SF), dxb_make_linear(DF)><<<g, 256, 0, stream>>>(jobs, hostJobs[0], P); return; }
-        DXB_CONVERT_PAIRS(DXB_X)
-#undef DXB_X
+        const auto hot = [&](auto SF, auto DF)
+        {
+            k_convert_vec<dxb_make_linear(decltype(SF)::value), dxb_make_linear(decltype(DF)::value)><<<g, 256, 0, stream>>>(jobs, hostJobs[0], P);
+        };
+        // the caller's (source, destination) pairs; (29, 28) and (28, 29) both run k_convert_vec<28, 28>: the direction of their
+        // sRGB step is in P.flags
+        if (dxb_on_pair<61, 41, 41, 61, 28, 2, 2, 28, 10, 2, 2, 10, 28, 10, 10, 28, 28, 87, 87, 28,
+                        61, 28, 28, 61, 11, 2, 2, 11, 41, 2, 2, 41, 29, 2, 2, 29, 29, 28, 28, 29>(P.srcFormat, P.dstFormat, hot))
+            return "k_convert_vec";
     }
     k_convert<<<grid, 256, 0, stream>>>(jobs, hostJobs[0], P);
+    return "k_convert";
 }
 
 // ------------------------------------------------------------------------------------------------ premultiplied alpha
@@ -233,7 +236,7 @@ __global__ void __launch_bounds__(256) k_pmalpha_vec(const dxb_job* __restrict__
             dxb_store_linear(FMT, drow, 0, x, 0, dxb_pmalpha_op(dxb_load_linear(FMT, srow, 0, x, 0, LF), REVERSE), LF);
 }
 
-void dxb_launch_pmalpha(unsigned grid, cudaStream_t stream, const dxb_job* jobs, const dxb_job* hostJobs, const dxb_convert_params& P)
+const char* dxb_launch_pmalpha(unsigned grid, cudaStream_t stream, const dxb_job* jobs, const dxb_job* hostJobs, const dxb_convert_params& P)
 {
     const uint32_t lf = P.flags & (DXB_FILTER_SRGB_IN | DXB_FILTER_SRGB_OUT);
     const bool srgb = (lf == (DXB_FILTER_SRGB_IN | DXB_FILTER_SRGB_OUT)), rev = (P.flags & 1u) != 0u;
@@ -243,16 +246,16 @@ void dxb_launch_pmalpha(unsigned grid, cudaStream_t stream, const dxb_job* jobs,
         const uint32_t ppt = 16u / B;
         const uint32_t chunksPerRow = (hostJobs[0].width + ppt - 1) / ppt;
         const dim3 g((chunksPerRow + 255u) / 256u, hostJobs[0].height, P.njobs);
-#define DXB_X(FMT) if (P.srcFormat == FMT) { \
-            if (rev && srgb) k_pmalpha_vec<dxb_make_linear(FMT), true, true><<<g, 256, 0, stream>>>(jobs, hostJobs[0], P); \
-            else if (rev) k_pmalpha_vec<dxb_make_linear(FMT), true, false><<<g, 256, 0, stream>>>(jobs, hostJobs[0], P); \
-            else if (srgb) k_pmalpha_vec<dxb_make_linear(FMT), false, true><<<g, 256, 0, stream>>>(jobs, hostJobs[0], P); \
-            else k_pmalpha_vec<dxb_make_linear(FMT), false, false><<<g, 256, 0, stream>>>(jobs, hostJobs[0], P); \
-            return; }
-        DXB_X(28) DXB_X(29) DXB_X(87) DXB_X(91) DXB_X(10) DXB_X(2)
-#undef DXB_X
+        const auto hot = [&](auto FMT)
+        {
+            dxb_on_bool(rev, [&](auto REV) { dxb_on_bool(srgb, [&](auto SRGB) {
+                k_pmalpha_vec<dxb_make_linear(decltype(FMT)::value), decltype(REV)::value, decltype(SRGB)::value><<<g, 256, 0, stream>>>(jobs, hostJobs[0], P);
+            }); });
+        };
+        if (dxb_on_value<28, 29, 87, 91, 10, 2>(P.srcFormat, hot)) return "k_pmalpha_vec";
     }
     k_pmalpha<<<grid, 256, 0, stream>>>(jobs, hostJobs[0], P);
+    return "k_pmalpha";
 }
 
 // ------------------------------------------------------------------------------------------------ alpha coverage
@@ -282,13 +285,15 @@ __global__ void __launch_bounds__(256) k_scale_alpha(dxb_job j, uint32_t fmt, fl
         dxb_scale_alpha_pixel(fmt, j.src + (size_t)y * j.srcPitch, j.dst + (size_t)y * j.dstPitch, x, scale);
     }
 }
-void dxb_launch_alpha_coverage(unsigned grid, cudaStream_t stream, const dxb_job& j, uint32_t fmt, float scale, float ref, unsigned long long* count)
+const char* dxb_launch_alpha_coverage(unsigned grid, cudaStream_t stream, const dxb_job& j, uint32_t fmt, float scale, float ref, unsigned long long* count)
 {
     k_alpha_coverage<<<grid, 256, 0, stream>>>(j, fmt, scale, ref, count);
+    return "k_alpha_coverage";
 }
-void dxb_launch_scale_alpha(unsigned grid, cudaStream_t stream, const dxb_job& j, uint32_t fmt, float scale)
+const char* dxb_launch_scale_alpha(unsigned grid, cudaStream_t stream, const dxb_job& j, uint32_t fmt, float scale)
 {
     k_scale_alpha<<<grid, 256, 0, stream>>>(j, fmt, scale);
+    return "k_scale_alpha";
 }
 
 // ------------------------------------------------------------------------------------------------ tiled mips
@@ -609,7 +614,16 @@ __global__ void __launch_bounds__(256) k_mip_box3(const dxb_mip_job* __restrict_
 }
 
 // ------------------------------------------------------------------------------------------------ chain launcher
-#define DXB_MIP_FORMATS(X, MODE) X(28, MODE) X(29, MODE) X(10, MODE) X(2, MODE) X(61, MODE) X(41, MODE) X(87, MODE)
+// The hot formats of the specialised mip kernels: fn(F) with F = the format's UNORM twin; false for any other format
+template <typename Fn> static bool on_mip_format(uint32_t fmt, Fn&& fn)
+{
+    return dxb_on_value<28, 29, 10, 2, 61, 41, 87>(fmt, [&](auto F) { fn(dxb_u32<dxb_make_linear(decltype(F)::value)>{}); });
+}
+// The filters of the specialised mip kernels: fn(MODE); false for any other filter
+template <typename Fn> static bool on_mip_mode(uint32_t mode, Fn&& fn)
+{
+    return dxb_on_value<DXB_FILTER_BOX, DXB_FILTER_LINEAR, DXB_FILTER_CUBIC>(mode, fn);
+}
 
 // hj: [3][items] records of levels l, l+1, l+2.  Returns false when the fused kernel does not apply (nothing launched).
 static bool launch_box3(cudaStream_t stream, const dxb_mip_job* jobs, const dxb_mip_job* hj, uint32_t items, const dxb_mip_params& P, bool srgb)
@@ -630,28 +644,17 @@ static bool launch_box3(cudaStream_t stream, const dxb_mip_job* jobs, const dxb_
     const dim3 blk(32, 8, 1);
     const dim3 g((a0.sw / 8 + 31) / 32, (a0.sh / 8 + 7) / 8, items);
     if (g.y > 65535u) return false;
-#define DXB_X(FMT, MODE) if (P.format == FMT) { \
-        if (lin) { if (srgb) k_mip_box3<dxb_make_linear(FMT), true, true><<<g, blk, 0, stream>>>(jobs, items, P); \
-                   else k_mip_box3<dxb_make_linear(FMT), false, true><<<g, blk, 0, stream>>>(jobs, items, P); } \
-        else { if (srgb) k_mip_box3<dxb_make_linear(FMT), true, false><<<g, blk, 0, stream>>>(jobs, items, P); \
-               else k_mip_box3<dxb_make_linear(FMT), false, false><<<g, blk, 0, stream>>>(jobs, items, P); } \
-        return true; }
-    DXB_MIP_FORMATS(DXB_X, 0)
-#undef DXB_X
-    return false;
+    return on_mip_format(P.format, [&](auto F) { dxb_on_bool(srgb, [&](auto SRGB) { dxb_on_bool(lin, [&](auto LIN) {
+        k_mip_box3<decltype(F)::value, decltype(SRGB)::value, decltype(LIN)::value><<<g, blk, 0, stream>>>(jobs, items, P);
+    }); }); });
 }
 
 // levels l .. l + count - 1 of every item in one launch; jobs: their [level][item] records
 static void launch_tail(cudaStream_t stream, const dxb_mip_job* jobs, uint32_t items, uint32_t count, const dxb_mip_params& P, bool srgb)
 {
-#define DXB_X(FMT, MODE) if (P.format == FMT && P.mode == MODE) { \
-        if (srgb) k_mip_tail<dxb_make_linear(FMT), MODE, true><<<items, 256, 0, stream>>>(jobs, items, count, P); \
-        else k_mip_tail<dxb_make_linear(FMT), MODE, false><<<items, 256, 0, stream>>>(jobs, items, count, P); \
-        return; }
-    DXB_MIP_FORMATS(DXB_X, DXB_FILTER_BOX)
-    DXB_MIP_FORMATS(DXB_X, DXB_FILTER_LINEAR)
-    DXB_MIP_FORMATS(DXB_X, DXB_FILTER_CUBIC)
-#undef DXB_X
+    on_mip_format(P.format, [&](auto F) { on_mip_mode(P.mode, [&](auto MODE) { dxb_on_bool(srgb, [&](auto SRGB) {
+        k_mip_tail<decltype(F)::value, decltype(MODE)::value, decltype(SRGB)::value><<<items, 256, 0, stream>>>(jobs, items, count, P);
+    }); }); });
 }
 
 // one level: hj = its records, jobs = their device copy (nullptr for a single item).  Returns the launched kernel's name.
@@ -668,27 +671,20 @@ static const char* launch_level(cudaStream_t stream, const dxb_mip_job* jobs, co
         for (uint32_t i = 0; i < P.njobs; ++i) pixAligned = pixAligned && vec_aligned(hj[i].src, hj[i].srcPitch, dxb_bytes_per_pixel(P.format));
         const dim3 gs((j0.dw + DXB_SEP_TW - 1) / DXB_SEP_TW, (j0.dh + DXB_SEP_TH - 1) / DXB_SEP_TH, P.njobs);
         const bool sepExtent = j0.sw <= DXB_SEP_MAX_EXTENT && j0.dw <= DXB_SEP_MAX_EXTENT && j0.sh <= DXB_SEP_MAX_EXTENT && j0.dh <= DXB_SEP_MAX_EXTENT;
-        if (P.mode == DXB_FILTER_CUBIC && pixAligned && sepExtent && j0.sw <= 3u * j0.dw && j0.sh <= 3u * j0.dh && gs.y <= 65535u)
-        {
-#define DXB_X(FMT, MODE) if (P.format == FMT) { \
-                if (srgb) k_mip_sep<dxb_make_linear(FMT), true><<<gs, blk, 0, stream>>>(jobs, j0, P); \
-                else k_mip_sep<dxb_make_linear(FMT), false><<<gs, blk, 0, stream>>>(jobs, j0, P); \
-                return "k_mip_sep"; }
-            DXB_MIP_FORMATS(DXB_X, 0)
-#undef DXB_X
-        }
+        if (P.mode == DXB_FILTER_CUBIC && pixAligned && sepExtent && j0.sw <= 3u * j0.dw && j0.sh <= 3u * j0.dh && gs.y <= 65535u &&
+            on_mip_format(P.format, [&](auto F) { dxb_on_bool(srgb, [&](auto SRGB) {
+                k_mip_sep<decltype(F)::value, decltype(SRGB)::value><<<gs, blk, 0, stream>>>(jobs, j0, P);
+            }); }))
+            return "k_mip_sep";
         const uint32_t rowsPerCta = (P.mode == DXB_FILTER_CUBIC) ? 8u * DXB_CUBIC_KY : 8u;
         const dim3 g((j0.dw + 31) / 32, (j0.dh + rowsPerCta - 1) / rowsPerCta, P.njobs);
         if (g.y <= 65535u)
         {
-#define DXB_X(FMT, MODE) if (P.format == FMT && P.mode == MODE) { \
-                if (srgb) k_mip_tile<dxb_make_linear(FMT), MODE, true><<<g, blk, 0, stream>>>(jobs, j0, P); \
-                else k_mip_tile<dxb_make_linear(FMT), MODE, false><<<g, blk, 0, stream>>>(jobs, j0, P); \
-                return "k_mip_tile"; }
-            DXB_MIP_FORMATS(DXB_X, DXB_FILTER_BOX)
-            DXB_MIP_FORMATS(DXB_X, DXB_FILTER_LINEAR)
-            DXB_MIP_FORMATS(DXB_X, DXB_FILTER_CUBIC)
-#undef DXB_X
+            // `special` admits only the formats and filters the dispatch lists
+            on_mip_format(P.format, [&](auto F) { on_mip_mode(P.mode, [&](auto MODE) { dxb_on_bool(srgb, [&](auto SRGB) {
+                k_mip_tile<decltype(F)::value, decltype(MODE)::value, decltype(SRGB)::value><<<g, blk, 0, stream>>>(jobs, j0, P);
+            }); }); });
+            return "k_mip_tile";
         }
     }
     const uint32_t need = (uint32_t)(((uint64_t)P.totalUnits + 255) / 256);
@@ -703,12 +699,8 @@ int32_t dxb_launch_mip_chain(cudaStream_t stream, const dxb_mip_job* jobs, const
     // The specialised kernels take BOX / LINEAR / CUBIC on the hot formats with both sRGB steps or none (the only combinations
     // a chain produces); anything else runs the generic k_mip_level.
     const bool srgb = (P.lflags == (DXB_FILTER_SRGB_IN | DXB_FILTER_SRGB_OUT));
-    bool special = false;
-#define DXB_X(FMT, MODE) special = special || P.format == FMT;
-    DXB_MIP_FORMATS(DXB_X, 0)
-#undef DXB_X
-    special = special && !genericOnly && (srgb || P.lflags == 0) &&
-              (P.mode == DXB_FILTER_BOX || P.mode == DXB_FILTER_LINEAR || P.mode == DXB_FILTER_CUBIC);
+    const auto none = [](auto) {};
+    const bool special = !genericOnly && (srgb || P.lflags == 0) && on_mip_format(P.format, none) && on_mip_mode(P.mode, none);
     // first level whose SOURCE is at most 64x64: from there on one CTA per item finishes the chain in one launch
     uint32_t tailStart = levels;
     for (uint32_t l = 1; l < levels; ++l)

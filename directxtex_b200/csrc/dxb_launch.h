@@ -20,16 +20,18 @@
 #endif
 
 // launchers: `grid` CTAs on `stream`; hostJobs = the njobs job records on the host, jobs = their device copy, or nullptr when
-// njobs == 1 (the kernel then takes hostJobs[0] by value)
-void dxb_launch_bc15(unsigned grid, cudaStream_t stream, const dxb_job* jobs, const dxb_job* hostJobs, const dxb_compress_params& P);
-void dxb_launch_bc7(unsigned grid, cudaStream_t stream, const dxb_job* jobs, const dxb_job* hostJobs, const dxb_compress_params& P);
-// TMA-fed persistent variant (RGBA32F sources of full 4x4 blocks, equal images at a constant stride); false = not eligible, nothing launched
-bool dxb_launch_bc7_tma(unsigned residentCtas, cudaStream_t stream, const dxb_job* hostJobs, const dxb_compress_params& P);
+// njobs == 1 (the kernel then takes hostJobs[0] by value).  Each enqueues one kernel and returns the name of its __global__
+// function without template arguments.
+const char* dxb_launch_bc15(unsigned grid, cudaStream_t stream, const dxb_job* jobs, const dxb_job* hostJobs, const dxb_compress_params& P);
+// RGBA32F sources of full 4x4 blocks, equal images at a constant stride: the TMA-fed persistent kernel on `residentCtas` CTAs
+// (DXB200_OPT_BC7_FEED); everything else: the direct kernel on `grid` CTAs
+const char* dxb_launch_bc7(unsigned grid, unsigned residentCtas, cudaStream_t stream, const dxb_job* jobs, const dxb_job* hostJobs,
+                           const dxb_compress_params& P);
 int dxb_bc7_get_feed();            // 0 direct kernel, 1-3 TMA-fed variants (dxb_k_bc7.cu)
 void dxb_bc7_set_feed(int mode);
-void dxb_launch_decompress(unsigned grid, cudaStream_t stream, const dxb_job* jobs, const dxb_job* hostJobs, const dxb_compress_params& P);
-void dxb_launch_bc6h(unsigned grid, cudaStream_t stream, const dxb_job* jobs, const dxb_job* hostJobs, const dxb_compress_params& P);
-void dxb_launch_convert(unsigned grid, cudaStream_t stream, const dxb_job* jobs, const dxb_job* hostJobs, const dxb_convert_params& P);
+const char* dxb_launch_decompress(unsigned grid, cudaStream_t stream, const dxb_job* jobs, const dxb_job* hostJobs, const dxb_compress_params& P);
+const char* dxb_launch_bc6h(unsigned grid, cudaStream_t stream, const dxb_job* jobs, const dxb_job* hostJobs, const dxb_compress_params& P);
+const char* dxb_launch_convert(unsigned grid, cudaStream_t stream, const dxb_job* jobs, const dxb_job* hostJobs, const dxb_convert_params& P);
 // Levels 1 .. levels-1 of `items` chains whose items all have the same sizes (a resize is a chain of two levels), each level
 // from the stored previous one.  hostJobs: the (levels - 1) x items records laid out [level - 1][item]; jobs: their device
 // copy, nullptr only when there is a single record.  P: format, mode, filter and lflags.  tri: TRIANGLE's device gather
@@ -39,10 +41,10 @@ void dxb_launch_convert(unsigned grid, cudaStream_t stream, const dxb_job* jobs,
 int32_t dxb_launch_mip_chain(cudaStream_t stream, const dxb_mip_job* jobs, const dxb_mip_job* hostJobs, uint32_t items, uint32_t levels,
                              dxb_mip_params P, const dxb_tri_axis* tri, unsigned gridCap, bool genericOnly,
                              int32_t (*launched)(const char* kernel));
-void dxb_launch_convert_diffuse(cudaStream_t stream, const dxb_job* jobs, const dxb_job* hostJobs, const dxb_convert_params& P, void* errors, uint32_t errStride);
-void dxb_launch_alpha_coverage(unsigned grid, cudaStream_t stream, const dxb_job& j, uint32_t fmt, float scale, float ref, unsigned long long* count);
-void dxb_launch_scale_alpha(unsigned grid, cudaStream_t stream, const dxb_job& j, uint32_t fmt, float scale);
-void dxb_launch_pmalpha(unsigned grid, cudaStream_t stream, const dxb_job* jobs, const dxb_job* hostJobs, const dxb_convert_params& P);
+const char* dxb_launch_convert_diffuse(cudaStream_t stream, const dxb_job* jobs, const dxb_job* hostJobs, const dxb_convert_params& P, void* errors, uint32_t errStride);
+const char* dxb_launch_alpha_coverage(unsigned grid, cudaStream_t stream, const dxb_job& j, uint32_t fmt, float scale, float ref, unsigned long long* count);
+const char* dxb_launch_scale_alpha(unsigned grid, cudaStream_t stream, const dxb_job& j, uint32_t fmt, float scale);
+const char* dxb_launch_pmalpha(unsigned grid, cudaStream_t stream, const dxb_job* jobs, const dxb_job* hostJobs, const dxb_convert_params& P);
 // resident CTAs per SM of each kernel at its block size
 int dxb_occupancy_bc15();
 int dxb_occupancy_bc7();

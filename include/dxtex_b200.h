@@ -62,8 +62,9 @@ DXB200_API void     dxb200_shutdown(void);                   /* release cached d
 DXB200_API int32_t  dxb200_device_count(void);
 DXB200_API uint64_t dxb200_launch_count(void);               /* number of kernels this library has launched so far */
 DXB200_API uint64_t dxb200_tma_launch_count(void);           /* ... of which fed by TMA tensor-map tile loads (k_compress_bc7_tma) */
-/* ... of which launched the kernel family `kernel` (e.g. "k_mip_box3", "k_mip_tail", "k_mip_sep", "k_mip_tile", "k_mip_level",
- * "k_compress_bc7"); 0 for a name that never ran.  Lets a caller or a test see which route a call took. */
+/* ... of which launched the __global__ function `kernel`, named without template arguments (e.g. "k_compress_bc15_t" and
+ * "k_compress_bc15", "k_compress_bc7_tma" and the direct "k_compress_bc7", "k_convert_vec", "k_mip_box3", "k_mip_level");
+ * 0 for a name that never ran.  Lets a caller or a test see which route a call took. */
 DXB200_API uint64_t dxb200_kernel_launch_count(const char* kernel);
 /* process-wide tuning options (no reference counterpart; results never depend on them).
  *   DXB200_OPT_BC7_FEED  how k_compress_bc7 gets RGBA32F sources made of full blocks: 0 = direct vector loads, one CTA per 16 blocks,

@@ -1,38 +1,28 @@
 """CPU mirror of tests/test_gpu_bc_formats.py: the host lock-step emulator of our kernels against the oracle over every source
 format into every BC1-BC5 target (sRGB targets and flags included), every BC source into every destination, and the
-BC7_UNORM_SRGB contract against the reference encoder; plus a check that the GPU suite's kernel pair lists hold every
-specialised instantiation in the CUDA sources.  No GPU needed."""
-import os
-import re
-
+BC7_UNORM_SRGB contract against the reference encoder; plus a check that the GPU suite's kernel pair lists name exactly the
+specialised instantiations compiled into the library.  No GPU needed."""
 import numpy as np
 import pytest
 
 from directxtex_b200 import formats as F, synth
 from tests import special_values as S, tolerance
-from tests import test_gpu_bc_formats as G
+from tests import test_gpu_bc_formats as G, test_gpu_mip_routes as R
+from tests.kernel_routes import kernel_entries
 
-CSRC = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "directxtex_b200", "csrc")
-
-
-def _instantiated_pairs(source, macro):
-    """the X(a, b) entries of `#define macro(X) ...` in a CUDA source"""
-    text = open(os.path.join(CSRC, source)).read()
-    m = re.search(r"#define\s+%s\(X\)((?:[^\n]*\\\n)*[^\n]*)" % macro, text)
-    assert m, (source, macro)
-    pairs = [(int(a), int(b)) for a, b in re.findall(r"X\((\d+),\s*(\d+)\)", m.group(1))]
-    assert pairs, (source, macro)
-    return pairs
+def twins(pairs):
+    """the instantiations the launchers run (a, b) pairs on: each format replaced by its UNORM twin (dxb_make_linear)"""
+    return {(R.TWIN.get(a, a), R.TWIN.get(b, b)) for a, b in pairs}
 
 
-def test_gpu_pair_lists_cover_every_specialised_kernel():
-    """a new k_compress_bc15_t or k_decompress_t instantiation cannot go untested: the GPU suite's lists must hold it"""
-    bc15 = _instantiated_pairs("dxb_k_bc15.cu", "DXB_BC15_PAIRS")
-    dec = _instantiated_pairs("dxb_k_decode.cu", "DXB_DEC_PAIRS")
-    assert set(bc15) <= set(G.BC15_PAIRS), sorted(set(bc15) - set(G.BC15_PAIRS))
-    assert set(bc15) <= set(G.BC15_ALIAS_CASES)
-    assert set(dec) <= set(G.DEC_PAIRS), sorted(set(dec) - set(G.DEC_PAIRS))
-    assert set(dec) <= set(G.DECOMPRESS_PAIRS)
+def test_gpu_pair_lists_equal_the_compiled_specialised_kernels():
+    """the GPU suite's pair lists name exactly the k_compress_bc15_t and k_decompress_t instantiations compiled into the library:
+    a new instantiation cannot go untested, and none is compiled that the lists do not route to"""
+    k = kernel_entries()
+    assert twins(G.BC15_PAIRS) == k["k_compress_bc15_t"], sorted(twins(G.BC15_PAIRS) ^ k["k_compress_bc15_t"])
+    assert twins(G.DEC_PAIRS) == k["k_decompress_t"], sorted(twins(G.DEC_PAIRS) ^ k["k_decompress_t"])
+    assert k["k_compress_bc15_t"] <= set(G.BC15_ALIAS_CASES)
+    assert k["k_decompress_t"] <= set(G.DECOMPRESS_PAIRS)
     # the sRGB aliases the launchers remap onto the specialised kernels are in the lists too
     for d, s in ((72, 29), (72, 91), (75, 29), (75, 91), (78, 29), (78, 91)):
         assert (d, s) in G.BC15_ALIAS_CASES

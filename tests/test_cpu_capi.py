@@ -9,8 +9,15 @@ import numpy as np
 import pytest
 
 from directxtex_b200 import capi, formats as F
+from tests.kernel_routes import kernel_entries
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+# every __global__ function of the library and how many instantiations it has: the route tests check each template's list
+# against its launcher, and this keeps a kernel that no route takes from appearing unnoticed
+KERNELS = {"k_compress_bc15_t": 28, "k_decompress_t": 10, "k_convert_vec": 17, "k_pmalpha_vec": 16, "k_mip_box3": 24, "k_mip_tail": 36,
+           "k_mip_sep": 12, "k_mip_tile": 36, "k_compress_bc7": 2, "k_compress_bc7_tma": 4, "k_compress_bc15": 1, "k_compress_bc6h": 1,
+           "k_decompress": 1, "k_convert": 1, "k_convert_diffuse": 1, "k_pmalpha": 1, "k_mip_level": 1, "k_alpha_coverage": 1,
+           "k_scale_alpha": 1}
 
 
 def header_symbols():
@@ -24,6 +31,12 @@ def test_library_exports_every_declared_symbol():
     for s in syms:
         assert hasattr(capi.lib, s), s
     assert sorted(capi.SYMBOLS) == syms
+
+
+def test_library_compiles_exactly_the_listed_kernels():
+    compiled = {name: len(args) for name, args in kernel_entries().items()}
+    assert compiled == KERNELS
+    assert sum(compiled.values()) == 194
 
 
 def test_version_and_device_count():
@@ -172,4 +185,4 @@ def test_options_round_trip_and_reject_unknown_ids():
     assert capi.kernel_launch_count("k_no_such_kernel") == 0
     assert capi.lib.dxb200_kernel_launch_count(None) == 0
     if capi.lib.dxb200_device_count() == 0:
-        assert all(capi.kernel_launch_count(k) == 0 for k in ("k_mip_box3", "k_mip_tail", "k_mip_sep", "k_mip_tile", "k_mip_level"))
+        assert all(capi.kernel_launch_count(k) == 0 for k in KERNELS)

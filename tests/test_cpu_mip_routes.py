@@ -1,8 +1,8 @@
 """CPU suite for the mip / resize kernel routes (no GPU needed).
 
-- Every specialised mip kernel instantiation that dxb_k_rows.cu compiles (family x UNORM twin of a hot format x filter mode x
-  sRGB x LIN) is reached by a case of the GPU route table in tests/test_gpu_mip_routes.py, so a new instantiation cannot go
-  untested and none is compiled that no call selects.
+- The specialised mip kernel instantiations compiled into the library (family x UNORM twin of a hot format x filter mode x
+  sRGB x LIN, read from its kernel entry points) are exactly those the cases of the GPU route table in
+  tests/test_gpu_mip_routes.py reach, so a new instantiation cannot go untested and none is compiled that no call selects.
 - k_mip_sep's fp32 tap coordinates, run as the kernel runs them, stay inside the image and inside its shared-memory tile
   buffers up to the extent limit the launcher gives it.
 - The host emulator of the mip arithmetic (the inline code every mip kernel runs) against the oracle under TEX_FILTER_SRGB,
@@ -16,43 +16,35 @@ import pytest
 
 from directxtex_b200 import formats as F
 from tests import oracle_lib, test_gpu_mip_routes as R
+from tests.kernel_routes import kernel_entries
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-MODES = {"DXB_FILTER_BOX": R.BOX, "DXB_FILTER_LINEAR": R.LIN, "DXB_FILTER_CUBIC": R.CUB, "0": 0}
 
 
 def compiled_instantiations():
-    """(routed formats, {(family, format, mode, sRGB, LIN)} of every k_mip_box3 / k_mip_tail / k_mip_sep / k_mip_tile template
-    the launcher instantiates), read from the DXB_X dispatch blocks of dxb_k_rows.cu; a template's format is the routed
-    format's UNORM twin where the launcher passes dxb_make_linear(FMT), the routed format itself where it passes FMT"""
-    src = open(os.path.join(ROOT, "directxtex_b200", "csrc", "dxb_k_rows.cu")).read()
-    fm = re.search(r"#define DXB_MIP_FORMATS\(X, MODE\)((?: X\(\d+, MODE\))+)", src)
-    formats = [int(v) for v in re.findall(r"X\((\d+), MODE\)", fm.group(1))]
+    """{(family, format, mode, sRGB, LIN)} of every k_mip_box3 / k_mip_tail / k_mip_sep / k_mip_tile kernel compiled into the
+    library, in the form of test_gpu_mip_routes.instantiations"""
     out = set()
-    for block in re.findall(r"#define DXB_X\(FMT, MODE\)(.*?)#undef DXB_X", src, re.S):
-        modes = [MODES[m] for m in re.findall(r"DXB_MIP_FORMATS\(DXB_X, (\w+)\)", block)]
-        for fam, fmtarg, args in re.findall(r"k_mip_(box3|tail|sep|tile)<(FMT|dxb_make_linear\(FMT\))((?:, \w+)*)>", block):
-            args = [a.strip() for a in args.split(",")[1:]]
-            for fmt in ({R.TWIN.get(f, f) for f in formats} if fmtarg != "FMT" else formats):
-                for mode in modes:
-                    if fam == "box3":                     # <FMT, SRGB, LIN>
-                        out.add((fam, fmt, 0, args[0] == "true", args[1] == "true"))
-                    elif fam == "sep":                    # <FMT, SRGB>
-                        out.add((fam, fmt, 0, args[0] == "true", False))
-                    else:                                 # <FMT, MODE, SRGB>
-                        assert args[0] == "MODE", args
-                        out.add((fam, fmt, mode, args[1] == "true", False))
-    return formats, out
+    for fam, insts in kernel_entries().items():
+        for args in insts:
+            if fam == "k_mip_box3":                       # <FMT, SRGB, LIN>
+                out.add(("box3", args[0], 0, args[1], args[2]))
+            elif fam == "k_mip_sep":                      # <FMT, SRGB>
+                out.add(("sep", args[0], 0, args[1], False))
+            elif fam in ("k_mip_tail", "k_mip_tile"):     # <FMT, MODE, SRGB>
+                out.add((fam[len("k_mip_"):], args[0], args[1], args[2], False))
+    return out
 
 
-def test_route_table_reaches_every_twin_instantiation():
-    formats, compiled = compiled_instantiations()
-    assert tuple(formats) == R.HOT
+def test_route_table_reaches_exactly_the_compiled_instantiations():
+    """the route table's cases reach every specialised mip kernel in the library and no other, and the kernels are compiled on
+    the UNORM twins of the hot formats only"""
+    compiled = compiled_instantiations()
     assert len(compiled) == 108, len(compiled)                 # 6 twins x (box3 4 + tail 6 + sep 2 + tile 6)
+    assert {fmt for (_, fmt, _, _, _) in compiled} == {R.TWIN.get(f, f) for f in R.HOT}
     reached = set().union(*(R.instantiations(c) for c in R.CASES))
-    assert reached <= compiled, sorted(reached - compiled)
-    missing = compiled - reached
-    assert not missing, sorted(missing)
+    assert not reached - compiled, sorted(reached - compiled)
+    assert not compiled - reached, sorted(compiled - reached)
 
 
 def test_route_table_cases_are_well_formed():

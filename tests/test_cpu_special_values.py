@@ -1,12 +1,14 @@
 """CPU suite: the host lock-step emulator of our kernels against the oracle on the special-value corpus
 (tests/special_values.py): +-0, denormals, the half overflow points, +-Inf, FLT_MAX, the rounding ties of every store, every
 non-NaN half pattern and the packed-source patterns.  Convert over every supported pair and flag family, mip chains with
-every filter, BC1-BC5.  No GPU needed."""
+every filter, BC1-BC5; and the GPU suite's lists of vector-kernel routes against the kernels compiled into the library.
+No GPU needed."""
 import numpy as np
 import pytest
 
 from directxtex_b200 import formats as F
-from tests import special_values as S
+from tests import special_values as S, test_gpu_mip_routes as R, test_gpu_special_values as V
+from tests.kernel_routes import kernel_entries
 
 PIXEL_FORMATS = sorted(F.BYTES_PER_PIXEL)
 CONVERT_FLAGS = (0, F.TEX_FILTER_FLOAT_X2BIAS, F.TEX_FILTER_RGB_COPY_RED, F.TEX_FILTER_RGB_COPY_GREEN, F.TEX_FILTER_RGB_COPY_BLUE,
@@ -22,6 +24,15 @@ def corpus_source(fmt):
         img, h = S.half_image(fmt, 256)
         return img.view(np.uint8).reshape(-1), 256, h
     return S.source_image(fmt, 256, 256), 256, 256
+
+
+def test_gpu_vector_kernel_lists_name_every_compiled_instantiation():
+    """the GPU suite's k_convert_vec pairs and k_pmalpha_vec formats, each format replaced by its UNORM twin (dxb_make_linear),
+    are exactly the instantiations compiled into the library (k_pmalpha_vec: each format in both directions, sRGB or not)"""
+    twin = lambda f: R.TWIN.get(f, f)
+    k = kernel_entries()
+    assert {(twin(a), twin(b)) for a, b in V.VEC_PAIRS} == k["k_convert_vec"]
+    assert {(twin(f), rev, srgb) for f in V.PMALPHA_VEC_FORMATS for rev in (False, True) for srgb in (False, True)} == k["k_pmalpha_vec"]
 
 
 @pytest.mark.parametrize("sf", CORPUS_SOURCES)

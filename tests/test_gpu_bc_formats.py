@@ -13,6 +13,7 @@ import pytest
 
 from directxtex_b200 import capi, formats as F, synth
 from tests import oracle_lib, special_values as S, tolerance
+from tests.kernel_routes import launched
 
 pytestmark = pytest.mark.gpu
 
@@ -23,8 +24,9 @@ COMPRESS_FLAGS = (0, F.TEX_COMPRESS_SRGB_IN, F.TEX_COMPRESS_SRGB_OUT, F.TEX_COMP
 # 22 x 14: partial blocks and rows that are not 16-byte aligned (the scalar gather); 32 x 16: full blocks, aligned rows (the vector gather)
 SIZES = ((22, 14), (32, 16))
 
-# the (target, source) pairs k_compress_bc15_t is instantiated for (DXB_BC15_PAIRS, dxb_k_bc15.cu) and the (source, target) pairs of
-# k_decompress_t (DXB_DEC_PAIRS, dxb_k_decode.cu); test_cpu_bc_formats checks that these lists hold every instantiation
+# the (target, source) pairs dxb_launch_bc15 routes to k_compress_bc15_t (dxb_k_bc15.cu) and the (source, target) pairs
+# dxb_launch_decompress routes to k_decompress_t (dxb_k_decode.cu); test_cpu_bc_formats checks them against the instantiations
+# compiled into the library
 BC15_PAIRS = [(71, 28), (71, 87), (71, 10), (71, 2), (74, 28), (74, 87), (74, 10), (74, 2), (77, 28), (77, 87), (77, 10), (77, 2),
               (80, 61), (80, 28), (80, 41), (80, 2), (81, 61), (81, 28), (81, 41), (81, 2),
               (83, 49), (83, 28), (83, 16), (83, 2), (84, 49), (84, 28), (84, 16), (84, 2)]
@@ -36,6 +38,23 @@ SRGB_TWIN = {71: 72, 74: 75, 77: 78, 98: 99, 28: 29, 87: 91}
 BC15_ALIAS_CASES = sorted({(d, s) for (df, sf) in BC15_PAIRS for d in {df, SRGB_TWIN.get(df, df)} for s in {sf, SRGB_TWIN.get(sf, sf)}})
 # decompress pairs whose sRGB sides cancel (no powf): exact, and 72 / 75 / 78 / 99 -> 29 take k_decompress_t after the remap
 EXACT_SRGB_DECOMPRESS = [(bc, df) for bc in S.SRGB_BLOCK_FORMATS for df in S.SRGB_FORMATS]
+UNORM_TWIN = {s: u for u, s in SRGB_TWIN.items()}
+BC15_KERNELS = ("k_compress_bc15_t", "k_compress_bc15")
+DEC_KERNELS = ("k_decompress_t", "k_decompress")
+
+
+def bc15_kernel(sf, df, flags):
+    """the kernel dxb_launch_bc15 takes: k_compress_bc15_t for a listed pair of UNORM twins without DITHER or UNIFORM whose
+    resolved sRGB steps cancel (the default flag set), else k_compress_bc15"""
+    hot = ((UNORM_TWIN.get(df, df), UNORM_TWIN.get(sf, sf)) in BC15_PAIRS and not flags & (F.TEX_COMPRESS_DITHER | F.TEX_COMPRESS_UNIFORM)
+           and not S.resolve_srgb(flags, sf, df))
+    return "k_compress_bc15_t" if hot else "k_compress_bc15"
+
+
+def decompress_kernel(bc, df):
+    """the kernel dxb_launch_decompress takes: k_decompress_t for a listed pair of UNORM twins without an sRGB step, else k_decompress"""
+    hot = (UNORM_TWIN.get(bc, bc), UNORM_TWIN.get(df, df)) in DEC_PAIRS and not S.resolve_srgb(0, bc, df)
+    return "k_decompress_t" if hot else "k_decompress"
 
 
 @pytest.fixture(scope="module", autouse=True)
@@ -85,7 +104,7 @@ def _fail_report(bad, total):
 @pytest.mark.parametrize("sf", PIXEL_FORMATS)
 def test_compress_every_source_into_every_bc15_target(oracle, sf):
     """Each source format into BC1-BC5 and their sRGB variants with no flag, SRGB_IN, SRGB_OUT, both, DITHER and UNIFORM, at
-    22 x 14 and 32 x 16, through the host API: bit for bit the oracle."""
+    22 x 14 and 32 x 16, through the host API: bit for bit the oracle, on the kernel bc15_kernel names."""
     bad, total = [], 0
     for df in BC15_TARGETS:
         for fl in COMPRESS_FLAGS:
@@ -93,10 +112,10 @@ def test_compress_every_source_into_every_bc15_target(oracle, sf):
                 src = compress_source(sf, df, fl, w, h, seed=w + df)
                 hr, want = oracle.compress(src, w, h, sf, df, fl)
                 assert hr == 0
-                got = capi.compress(src, w, h, sf, df, fl)
+                got, ran = launched(BC15_KERNELS, capi.compress, src, w, h, sf, df, fl)
                 total += 1
-                if S.mismatches(got, want, df).any():
-                    bad.append("%d -> %d flags %#x %dx%d" % (sf, df, fl, w, h))
+                if S.mismatches(got, want, df).any() or ran != {bc15_kernel(sf, df, fl)}:
+                    bad.append("%d -> %d flags %#x %dx%d on %s" % (sf, df, fl, w, h, sorted(ran)))
     _fail_report(bad, total)
 
 
@@ -104,7 +123,8 @@ def test_compress_every_source_into_every_bc15_target(oracle, sf):
 def test_bc15_kernel_pairs_and_srgb_aliases_on_device_layouts(oracle, df, sf):
     """Every k_compress_bc15_t pair and its sRGB aliases through the device API with the source row pitch tight, tight + 16 and
     tight + 4 and with the base pointer 4 bytes past an aligned one (the vector and the scalar paths of dxb_gather_block_t):
-    bit for bit the oracle."""
+    bit for bit the oracle, on k_compress_bc15_t where the sRGB sides agree or cancel and on k_compress_bc15 where a powf step
+    remains."""
     bad, total = [], 0
     for (w, h) in SIZES:
         src = compress_source(sf, df, 0, w, h, seed=3 * w + sf)
@@ -112,10 +132,10 @@ def test_bc15_kernel_pairs_and_srgb_aliases_on_device_layouts(oracle, df, sf):
         assert hr == 0
         row = w * F.BYTES_PER_PIXEL[sf]
         for spitch, soff in ((row, 0), (row + 16, 0), (row + 4, 0), (row, 4)):
-            got = device_call(capi.lib.dxb200_compress_device, (df, 0, 0.5, 1.0), src, w, h, sf, df, spitch, soff)
+            got, ran = launched(BC15_KERNELS, device_call, capi.lib.dxb200_compress_device, (df, 0, 0.5, 1.0), src, w, h, sf, df, spitch, soff)
             total += 1
-            if S.mismatches(got, want, df).any():
-                bad.append("%d -> %d %dx%d pitch %d offset %d" % (sf, df, w, h, spitch, soff))
+            if S.mismatches(got, want, df).any() or ran != {bc15_kernel(sf, df, 0)}:
+                bad.append("%d -> %d %dx%d pitch %d offset %d on %s" % (sf, df, w, h, spitch, soff, sorted(ran)))
     _fail_report(bad, total)
 
 
@@ -236,7 +256,8 @@ def decompress_matches(oracle, got, want, w, h, bc, df):
 def test_decompress_every_bc_source_into_every_destination(oracle, bc):
     """Each BC format (72 / 75 / 78 / 99 included) into every destination at 13 x 9 and 32 x 16, random and encoded streams,
     through the host API and through the device API with the destination pitch padded to 16 bytes + 16 (the table-driven and
-    the row-store paths of k_decompress_t) and with pitch + 4 at a base pointer 4 bytes off (the scalar stores)."""
+    the row-store paths of k_decompress_t) and with pitch + 4 at a base pointer 4 bytes off (the scalar stores); each call on
+    the kernel decompress_kernel names."""
     bad, total = [], 0
     for (w, h) in ((13, 9), (32, 16)):
         for kind, blocks in bc_streams(oracle, bc, w, h, seed=bc * 31 + w):
@@ -244,15 +265,15 @@ def test_decompress_every_bc_source_into_every_destination(oracle, bc):
                 hr, want = oracle.decompress(blocks, w, h, bc, df)
                 assert hr == 0
                 row = w * F.BYTES_PER_PIXEL[df]
-                outs = (("host", capi.decompress(blocks, w, h, bc, df)),
+                outs = (("host", launched(DEC_KERNELS, capi.decompress, blocks, w, h, bc, df)),
                         ("device pitch %d" % (_round16(row) + 16),
-                         device_call(capi.lib.dxb200_decompress_device, (df,), blocks, w, h, bc, df, dpitch=_round16(row) + 16)),
+                         launched(DEC_KERNELS, device_call, capi.lib.dxb200_decompress_device, (df,), blocks, w, h, bc, df, dpitch=_round16(row) + 16)),
                         ("device pitch %d offset 4" % (row + 4),
-                         device_call(capi.lib.dxb200_decompress_device, (df,), blocks, w, h, bc, df, dpitch=row + 4, doff=4)))
-                for path, got in outs:
+                         launched(DEC_KERNELS, device_call, capi.lib.dxb200_decompress_device, (df,), blocks, w, h, bc, df, dpitch=row + 4, doff=4)))
+                for path, (got, ran) in outs:
                     total += 1
-                    if not decompress_matches(oracle, got, want, w, h, bc, df):
-                        bad.append("%d -> %d %s %dx%d %s" % (bc, df, kind, w, h, path))
+                    if not decompress_matches(oracle, got, want, w, h, bc, df) or ran != {decompress_kernel(bc, df)}:
+                        bad.append("%d -> %d %s %dx%d %s on %s" % (bc, df, kind, w, h, path, sorted(ran)))
     _fail_report(bad, total)
 
 

@@ -29,7 +29,7 @@ from tests import oracle_lib
 BOX, LIN, CUB, TRI, PT = F.TEX_FILTER_BOX, F.TEX_FILTER_LINEAR, F.TEX_FILTER_CUBIC, F.TEX_FILTER_TRIANGLE, F.TEX_FILTER_POINT
 SRGB, SRGB_IN = F.TEX_FILTER_SRGB, F.TEX_FILTER_SRGB_IN
 MODE_MASK = 0xF00000
-HOT = (28, 29, 10, 2, 61, 41, 87)                   # DXB_MIP_FORMATS
+HOT = (28, 29, 10, 2, 61, 41, 87)                   # on_mip_format in dxb_k_rows.cu
 FAMILIES = ("k_mip_box3", "k_mip_tail", "k_mip_sep", "k_mip_tile", "k_mip_level")
 
 

@@ -8,8 +8,10 @@ import pytest
 
 from directxtex_b200 import capi, formats as F, synth
 from tests import golden_util, oracle_lib, tolerance
+from tests.kernel_routes import launched
 
 pytestmark = pytest.mark.gpu
+BC7_KERNELS = ("k_compress_bc7_tma", "k_compress_bc7")
 
 
 @pytest.fixture(scope="module", autouse=True)
@@ -345,7 +347,8 @@ def test_bc7_tma_fed_kernel_equals_emulator(emul):
     """RGBA32F sources made of full 4x4 blocks go through k_compress_bc7_tma (persistent CTAs, one TMA box of 64 x 4 pixels per
     tile): widths that end in a partial, zero-filled tile, a single tile, more tiles than resident CTAs, the three-subset
     instantiation, and an array at a constant pointer stride (rank-3 tensor map) on the device API -- all must equal the emulator,
-    as must a source whose rows are not 16-byte aligned for the tensor map (pitch padded by 4 bytes: the direct kernel)."""
+    as must a source whose rows are not 16-byte aligned for the tensor map (pitch padded by 4 bytes: the direct kernel).  Each
+    call reports the kernel it ran: k_compress_bc7_tma, or k_compress_bc7 for the padded pitch."""
     torch = pytest.importorskip("torch")
     rng = np.random.default_rng(23)
     before, feed = capi.tma_launch_count(), capi.lib.dxb200_get_option(capi.OPT_BC7_FEED)
@@ -362,9 +365,10 @@ def _tma_cases(emul, torch, rng):
         img = rng.random((h, w, 4), dtype=np.float32)
         if w == 100:
             img[:, :48, 3] = 1.0
-        got = capi.compress(img, w, h, 2, 98, flags)
+        got, ran = launched(BC7_KERNELS, capi.compress, img, w, h, 2, 98, flags)
         he, em = emul.compress(img, w, h, 2, 98, flags)
         assert he == 0 and np.array_equal(got, em), (w, h, flags)
+        assert ran == {"k_compress_bc7_tma"}, (w, h, flags, ran)
     w, h, n = 72, 20, 3
     imgs = rng.random((n, h, w, 4), dtype=np.float32)
     st = C.c_void_p(torch.cuda.current_stream().cuda_stream)
@@ -377,7 +381,8 @@ def _tma_cases(emul, torch, rng):
         d_out = torch.zeros(n * sl, dtype=torch.uint8, device="cuda")
         s = capi.images([capi.Image(w, h, 2, pitch, pitch * h, d_in.data_ptr() + i * pitch * h) for i in range(n)])
         d = capi.images([capi.Image(w, h, 98, row, sl, d_out.data_ptr() + i * sl) for i in range(n)])
-        assert capi.lib.dxb200_compress_device(s, n, 98, 0, 0.5, 1.0, d, st) == 0
+        hr, ran = launched(BC7_KERNELS, capi.lib.dxb200_compress_device, s, n, 98, 0, 0.5, 1.0, d, st)
+        assert hr == 0 and ran == {"k_compress_bc7" if pad else "k_compress_bc7_tma"}, (pad, ran)
         torch.cuda.synchronize()
         out = d_out.cpu().numpy().reshape(n, sl)
         for i in range(n):
@@ -411,7 +416,8 @@ def test_bc7_every_feed_equals_emulator(emul, feed, flags, df):
     whole tiles, and an array at a constant stride, all equal the emulator.  One image has 16 x 128 = 2048 tiles, more than a launch
     has resident CTAs (132 SMs x at most 3 CTAs of ~76 KB shared memory), so under feeds 1 and 2 every CTA takes further tiles after
     its first from the counter or the grid stride; a skipped, repeated or misplaced tile leaves blocks that differ from the
-    emulator.  The TMA launch counter moves for single images exactly under feeds 1-3, and for the array under feeds 1-4."""
+    emulator.  The TMA launch counter moves for single images exactly under feeds 1-3, and for the array under feeds 1-4; every
+    other call runs the direct k_compress_bc7."""
     rng = np.random.default_rng(1000 + 10 * feed + df + (flags != 0))
     old = capi.lib.dxb200_get_option(capi.OPT_BC7_FEED)
     assert capi.lib.dxb200_set_option(capi.OPT_BC7_FEED, feed) == 0
@@ -425,18 +431,20 @@ def test_bc7_every_feed_equals_emulator(emul, feed, flags, df):
                 he, em = emul.compress(img, w, h, 2, df, flags)
                 assert he == 0
             before = capi.tma_launch_count()
-            got = capi.compress(img, w, h, 2, df, flags)
+            got, ran = launched(BC7_KERNELS, capi.compress, img, w, h, 2, df, flags)
             moved = capi.tma_launch_count() - before
             assert np.array_equal(got, em), ("single", w, h)
             assert (moved > 0) == (feed in (1, 2, 3)), ("single", w, h, moved)
+            assert ran == {"k_compress_bc7_tma" if feed in (1, 2, 3) else "k_compress_bc7"}, ("single", w, h, ran)
         imgs = [rng.random((20, 72, 4), dtype=np.float32) for _ in range(3)]
         before = capi.tma_launch_count()
-        outs = capi.compress_array(imgs, 72, 20, 2, df, flags)
+        outs, ran = launched(BC7_KERNELS, capi.compress_array, imgs, 72, 20, 2, df, flags)
         moved = capi.tma_launch_count() - before
         for i, (img, got) in enumerate(zip(imgs, outs)):
             he, em = emul.compress(img, 72, 20, 2, df, flags)
             assert he == 0 and np.array_equal(got, em), ("array", i)
         assert (moved > 0) == (feed != 0), ("array", moved)
+        assert ran == {"k_compress_bc7_tma" if feed != 0 else "k_compress_bc7"}, ("array", ran)
     finally:
         capi.lib.dxb200_set_option(capi.OPT_BC7_FEED, old)
 

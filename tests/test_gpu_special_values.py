@@ -10,6 +10,7 @@ import pytest
 
 from directxtex_b200 import capi, formats as F
 from tests import special_values as S
+from tests.kernel_routes import launched
 
 pytestmark = pytest.mark.gpu
 
@@ -17,9 +18,13 @@ PIXEL_FORMATS = sorted(F.BYTES_PER_PIXEL)
 CORPUS_SOURCES = S.F32_FORMATS + S.F16_FORMATS + S.PACKED16 + (26, 67)
 CONVERT_FLAGS = (0, F.TEX_FILTER_FLOAT_X2BIAS, F.TEX_FILTER_RGB_COPY_RED, F.TEX_FILTER_RGB_COPY_GREEN, F.TEX_FILTER_RGB_COPY_BLUE,
                  F.TEX_FILTER_DITHER, F.TEX_FILTER_DITHER_DIFFUSION, F.TEX_FILTER_SRGB_IN, F.TEX_FILTER_SRGB_OUT, F.TEX_FILTER_SRGB)
-# the pairs k_convert_vec is instantiated for (DXB_CONVERT_PAIRS, dxb_k_rows.cu)
+# the (source, destination) pairs dxb_launch_convert routes to k_convert_vec and the formats dxb_launch_pmalpha routes to
+# k_pmalpha_vec (dxb_k_rows.cu); test_cpu_special_values checks them against the instantiations compiled into the library
 VEC_PAIRS = [(61, 41), (41, 61), (28, 2), (2, 28), (10, 2), (2, 10), (28, 10), (10, 28), (28, 87), (87, 28),
              (61, 28), (28, 61), (11, 2), (2, 11), (41, 2), (2, 41), (29, 2), (2, 29), (29, 28), (28, 29)]
+PMALPHA_VEC_FORMATS = (28, 29, 87, 91, 10, 2)
+CONVERT_KERNELS = ("k_convert_vec", "k_convert", "k_convert_diffuse")
+PMALPHA_KERNELS = ("k_pmalpha_vec", "k_pmalpha")
 
 
 @pytest.fixture(scope="module", autouse=True)
@@ -85,8 +90,8 @@ def _round16(n):
 def test_convert_every_pair_widths(oracle, sf):
     """Every (src, dst) pair at widths 1, PPT-1, PPT, PPT+1, 257 and 1031 (PPT = pixels per 16-byte vector of the wider side),
     3 rows, through the device API with both row pitches rounded up to 16 bytes.  Per convert_vec_ok that takes k_convert_vec
-    for the DXB_CONVERT_PAIRS pairs -- its vector body, its ragged end (widths that are not a multiple of PPT) and, at 1031
-    pixels of 16 bytes, two CTAs per row -- and k_convert for every other pair."""
+    for the VEC_PAIRS pairs -- its vector body, its ragged end (widths that are not a multiple of PPT) and, at 1031 pixels of
+    16 bytes, two CTAs per row -- and k_convert for every other pair."""
     for df in PIXEL_FORMATS:
         if df == sf:
             continue
@@ -96,8 +101,10 @@ def test_convert_every_pair_widths(oracle, sf):
             src = S.source_image(sf, w, h, seed=w)
             hr, want = oracle.convert(src, w, h, sf, df)
             assert hr == 0
-            got = convert_device(src, w, h, sf, df, 0, _round16(w * F.BYTES_PER_PIXEL[sf]), _round16(w * F.BYTES_PER_PIXEL[df]))
+            got, ran = launched(CONVERT_KERNELS, convert_device, src, w, h, sf, df, 0, _round16(w * F.BYTES_PER_PIXEL[sf]),
+                                _round16(w * F.BYTES_PER_PIXEL[df]))
             check(oracle, got, want, w, h, sf, df, 0, "convert %d -> %d width %d" % (sf, df, w))
+            assert ran == {"k_convert_vec" if (sf, df) in VEC_PAIRS else "k_convert"}, (sf, df, w, ran)
 
 
 @pytest.mark.parametrize("sf,df", VEC_PAIRS)
@@ -113,8 +120,9 @@ def test_convert_vec_pairs_vector_and_generic_kernel(oracle, sf, df):
         hr, want = oracle.convert(src, w, h, sf, df)
         assert hr == 0
         for pad in (0, 4):
-            got = convert_device(src, w, h, sf, df, 0, _round16(w * sb) + pad, _round16(w * db) + pad)
+            got, ran = launched(CONVERT_KERNELS, convert_device, src, w, h, sf, df, 0, _round16(w * sb) + pad, _round16(w * db) + pad)
             check(oracle, got, want, w, h, sf, df, 0, "convert %d -> %d width %d pad %d" % (sf, df, w, pad))
+            assert ran == {"k_convert_vec" if pad == 0 else "k_convert"}, (sf, df, w, pad, ran)
 
 
 def _corpus_source(fmt):
@@ -130,8 +138,9 @@ def _corpus_source(fmt):
 def test_convert_flags_special_values(oracle, sf):
     """The fp32 corpus (R32G32B32A32 / R32G32B32 / R32G32 / R32), every half pattern and the packed-source patterns to every
     destination with each flag family, through the host API.  Refused pairs (dithered stores to 85 / 86 / 115) must be
-    refused.  sRGB with error diffusion is left to the CPU suite: diffusion carries powf's last-place difference between
-    glibc and CUDA into later pixels, beyond the one-code rule."""
+    refused.  DITHER_DIFFUSION runs k_convert_diffuse, every other flag one of the other two convert kernels.  sRGB with error
+    diffusion is left to the CPU suite: diffusion carries powf's last-place difference between glibc and CUDA into later
+    pixels, beyond the one-code rule."""
     src, w, h = _corpus_source(sf)
     for df in PIXEL_FORMATS:
         if df == sf:
@@ -146,8 +155,10 @@ def test_convert_flags_special_values(oracle, sf):
                 continue
             hr, want = oracle.convert(src, w, h, sf, df, fl)
             assert hr == 0
-            got = capi.convert(src, w, h, sf, df, fl)
+            got, ran = launched(CONVERT_KERNELS, capi.convert, src, w, h, sf, df, fl)
             check(oracle, got, want, w, h, sf, df, fl, "convert %d -> %d flags %#x" % (sf, df, fl))
+            diffuse = bool(fl & F.TEX_FILTER_DITHER_DIFFUSION)
+            assert ran and ("k_convert_diffuse" in ran) == diffuse and (not diffuse or len(ran) == 1), (sf, df, hex(fl), ran)
 
 
 # ---- mips, resize, premultiplied alpha, alpha coverage ---------------------------------------------------------------------
@@ -207,6 +218,34 @@ def test_premultiply_alpha_special_values(oracle, flags):
             hr, want = oracle.premultiply_alpha(src, w, h, fmt, flags)
             assert hr == 0
             S.assert_same(capi.premultiply_alpha(src, w, h, fmt, flags), want, fmt, "pmalpha fmt %d %dx%d flags %d" % (fmt, w, h, flags))
+
+
+# (format, TEX_PMALPHA flags, resolved sRGB steps): both directions (0x2 = REVERSE); sRGB steps both (29 / 91, or
+# TEX_PMALPHA_SRGB = 0x3000000), none (no flag, or IGNORE_SRGB = 0x1) or one (0x1000000 / 0x2000000: k_pmalpha only)
+PMALPHA_ROUTES = [(28, 0, 0), (28, 2, 0), (28, 0x3000000, 3), (28, 0x3000002, 3), (28, 0x1000000, 1), (28, 0x2000002, 2),
+                  (29, 0, 3), (29, 2, 3), (29, 1, 0), (29, 3, 0), (87, 0x3000002, 3), (91, 0, 3), (91, 3, 0),
+                  (10, 0, 0), (10, 2, 0), (2, 0, 0), (2, 2, 0)]
+
+
+@pytest.mark.parametrize("fmt,flags,srgb", PMALPHA_ROUTES)
+def test_premultiply_alpha_vector_and_generic_kernel(oracle, fmt, flags, srgb):
+    """257 x 3 through the device API with both row pitches rounded up to 16 bytes (k_pmalpha_vec when the resolved sRGB steps
+    are both or none, k_pmalpha for one) and padded by 4 more bytes (k_pmalpha): the oracle bit for bit, or within one code
+    where an sRGB step runs powf."""
+    w, h = 257, 3
+    pitch = _round16(w * F.BYTES_PER_PIXEL[fmt])
+    src = _float_source(fmt, w, h, seed=fmt + flags)
+    hr, want = oracle.premultiply_alpha(src, w, h, fmt, flags)
+    assert hr == 0
+    for pad in (0, 4):
+        (got,), ran = launched(PMALPHA_KERNELS, device_call, capi.lib.dxb200_premultiply_alpha_device, (flags,), [src], [(w, h)], fmt, fmt,
+                               [pitch + pad], [pitch + pad])
+        ctx = "pmalpha fmt %d flags %#x pad %d" % (fmt, flags, pad)
+        if srgb:
+            assert np.abs(got.astype(np.int32) - want.astype(np.int32)).max() <= 1, ctx
+        else:
+            S.assert_same(got, want, fmt, ctx)
+        assert ran == {"k_pmalpha_vec" if pad == 0 and srgb in (0, 3) else "k_pmalpha"}, (ctx, ran)
 
 
 def test_scale_mipmaps_alpha_for_coverage_threshold_values(oracle):
