@@ -696,6 +696,7 @@ int32_t dxb200_compress_device(const dxb200_image* src, size_t nimages, uint32_t
     CompressPlan plan;
     int32_t hr = plan_compress(src, nimages, dstFormat, flags, threshold, dst, &plan);
     if (hr != DXB_S_OK) return hr;
+    if (!bc_pointers_ok(dst, nimages)) return DXB_E_INVALIDARG;
     DevScope scope;
     hr = scope.enter(src[0].pixels);
     if (hr != DXB_S_OK) return hr;
@@ -734,6 +735,7 @@ int32_t dxb200_decompress_device(const dxb200_image* src, size_t nimages, uint32
     dxb_compress_params P;
     int32_t hr = plan_decompress(src, nimages, dstFormat, dst, &P);
     if (hr != DXB_S_OK) return hr;
+    if (!bc_pointers_ok(src, nimages)) return DXB_E_INVALIDARG;
     DevScope scope;
     hr = scope.enter(src[0].pixels);
     if (hr != DXB_S_OK) return hr;

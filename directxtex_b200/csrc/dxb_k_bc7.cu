@@ -50,11 +50,19 @@ __global__ void __launch_bounds__(DXB_BC7_WARPS * 32, DXB_BC7_MINB) k_compress_b
     }
 }
 
-// raises kernel K's dynamic shared memory limit to `bytes` on the first call for K; false when the runtime refused
+// raises kernel K's dynamic shared memory limit to `bytes` on the current device, on the first call for K there; false when the
+// runtime refused.  A function attribute belongs to the module loaded in one device's context, so every device needs its own call.
 template <auto K>
 static bool smem_limit(size_t bytes)
 {
-    static const bool ok = cudaFuncSetAttribute(K, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes) == cudaSuccess;
+    constexpr int kDevices = 64;
+    static std::atomic<int> state[kDevices];             // per device ordinal: 0 = not set yet, 1 = raised, -1 = refused
+    int dev = -1;
+    if (cudaGetDevice(&dev) != cudaSuccess) { (void)cudaGetLastError(); dev = -1; }
+    if (dev >= 0 && dev < kDevices && state[dev].load(std::memory_order_relaxed) != 0) return state[dev].load(std::memory_order_relaxed) > 0;
+    const bool ok = cudaFuncSetAttribute(K, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes) == cudaSuccess;
+    if (!ok) (void)cudaGetLastError();
+    if (dev >= 0 && dev < kDevices) state[dev].store(ok ? 1 : -1, std::memory_order_relaxed);
     return ok;
 }
 

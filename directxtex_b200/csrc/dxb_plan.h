@@ -42,6 +42,24 @@ size_t count_mips(size_t w, size_t h)
     return n;
 }
 
+// The kernels move whole blocks with 8- or 16-byte loads and stores, so every block row of a BC image they touch must start on a
+// multiple of the block size.  Host images are staged into 256-byte aligned device buffers at the caller's row pitch, so for them
+// only the row pitch matters (bc_pitch_ok, checked by every plan); a _device call also passes its pixel pointer straight to the
+// kernel (bc_pointers_ok).  A layout that breaks the rule would fault the kernel; the call is refused with E_INVALIDARG instead.
+bool bc_pitch_ok(const dxb200_image& im)
+{
+    const size_t bs = dxb_bc_block_bytes(im.format);
+    return bs == 0 || im.rowPitch % bs == 0;
+}
+
+bool bc_pointers_ok(const dxb200_image* im, size_t n)
+{
+    for (size_t i = 0; i < n; ++i)
+        if (const size_t bs = dxb_bc_block_bytes(im[i].format))
+            if (reinterpret_cast<uintptr_t>(im[i].pixels) % bs) return false;
+    return true;
+}
+
 // ---- Compress ---------------------------------------------------------------------------------
 struct CompressPlan { dxb_compress_params P; bool bc7, bc6h; };
 
@@ -59,6 +77,7 @@ int32_t plan_compress(const dxb200_image* src, size_t n, uint32_t dstFormat, uin
         if (src[i].format != srcFormat || dst[i].format != dstFormat) return DXB_E_INVALIDARG;
         if (src[i].width != dst[i].width || src[i].height != dst[i].height) return DXB_E_FAIL;
         if (!src[i].width || !src[i].height || src[i].width > 0xFFFFFFFFull || src[i].height > 0xFFFFFFFFull) return DXB_E_INVALIDARG;
+        if (!bc_pitch_ok(dst[i])) return DXB_E_INVALIDARG;
     }
     dxb_compress_params& P = plan->P;
     P.srcFormat = srcFormat; P.dstFormat = dstFormat;
@@ -86,6 +105,7 @@ int32_t plan_decompress(const dxb200_image* src, size_t n, uint32_t dstFormat, c
         if (src[i].format != srcFormat || dst[i].format != dstFormat) return DXB_E_INVALIDARG;
         if (src[i].width != dst[i].width || src[i].height != dst[i].height) return DXB_E_FAIL;
         if (!src[i].width || !src[i].height || src[i].width > 0xFFFFFFFFull || src[i].height > 0xFFFFFFFFull) return DXB_E_INVALIDARG;
+        if (!bc_pitch_ok(src[i])) return DXB_E_INVALIDARG;
     }
     memset(P, 0, sizeof(*P));
     P->srcFormat = srcFormat; P->dstFormat = dstFormat;

@@ -93,15 +93,19 @@ DXB200_API int32_t  dxb200_calculate_mip_levels(size_t width, size_t height, siz
  * (DirectXTexCompress.cpp:632-845; block walk CompressBC :72-205).
  *   flags     = TEX_COMPRESS_FLAGS (DirectXTex.h:887-917); TEX_COMPRESS_PARALLEL is accepted and ignored
  *   threshold = BC1 alpha threshold (TEX_THRESHOLD_DEFAULT 0.5)
- * src[i] and dst[i] must have equal width/height; dst[i].format == dstFormat, pitches per dxb200_compute_pitch. */
+ * src[i] and dst[i] must have equal width/height; dst[i].format == dstFormat, pitches per dxb200_compute_pitch.
+ * The row pitch of a BC image (the destination here, the source of a decompress) must be a multiple of its block size (8 bytes
+ * for BC1 / BC4, 16 for the others), and so must its pixel pointer in the _device variants: the kernels move whole blocks.
+ * Other layouts are refused with E_INVALIDARG. */
 DXB200_API int32_t  dxb200_compress(const dxb200_image* src, size_t nimages, uint32_t dstFormat,
                          uint32_t flags, float threshold, float alphaWeight, const dxb200_image* dst);
 DXB200_API int32_t  dxb200_compress_device(const dxb200_image* src, size_t nimages, uint32_t dstFormat,
                                 uint32_t flags, float threshold, float alphaWeight, const dxb200_image* dst, void* stream);
 /* CompressEx / ConvertEx status callback (DirectXTex.h:929-944; DirectXTexCompress.cpp:115-121, 356-360, 785-837): called with
- * (done, total) before every band of work rows goes to the device -- pixel rows of a single image, images of an array --
- * and with (total, total) at the end; returning 0 stops the call between bands with E_ABORT (0x80004004).  With several
- * devices the callback is serialised but may come from worker threads. */
+ * (done, total) before every chunk of bands goes to the device -- pixel rows of a single image, images of an array, done
+ * before that chunk (a chunk holds whole bands of work rows, about 48 MiB of source and destination) -- and with (total, total)
+ * at the end; returning 0 stops the call between chunks with E_ABORT (0x80004004).  With several devices each device reports
+ * its own chunks, so the values need not rise; the callback is serialised but may come from worker threads. */
 typedef int (*dxb200_status_fn)(size_t done, size_t total, void* user);
 DXB200_API int32_t  dxb200_compress_ex(const dxb200_image* src, size_t nimages, uint32_t dstFormat, uint32_t flags, float threshold,
                             float alphaWeight, const dxb200_image* dst, dxb200_status_fn status, void* user);
