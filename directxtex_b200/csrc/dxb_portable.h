@@ -117,6 +117,14 @@ DXB_DEV uint32_t dxb_popc16(uint32_t v)
     return (uint32_t)__builtin_popcount(v & 0xFFFFu);
 #endif
 }
+DXB_DEV uint32_t dxb_popc64(uint64_t v)
+{
+#if DXB_ON_DEVICE
+    return (uint32_t)__popcll(v);
+#else
+    return (uint32_t)__builtin_popcountll(v);
+#endif
+}
 DXB_DEV float dxb_uint_as_float(uint32_t u)
 {
 #if DXB_ON_DEVICE

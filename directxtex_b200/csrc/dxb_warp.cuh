@@ -75,6 +75,16 @@ DXB_DEV uint32_t dxb_warp_or_u32(const uint32_t* v)
     return m;
 #endif
 }
+DXB_DEV uint32_t dxb_warp_max_u32(const uint32_t* v)
+{
+#if DXB_ON_DEVICE
+    return __reduce_max_sync(DXB_FULLMASK, v[0]);
+#else
+    uint32_t m = v[0];
+    for (int l = 1; l < 32; ++l) m = (v[l] > m) ? v[l] : m;
+    return m;
+#endif
+}
 DXB_DEV uint64_t dxb_warp_min_u64(const uint64_t* v)
 {
 #if DXB_ON_DEVICE
@@ -149,5 +159,50 @@ DXB_DEV void dxb_half_gather_u32(const uint32_t* v, const uint32_t* src, uint32_
     uint32_t tmp[32];
     for (int l = 0; l < 32; ++l) tmp[l] = v[(l & 16) | (int)(src[l] & 15u)];
     for (int l = 0; l < 32; ++l) out[l] = tmp[l];
+#endif
+}
+// four predicates per lane (bit j of flags[lane], j < 4) to one 64-bit mask per half: bit 16 j + h of out[lane] = predicate j of the
+// lane whose index inside the half of `lane` is h
+DXB_DEV void dxb_half_ballot4_u64(const uint32_t* flags, uint64_t* out)
+{
+#if DXB_ON_DEVICE
+    const uint32_t sh = threadIdx.x & 16u;
+    uint64_t m = 0;
+    #pragma unroll
+    for (int j = 0; j < 4; ++j) m |= (uint64_t)((__ballot_sync(DXB_FULLMASK, (flags[0] >> j) & 1u) >> sh) & 0xFFFFu) << (16 * j);
+    out[0] = m;
+#else
+    for (int h = 0; h < 32; h += 16)
+    {
+        uint64_t m = 0;
+        for (int l = 0; l < 16; ++l)
+            for (int j = 0; j < 4; ++j) m |= (uint64_t)((flags[h + l] >> j) & 1u) << (16 * j + l);
+        for (int l = 0; l < 16; ++l) out[h + l] = m;
+    }
+#endif
+}
+
+// lane-private bit arithmetic: position of the n-th (from 0) set bit of m, 64 when m has n or fewer set bits
+DXB_DEV uint32_t dxb_nth_set_bit_u64(uint64_t m, uint32_t n)
+{
+#if DXB_ON_DEVICE
+    const uint32_t clo = (uint32_t)__popc((uint32_t)m);
+    const bool hi = (n >= clo);
+    uint32_t w = hi ? (uint32_t)(m >> 32) : (uint32_t)m, pos = hi ? 32u : 0u;
+    n = hi ? n - clo : n;
+    if (n >= (uint32_t)__popc(w)) return 64u;
+    // binary search: the wanted bit lies in w above `pos`, with n set bits of w below it
+    #pragma unroll
+    for (uint32_t s = 16; s >= 1; s >>= 1)
+    {
+        const uint32_t c = (uint32_t)__popc(w & ((1u << s) - 1u));
+        const bool up = (n >= c);
+        n = up ? n - c : n; w = up ? w >> s : w; pos = up ? pos + s : pos;
+    }
+    return pos;
+#else
+    for (uint32_t b = 0; b < 64; ++b)
+        if ((m >> b) & 1u) { if (n == 0u) return b; --n; }
+    return 64u;
 #endif
 }

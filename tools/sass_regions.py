@@ -32,8 +32,10 @@ REGIONS = [
     ("tma loop + convert", "dxb_k_bc7.cu", "k_compress_bc7_tma(const", None),
     ("direct loop + convert", "dxb_k_bc7.cu", "k_compress_bc7(const", None),
     ("s1 moments (mma)", "dxb_bc7.cuh", "DXB_DEV void dxb_bc7_build_moments", None),
-    ("s1 h1", "dxb_bc7.cuh", "DXB_DEV void dxb_bc7_subset_axes", None),
-    ("s1 h1", "dxb_bc7.cuh", "DXB_DEV float dxb_bc7_shape_h1", None),
+    ("s1 h1 part A (axes)", "dxb_bc7.cuh", "DXB_DEV void dxb_bc7_subset_axes", None),
+    ("s1 h1 part A (axes)", "dxb_bc7.cuh", "DXB_DEV void dxb_bc7_shape_axes", None),
+    ("s1 h1 part B (quantisation)", "dxb_bc7.cuh", "DXB_DEV float dxb_bc7_shape_qerr", None),
+    ("s1 h1 part B (quantisation)", "dxb_bc7.cuh", "DXB_DEV float dxb_bc7_shape_h1", None),
     ("s1 select", "dxb_bc7.cuh", "// ---- stage 1: moment table", "// ---- stage 2:"),
     ("s2 tasks + rotation", "dxb_bc7.cuh", "// ---- stage 2:", "// ---- stage 3:"),
     ("s2 rotation", "dxb_bc7.cuh", "DXB_DEV float dxb_bc7_rotation_estimate1", "// -----"),
