@@ -207,6 +207,19 @@ DXB_DEV void dxb_bc6h_fit(const dxb_px* px, uint32_t mask, uint32_t ib, int anch
     }
 }
 
+#if !DXB_ON_DEVICE
+// test-infrastructure hooks of the host emulator only (tests/bc67_blocks/record_host.cpp), null / -1 by default.
+// Record: per half, the winning mode index and shape (0 for one region), the quantised endpoints A0 B0 A1 B1 before the delta
+// transform, the 16 indices and the INT-domain value each pixel's index selects from the exact palette (what the decoder must return).
+struct dxb_bc6h_dbg_block { int32_t mode, shape, wq[12], idx[16], texel[16][3]; };
+static thread_local dxb_bc6h_dbg_block* dxb_bc6h_dbg_rec = nullptr;                 // [2]: half 0, half 1
+// Force, per half: mode (0..13) leaves dxb_bc6h_pick_mode that mode and its always-fitting fallback and drops every candidate of
+// another mode from the winner search; shape (0..31) replaces every two-region candidate shape.
+struct dxb_bc6h_dbg_forcing { int32_t mode, shape; };
+static thread_local const dxb_bc6h_dbg_forcing* dxb_bc6h_dbg_force = nullptr;       // [2]
+static thread_local int32_t dxb_bc6h_dbg_pick_only = -1;                             // the forced mode of the lane being picked
+#endif
+
 // ---------------------------------------------------------------------------------------------------
 // stage 3: pick the mode for a set of endpoints (ep[4][3]: A0 B0 A1 B1, INT domain) and quantise them.
 //   two = two regions.  Returns the mode index (0..13); q[4][3] = quantised endpoints (not yet delta-transformed).
@@ -231,6 +244,9 @@ DXB_DEV int dxb_bc6h_pick_mode(const int32_t ep[4][3], bool two, bool bSigned, i
     for (int ci = 0; ci < ncand; ++ci)
     {
         const int m = two ? order2[ci] : order1[ci];
+#if !DXB_ON_DEVICE
+        if (dxb_bc6h_dbg_pick_only >= 0 && m != dxb_bc6h_dbg_pick_only && ci + 1 < ncand) continue;
+#endif
         const uint32_t info = dxb_bc6h_info[m];
         const int32_t prec = (int32_t)((info >> 8) & 31u);
         const bool transformed = ((info >> 6) & 1u) != 0u;
@@ -451,6 +467,12 @@ DXB_DEV void dxb_bc6h_encode_pair(const dxb_px* spx, bool bSigned, uint8_t* out0
                 if (k0[L] == win[L]) { k0[L] = k1[L]; k1[L] = 0xFFFFFFFFu; }
             DXB_LANES_END
         }
+#if !DXB_ON_DEVICE
+        DXB_LANES_BEGIN
+            if (dxb_bc6h_dbg_force && dxb_bc6h_dbg_force[lane >> 4].shape >= 0)
+                for (int r = 0; r < DXB_BC6H_KSHAPES; ++r) sel[r][L] = (uint32_t)dxb_bc6h_dbg_force[lane >> 4].shape;
+        DXB_LANES_END
+#endif
     }
 
     // ---- stage 2: continuous fits
@@ -500,7 +522,13 @@ DXB_DEV void dxb_bc6h_encode_pair(const dxb_px* spx, bool bSigned, uint8_t* out0
         }
         int32_t q[4][3];
         for (int e = 0; e < 4; ++e) for (int c = 0; c < 3; ++c) q[e][c] = 0;
+#if !DXB_ON_DEVICE
+        dxb_bc6h_dbg_pick_only = dxb_bc6h_dbg_force ? dxb_bc6h_dbg_force[lane >> 4].mode : -1;
+#endif
         const int mode = dxb_bc6h_pick_mode(ep, !one, bSigned, q);
+#if !DXB_ON_DEVICE
+        dxb_bc6h_dbg_pick_only = -1;
+#endif
         const int32_t prec = (int32_t)((dxb_bc6h_info[mode] >> 8) & 31u);
         // +-1 code refinement of this lane's own region
         int32_t qa[3], qb[3];
@@ -555,6 +583,10 @@ DXB_DEV void dxb_bc6h_encode_pair(const dxb_px* spx, bool bSigned, uint8_t* out0
         float e = rErrF[L];
         if (hl < 2 * DXB_BC6H_KSHAPES) e = e + partnerF[L];
         wkeys[L] = ((dxb_float_as_uint(e) >> 5) << 4) | (uint32_t)hl;
+#if !DXB_ON_DEVICE
+        if (dxb_bc6h_dbg_force && dxb_bc6h_dbg_force[lane >> 4].mode >= 0 && (int32_t)rMode[L] != dxb_bc6h_dbg_force[lane >> 4].mode)
+            wkeys[L] = 0xFFFFFFE0u | (uint32_t)hl;
+#endif
         if (hl == 15) wkeys[L] = 0xFFFFFFFFu;
     DXB_LANES_END
     dxb_half_min_u32(wkeys, wkey);
@@ -600,6 +632,19 @@ DXB_DEV void dxb_bc6h_encode_pair(const dxb_px* spx, bool bSigned, uint8_t* out0
             if (k < nk && e < best) { best = e; bk = k; }
         }
         idx[L] = bk;
+#if !DXB_ON_DEVICE
+        if (dxb_bc6h_dbg_rec)
+        {
+            dxb_bc6h_dbg_block& R = dxb_bc6h_dbg_rec[lane >> 4];
+            R.idx[hl] = (int32_t)bk;
+            for (int c = 0; c < 3; ++c) R.texel[hl][c] = dxb_bc6h_palette(ua[c], ub[c], (int32_t)dxb_bc7_weight(ib, bk), bSigned);
+            if (hl == 0)
+            {
+                R.mode = (int32_t)wMode[L]; R.shape = two ? (int32_t)wShape[L] : 0;
+                for (int k = 0; k < 12; ++k) R.wq[k] = (int32_t)wq[k][L];
+            }
+        }
+#endif
     DXB_LANES_END
 
     // header fields: endpoint 0 A as is, the others as deltas in transformed modes, masked to their field widths;

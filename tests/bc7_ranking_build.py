@@ -1,4 +1,4 @@
-"""TEST INFRASTRUCTURE: builds the BC7 stage-1 test harnesses of tests/bc7_ranking/ into a temporary directory.
+"""TEST INFRASTRUCTURE: builds the encoder test harnesses (tests/bc7_ranking/, tests/bc67_blocks/) into a temporary directory.
 
 host_lib: g++ with the host emulator's flags (tests/emul/build.sh), so it runs the host branches the emulator runs.
 device_lib: nvcc for sm_90a with the library's own flags (directxtex_b200/build.py), so it runs the device branches the kernels run."""
@@ -13,19 +13,20 @@ HERE = os.path.join(ROOT, "tests", "bc7_ranking")
 HOST_FLAGS = ["-std=c++17", "-O2", "-msse2", "-mfpmath=sse", "-mfma", "-ffp-contract=off", "-fopenmp", "-fPIC", "-shared", "-x", "c++"]
 
 
-def host_lib(src, out_dir):
+def host_lib(src, out_dir, src_dir=HERE):
+    """src (a file of src_dir, by default tests/bc7_ranking/) built with the emulator's flags into out_dir"""
     cxx = "/usr/bin/g++" if os.path.exists("/usr/bin/g++") else shutil.which("g++")
     out = os.path.join(str(out_dir), os.path.splitext(src)[0] + "_host.so")
-    r = subprocess.run([cxx] + HOST_FLAGS + ["-I", CSRC, "-I", os.path.join(ROOT, "include"), os.path.join(HERE, src), "-o", out],
+    r = subprocess.run([cxx] + HOST_FLAGS + ["-I", CSRC, "-I", os.path.join(ROOT, "include"), os.path.join(src_dir, src), "-o", out],
                        capture_output=True, text=True)
     assert r.returncode == 0, r.stdout + r.stderr
     return C.CDLL(out)
 
 
-def device_lib(src, out_dir):
+def device_lib(src, out_dir, src_dir=HERE):
     from directxtex_b200 import build as b
     out = os.path.join(str(out_dir), os.path.splitext(src)[0] + "_device.so")
-    r = subprocess.run([b._nvcc()] + b._flags() + ["-shared", "-cudart", "static", os.path.join(HERE, src), "-o", out],
+    r = subprocess.run([b._nvcc()] + b._flags() + ["-shared", "-cudart", "static", os.path.join(src_dir, src), "-o", out],
                        capture_output=True, text=True)
     assert r.returncode == 0, r.stdout + r.stderr
     return C.CDLL(out)
