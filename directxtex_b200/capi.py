@@ -11,7 +11,7 @@ LIB_PATH = os.environ.get("DXTEX_B200_LIB") or os.path.join(_HERE, "_lib", "libd
 SYMBOLS = [
     "dxb200_version", "dxb200_init", "dxb200_init_devices", "dxb200_initialized_devices", "dxb200_shutdown", "dxb200_device_count", "dxb200_launch_count", "dxb200_tma_launch_count", "dxb200_kernel_launch_count", "dxb200_set_option", "dxb200_get_option", "dxb200_last_error",
     "dxb200_host_alloc", "dxb200_host_free", "dxb200_compute_pitch", "dxb200_calculate_mip_levels",
-    "dxb200_compress", "dxb200_compress_ex", "dxb200_compress_device", "dxb200_convert_ex", "dxb200_mipmaps_compress", "dxb200_decompress", "dxb200_decompress_device",
+    "dxb200_compress", "dxb200_compress_ex", "dxb200_compress_device", "dxb200_convert_ex", "dxb200_mipmaps_compress", "dxb200_mipmaps_compress_ex", "dxb200_decompress", "dxb200_decompress_device",
     "dxb200_convert", "dxb200_convert_device", "dxb200_generate_mipmaps", "dxb200_generate_mipmaps_device",
     "dxb200_resize", "dxb200_resize_device", "dxb200_premultiply_alpha", "dxb200_premultiply_alpha_device",
     "dxb200_scale_mipmaps_alpha_for_coverage", "dxb200_scale_mipmaps_alpha_for_coverage_device",
@@ -29,6 +29,11 @@ class Metadata(C.Structure):
     """dxb200_metadata == DirectX::TexMetadata (DirectXTex.h:187-216)."""
     _fields_ = [("width", C.c_size_t), ("height", C.c_size_t), ("depth", C.c_size_t), ("arraySize", C.c_size_t), ("mipLevels", C.c_size_t),
                 ("miscFlags", C.c_uint32), ("miscFlags2", C.c_uint32), ("format", C.c_uint32), ("dimension", C.c_uint32)]
+
+
+class ChainSteps(C.Structure):
+    """dxb200_chain_steps: the steps dxb200_mipmaps_compress_ex runs between the mips and the compression."""
+    _fields_ = [("alphaReference", C.c_float), ("premultiply", C.c_uint32), ("pmalphaFlags", C.c_uint32)]
 
 
 STATUS_FN = C.CFUNCTYPE(C.c_int, C.c_size_t, C.c_size_t, C.c_void_p)      # dxb200_status_fn
@@ -66,6 +71,8 @@ def _load():
     lib.dxb200_compress_ex.argtypes = [IP, C.c_size_t, C.c_uint32, C.c_uint32, C.c_float, C.c_float, IP, STATUS_FN, C.c_void_p]
     lib.dxb200_convert_ex.argtypes = [IP, C.c_size_t, C.c_uint32, C.c_uint32, C.c_float, IP, STATUS_FN, C.c_void_p]
     lib.dxb200_mipmaps_compress.argtypes = [IP, C.c_size_t, C.c_size_t, C.c_uint32, C.c_uint32, C.c_uint32, C.c_float, C.c_float, IP]
+    lib.dxb200_mipmaps_compress_ex.argtypes = [IP, C.c_size_t, C.c_size_t, C.c_uint32, C.POINTER(ChainSteps), C.c_uint32, C.c_uint32, C.c_float,
+                                               C.c_float, IP]
     lib.dxb200_compute_pitch.argtypes = [C.c_uint32, C.c_size_t, C.c_size_t, C.POINTER(C.c_size_t), C.POINTER(C.c_size_t)]
     lib.dxb200_calculate_mip_levels.argtypes = [C.c_size_t, C.c_size_t, C.POINTER(C.c_size_t)]
     lib.dxb200_compress.argtypes = [IP, C.c_size_t, C.c_uint32, C.c_uint32, C.c_float, C.c_float, IP]
@@ -91,7 +98,7 @@ def _load():
     lib.dxb200_dds_load_memory.argtypes = [C.c_void_p, C.c_size_t, C.c_uint32, IP, C.c_size_t]
     for name in ("dxb200_dds_encode_header", "dxb200_dds_save_memory", "dxb200_dds_get_metadata", "dxb200_dds_load_memory"):
         getattr(lib, name).restype = C.c_int32
-    for name in ("dxb200_init", "dxb200_init_devices", "dxb200_initialized_devices", "dxb200_compress_ex", "dxb200_convert_ex", "dxb200_mipmaps_compress", "dxb200_device_count", "dxb200_compute_pitch", "dxb200_calculate_mip_levels", "dxb200_compress",
+    for name in ("dxb200_init", "dxb200_init_devices", "dxb200_initialized_devices", "dxb200_compress_ex", "dxb200_convert_ex", "dxb200_mipmaps_compress", "dxb200_mipmaps_compress_ex", "dxb200_device_count", "dxb200_compute_pitch", "dxb200_calculate_mip_levels", "dxb200_compress",
                  "dxb200_compress_device", "dxb200_decompress", "dxb200_decompress_device", "dxb200_convert",
                  "dxb200_convert_device", "dxb200_generate_mipmaps", "dxb200_generate_mipmaps_device", "dxb200_resize", "dxb200_resize_device", "dxb200_premultiply_alpha", "dxb200_premultiply_alpha_device"):
         getattr(lib, name).restype = C.c_int32
@@ -173,8 +180,14 @@ def compress_with_status(src, w, h, src_fmt, dst_fmt, callback, flags=0):
     return F.hr_u32(hr), out
 
 
-def mipmaps_compress(srcs, w, h, src_fmt, dst_fmt, filter=0, levels=0, flags=0):
-    """dxb200_mipmaps_compress of an array of equally sized host images; returns one packed BC chain (bytes) per image."""
+def chain_steps(alpha_reference=0.0, premultiply=False, pmalpha_flags=0):
+    """the dxb200_chain_steps of texconv's -keepcoverage (alpha_reference > 0) and -pmalpha (premultiply, with pmalpha_flags)"""
+    return ChainSteps(alpha_reference, 1 if premultiply else 0, pmalpha_flags)
+
+
+def mipmaps_compress(srcs, w, h, src_fmt, dst_fmt, filter=0, levels=0, flags=0, steps=None):
+    """dxb200_mipmaps_compress_ex of an array of equally sized host images, with the ChainSteps `steps` (None: mips and compression
+    only); returns one packed BC chain (bytes) per image."""
     srcs = [np.ascontiguousarray(a).view(np.uint8).reshape(-1) for a in srcs]
     levels = levels or F.count_mips(w, h)
     olayout, total = texture_layout(dst_fmt, w, h, 1, levels)
@@ -182,9 +195,9 @@ def mipmaps_compress(srcs, w, h, src_fmt, dst_fmt, filter=0, levels=0, flags=0):
     outs = [np.zeros(total, np.uint8) for _ in srcs]
     s = images([Image(w, h, src_fmt, row, sl, _np_ptr(a)) for a in srcs])
     d = images([Image(lw, lh, dst_fmt, r, sp, _np_ptr(o) + off) for o in outs for (off, lw, lh, r, sp) in olayout])
-    hr = lib.dxb200_mipmaps_compress(s, len(srcs), levels, filter, dst_fmt, flags, 0.5, 1.0, d)
+    hr = lib.dxb200_mipmaps_compress_ex(s, len(srcs), levels, filter, C.byref(steps) if steps is not None else None, dst_fmt, flags, 0.5, 1.0, d)
     if hr != 0:
-        raise DxTexError(hr, "dxb200_mipmaps_compress")
+        raise DxTexError(hr, "dxb200_mipmaps_compress_ex")
     return outs
 
 

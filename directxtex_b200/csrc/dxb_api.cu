@@ -6,7 +6,8 @@
 // pair) are grouped into chunks that pipeline H2D -> kernels -> D2H over the NSLOT (stream, buffer) slots of a lane.  Band calls
 // (compress, decompress, convert, premultiply) cut images into ~32 MiB bands and stage 48 MiB per chunk; chain and pair calls
 // (generate_mipmaps, resize, mipmaps_compress) stage 80 MiB per chunk.  ScaleMipMapsAlphaForCoverage stages on its own: it
-// downloads with a 2D copy into the caller's pitch and its bisection synchronises on the host.
+// downloads with a 2D copy into the caller's pitch.  Its search runs on the device for a whole batch (launch_coverage) with no
+// host round trip; the per-item call synchronises once, at its end.
 //
 // Compiled with: nvcc -gencode arch=compute_90a,code=sm_90a -fmad=false (bit-exact fp32 contract
 // of the BC1-5 / convert / mip kernels) -lineinfo.  There is no host implementation of any codec in
@@ -565,6 +566,39 @@ int32_t launch_mips(const dxb200_image* chain, size_t items, size_t levels, uint
     return hr;
 }
 
+// ---- ScaleMipMapsAlphaForCoverage -------------------------------------------------------------------------------------
+// chains[it * levels + l] (DEVICE pointers) -> out[...]: levels >= 1 of every item scaled so that their alpha-test coverage at `ref`
+// matches level 0's; level 0 is not written.  Always DXB_COVERAGE_STEPS k_alpha_coverage launches and one k_scale_alpha, with
+// no host round trip in between, whatever the item and level counts.  The job table and the counts are allocated on `stream`.
+int32_t launch_coverage(const dxb200_image* chains, const dxb200_image* out, size_t items, size_t levels, float ref, cudaStream_t stream)
+{
+    CoveragePlan cp;
+    int32_t hr = plan_coverage_jobs(chains, out, items, levels, ref, &cp);
+    if (hr != DXB_S_OK) return hr;
+    const size_t countBytes = cp.jobs.size() * DXB_COVERAGE_STEPS * sizeof(unsigned long long);
+    uint8_t* dev = nullptr;
+    DXB_CUDA(cudaMallocAsync(reinterpret_cast<void**>(&dev), countBytes + cp.jobs.size() * sizeof(dxb_coverage_job), stream));
+    unsigned long long* counts = reinterpret_cast<unsigned long long*>(dev);
+    const dxb_coverage_job* jobs = reinterpret_cast<const dxb_coverage_job*>(dev + countBytes);
+    hr = cuda_hr(cudaMemsetAsync(counts, 0, countBytes, stream), "cudaMemsetAsync(coverage counts)");
+    if (hr == DXB_S_OK)
+        hr = cuda_hr(cudaMemcpyAsync(dev + countBytes, cp.jobs.data(), cp.jobs.size() * sizeof(dxb_coverage_job), cudaMemcpyHostToDevice, stream), "H2D");
+    const uint32_t cap = (uint32_t)t_v.dev->gridRow * 8u;
+    for (uint32_t step = 0; step < DXB_COVERAGE_STEPS && hr == DXB_S_OK; ++step)
+        hr = check_launch(dxb_launch_alpha_coverage(grid_for(cp.P.totalCells - (step ? cp.P.baseCells : 0u), 256, cap), stream, jobs, cp.P, counts, step));
+    if (hr == DXB_S_OK) hr = check_launch(dxb_launch_scale_alpha(grid_for(cp.P.scaledPixels, 256, cap), stream, jobs, cp.P, counts));
+    cudaFreeAsync(dev, stream);
+    return hr;
+}
+
+// ScaleMipMapsAlphaForCoverage of one item (DEVICE pointers): level 0 copied (:3511-3530), the others scaled
+int32_t scale_alpha_for_coverage_device(const dxb200_image* src, size_t n, float ref, const dxb200_image* dst, cudaStream_t st)
+{
+    DXB_CUDA(cudaMemcpy2DAsync(dst[0].pixels, dst[0].rowPitch, src[0].pixels, src[0].rowPitch, std::min(src[0].rowPitch, dst[0].rowPitch),
+                               src[0].slicePitch / std::max<size_t>(src[0].rowPitch, 1), cudaMemcpyDeviceToDevice, st));
+    return launch_coverage(src, dst, 1, n, ref, st);
+}
+
 } // namespace
 
 // =================================================================================================
@@ -818,47 +852,42 @@ int32_t dxb200_generate_mipmaps(const dxb200_image* chain, size_t items, size_t 
 // compressed in device memory, and only the packed blocks come back: 4 B/texel up + 1.33 B/texel down (BC3 from RGBA8)
 // instead of 4 + 5.33 + 5.33 + 1.33.  Per item: base[i] = level 0 (host), dst[i * levels + l] = the BC image of level l (host).
 // Chunks of whole items are pipelined over the lane's NSLOT (stream, buffer) slots: H2D, mip kernels, compress kernel, D2H.
-int32_t dxb200_mipmaps_compress(const dxb200_image* base, size_t items, size_t levels, uint32_t filter, uint32_t dstFormat,
-                                uint32_t flags, float threshold, float alphaWeight, const dxb200_image* dst)
+// dxb200_mipmaps_compress_ex adds texconv's two steps between the mips and the compression (-keepcoverage :3480, -pmalpha :3526),
+// both in place on the chunk's chains in device memory.
+int32_t dxb200_mipmaps_compress_ex(const dxb200_image* base, size_t items, size_t levels, uint32_t filter, const dxb200_chain_steps* steps,
+                                   uint32_t dstFormat, uint32_t flags, float threshold, float alphaWeight, const dxb200_image* dst)
 {
     (void)alphaWeight;
-    if (!base || !dst || !items || !levels) return DXB_E_INVALIDARG;
-    // the chain every item will have on the device (ScratchImage layout of the source format)
-    std::vector<dxb200_image> chain(items * levels);
-    for (size_t i = 0; i < items; ++i)
-    {
-        size_t w = base[i].width, h = base[i].height;
-        if (!base[i].pixels) return DXB_E_POINTER;
-        if (levels > count_mips(w, h)) return DXB_E_INVALIDARG;
-        for (size_t l = 0; l < levels; ++l)
-        {
-            dxb200_image& c = chain[i * levels + l];
-            c.width = w; c.height = h; c.format = base[i].format;
-            const int32_t hp = compute_pitch(c.format, w, h, &c.rowPitch, &c.slicePitch);
-            if (hp != DXB_S_OK) return hp;
-            c.pixels = const_cast<uint8_t*>(base[i].pixels);          // level 0's upload source; the other levels only need it for validation
-            if (h > 1) h >>= 1;
-            if (w > 1) w >>= 1;
-        }
-        chain[i * levels].rowPitch = base[i].rowPitch; chain[i * levels].slicePitch = base[i].slicePitch;
-    }
-    uint32_t mode = 0;
-    int32_t hr = plan_mips(chain.data(), items, levels, filter, &mode);
-    if (hr != DXB_S_OK) return hr;
-    CompressPlan plan;
-    hr = plan_compress(chain.data(), items * levels, dstFormat, flags, threshold, dst, &plan);
+    ChainPlan cp;
+    const int32_t hr = plan_mipmaps_compress(base, items, levels, filter, steps, dstFormat, flags, threshold, dst, &cp);
     if (hr != DXB_S_OK) return hr;
     return run_sharded(items, [&](size_t i) { return base[i].slicePitch; },
         [&](size_t lo, size_t hi)
         {
-            const Plane planes[2] = { { chain.data() + lo * levels, levels, Copy::Up, Copy::None }, { dst + lo * levels, levels, Copy::Down, Copy::Down } };
+            const Plane planes[2] = { { cp.chain.data() + lo * levels, levels, Copy::Up, Copy::None }, { dst + lo * levels, levels, Copy::Down, Copy::Down } };
             return run_staged(planes, 2, hi - lo, ITEM_CHUNK,
                 [&](const std::vector<dxb200_image>* dev, size_t cnt, cudaStream_t st)
                 {
-                    const int32_t h2 = launch_mips(dev[0].data(), cnt, levels, filter, mode, st);
-                    return h2 != DXB_S_OK ? h2 : launch_compress(plan, dev[0].data(), dev[1].data(), cnt * levels, st);
+                    const dxb200_image* chains = dev[0].data();
+                    int32_t h2 = launch_mips(chains, cnt, levels, filter, cp.mode, st);
+                    if (h2 == DXB_S_OK && cp.coverage) h2 = launch_coverage(chains, chains, cnt, levels, cp.ref, st);
+                    // one launch per level: the chunk's images of a level are equal, as the separate calls' images are, so they take the
+                    // same premultiply kernel
+                    std::vector<dxb200_image> level(cnt);
+                    for (size_t l = 0; l < levels && h2 == DXB_S_OK && cp.premultiply; ++l)
+                    {
+                        for (size_t it = 0; it < cnt; ++it) level[it] = chains[it * levels + l];
+                        h2 = launch_pmalpha(cp.pm, level.data(), level.data(), cnt, st);
+                    }
+                    return h2 != DXB_S_OK ? h2 : launch_compress(cp.compress, chains, dev[1].data(), cnt * levels, st);
                 });
         });
+}
+
+int32_t dxb200_mipmaps_compress(const dxb200_image* base, size_t items, size_t levels, uint32_t filter, uint32_t dstFormat,
+                                uint32_t flags, float threshold, float alphaWeight, const dxb200_image* dst)
+{
+    return dxb200_mipmaps_compress_ex(base, items, levels, filter, nullptr, dstFormat, flags, threshold, alphaWeight, dst);
 }
 
 int32_t dxb200_premultiply_alpha_device(const dxb200_image* src, size_t nimages, uint32_t flags, const dxb200_image* dst, void* stream)
@@ -882,51 +911,6 @@ int32_t dxb200_premultiply_alpha(const dxb200_image* src, size_t nimages, uint32
 }
 
 // ---- ScaleMipMapsAlphaForCoverage ----------------------------------------------------------------
-// device pointers; count = device scratch (8 bytes).  Mirrors CalculateAlphaCoverage / EstimateAlphaScaleForCoverage.
-static int32_t alpha_coverage_device(const dxb200_image& img, float ref, float scale, unsigned long long* dCount, cudaStream_t st, float* coverage)
-{
-    *coverage = 0.0f;
-    if (img.width < 2 || img.height < 2) return DXB_S_OK;                      // no 2x2 cell: the reference's loops do not run
-    dxb_job j; memset(&j, 0, sizeof(j));
-    j.src = img.pixels; j.srcPitch = img.rowPitch; j.width = (uint32_t)img.width; j.height = (uint32_t)img.height;
-    DXB_CUDA(cudaMemsetAsync(dCount, 0, sizeof(unsigned long long), st));
-    const uint64_t cells = (uint64_t)(img.width - 1) * (img.height - 1);
-    const uint32_t grid = (uint32_t)std::max<uint64_t>(1, std::min<uint64_t>((cells + 255) / 256, (uint64_t)t_v.dev->gridRow * 8u));
-    const int32_t hr = check_launch(dxb_launch_alpha_coverage(grid, st, j, img.format, scale, ref, dCount));
-    if (hr != DXB_S_OK) return hr;
-    unsigned long long hCount = 0;
-    DXB_CUDA(cudaMemcpyAsync(&hCount, dCount, sizeof(hCount), cudaMemcpyDeviceToHost, st));
-    DXB_CUDA(cudaStreamSynchronize(st));
-    *coverage = alpha_coverage_fraction(hCount, img.width, img.height);
-    return DXB_S_OK;
-}
-
-static int32_t scale_alpha_for_coverage_device(const dxb200_image* src, size_t n, float ref, const dxb200_image* dst, cudaStream_t st)
-{
-    unsigned long long* dCount = nullptr;
-    DXB_CUDA(cudaMallocAsync(reinterpret_cast<void**>(&dCount), sizeof(unsigned long long), st));
-    float target = 0.0f;
-    int32_t hr = alpha_coverage_device(src[0], ref, 1.0f, dCount, st, &target);
-    // base level: plain copy (:3511-3530)
-    if (hr == DXB_S_OK)
-        hr = cuda_hr(cudaMemcpy2DAsync(dst[0].pixels, dst[0].rowPitch, src[0].pixels, src[0].rowPitch, std::min(src[0].rowPitch, dst[0].rowPitch),
-                                       src[0].slicePitch / std::max<size_t>(src[0].rowPitch, 1), cudaMemcpyDeviceToDevice, st), "copy base level");
-    for (size_t l = 1; l < n && hr == DXB_S_OK; ++l)
-    {
-        float scale = 1.0f;
-        hr = estimate_alpha_scale(target, [&](float s, float* cov) { return alpha_coverage_device(src[l], ref, s, dCount, st, cov); }, &scale);
-        if (hr != DXB_S_OK) break;
-        dxb_job j; memset(&j, 0, sizeof(j));
-        j.src = src[l].pixels; j.dst = dst[l].pixels; j.srcPitch = src[l].rowPitch; j.dstPitch = dst[l].rowPitch;
-        j.width = (uint32_t)src[l].width; j.height = (uint32_t)src[l].height;
-        const uint64_t px = (uint64_t)j.width * j.height;
-        const uint32_t grid = (uint32_t)std::max<uint64_t>(1, std::min<uint64_t>((px + 255) / 256, (uint64_t)t_v.dev->gridRow * 8u));
-        hr = check_launch(dxb_launch_scale_alpha(grid, st, j, src[l].format, scale));
-    }
-    cudaFreeAsync(dCount, st);
-    return hr;
-}
-
 int32_t dxb200_scale_mipmaps_alpha_for_coverage_device(const dxb200_image* src, size_t nlevels, float alphaReference, const dxb200_image* dst, void* stream)
 {
     int32_t hr = plan_alpha_coverage(src, nlevels, dst);
@@ -934,7 +918,10 @@ int32_t dxb200_scale_mipmaps_alpha_for_coverage_device(const dxb200_image* src, 
     DevScope scope;
     hr = scope.enter(src[0].pixels);
     if (hr != DXB_S_OK) return hr;
-    return scale_alpha_for_coverage_device(src, nlevels, alphaReference, dst, static_cast<cudaStream_t>(stream));
+    const cudaStream_t st = static_cast<cudaStream_t>(stream);
+    hr = scale_alpha_for_coverage_device(src, nlevels, alphaReference, dst, st);
+    const int32_t hs = cuda_hr(cudaStreamSynchronize(st), "alpha coverage sync");       // the documented end of the call
+    return hr != DXB_S_OK ? hr : hs;
 }
 
 int32_t dxb200_scale_mipmaps_alpha_for_coverage(const dxb200_image* src, size_t nlevels, float alphaReference, const dxb200_image* dst)

@@ -15,6 +15,7 @@
 #include "dxb_dispatch.h"
 #include "dxb_pixel.cuh"
 #include "dxb_mips.cuh"
+#include "dxb_coverage.h"
 
 // ------------------------------------------------------------------------------------------------ generic
 __global__ void __launch_bounds__(256) k_convert(const dxb_job* __restrict__ jobs, dxb_job single, dxb_convert_params P)
@@ -259,40 +260,80 @@ const char* dxb_launch_pmalpha(unsigned grid, cudaStream_t stream, const dxb_job
 }
 
 // ------------------------------------------------------------------------------------------------ alpha coverage
-// k_alpha_coverage: one thread per 2x2 cell of one image, integer count accumulated with one atomicAdd per warp.
-__global__ void __launch_bounds__(256) k_alpha_coverage(dxb_job j, uint32_t fmt, float scale, float ref, unsigned long long* count)
+// The search of every (item, level) job of a batch advances one step per k_alpha_coverage launch; each job's scale comes from
+// replaying the search over the counts of the earlier launches (dxb_coverage_scale), so no count goes back to the host.
+// Returns false when the job's search has stopped before step `step`.
+__device__ __forceinline__ bool dxb_job_scale(const dxb_coverage_job* jobs, const unsigned long long* counts, uint32_t ji, uint32_t step, float* scale)
 {
-    const uint32_t cw = j.width - 1u, ch = j.height - 1u;
-    const uint32_t cells = cw * ch;
-    uint32_t local = 0;
-    for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < cells; i += gridDim.x * blockDim.x)
-    {
-        const uint32_t y = i / cw, x = i - y * cw;
-        const uint8_t* r0 = j.src + (size_t)y * j.srcPitch;
-        const uint8_t* r1 = r0 + j.srcPitch;
-        local += dxb_alpha_coverage_cell(dxb_load_pixel(fmt, r0, x).w, dxb_load_pixel(fmt, r1, x).w,
-                                         dxb_load_pixel(fmt, r0, x + 1u).w, dxb_load_pixel(fmt, r1, x + 1u).w, scale, ref);
-    }
-    local = __reduce_add_sync(0xffffffffu, local);
-    if ((threadIdx.x & 31u) == 0 && local) atomicAdd(count, (unsigned long long)local);
+    const dxb_coverage_job& j = jobs[ji];
+    const dxb_coverage_job& b = jobs[j.item];
+    // step 0 does not look at the target, which that same launch is still counting
+    const unsigned long long target = step ? counts[(size_t)j.item * DXB_COVERAGE_STEPS] : 0ull;
+    return dxb_coverage_scale(target, b.width, b.height, counts + (size_t)ji * DXB_COVERAGE_STEPS, step, j.width, j.height, scale);
 }
-__global__ void __launch_bounds__(256) k_scale_alpha(dxb_job j, uint32_t fmt, float scale)
+
+// k_alpha_coverage: step `step` of the search of every job, one thread per 2x2 cell.  Step 0 measures every level at scale 1
+// (level 0's count is the item's target); later steps only the levels >= 1 whose search still runs, and their cells follow
+// the level-0 cells in the table.  A warp's cells can belong to two jobs: each job's lanes add up their counts before one
+// atomicAdd.
+__global__ void __launch_bounds__(256) k_alpha_coverage(const dxb_coverage_job* __restrict__ jobs, dxb_coverage_params P, unsigned long long* counts,
+                                                        uint32_t step)
 {
-    const uint32_t n = j.width * j.height;
-    for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x)
+    const uint32_t lane = threadIdx.x & 31u, stride = gridDim.x * blockDim.x;
+    uint32_t cached = UINT32_MAX; bool active = false; float scale = 1.0f;
+    // the loop bound is the same for every lane of a warp, so the whole warp takes part in each reduction
+    for (uint32_t w0 = (step ? P.baseCells : 0u) + blockIdx.x * blockDim.x + (threadIdx.x & ~31u); w0 < P.totalCells; w0 += stride)
     {
+        const uint32_t unit = w0 + lane;
+        uint32_t key = UINT32_MAX, n = 0;
+        if (unit < P.totalCells)
+        {
+            const dxb_coverage_job& j = dxb_find_job(jobs, P.njobs, jobs[0], unit);
+            const uint32_t ji = (uint32_t)(&j - jobs);
+            if (ji != cached) { cached = ji; active = dxb_job_scale(jobs, counts, ji, step, &scale); }
+            if (active)
+            {
+                const uint32_t cw = j.width - 1u, i = unit - j.firstUnit;
+                const uint32_t y = i / cw, x = i - y * cw;
+                const uint8_t* r0 = j.src + (size_t)y * j.srcPitch;
+                const uint8_t* r1 = r0 + j.srcPitch;
+                n = dxb_alpha_coverage_cell(dxb_load_pixel(P.format, r0, x).w, dxb_load_pixel(P.format, r1, x).w,
+                                            dxb_load_pixel(P.format, r0, x + 1u).w, dxb_load_pixel(P.format, r1, x + 1u).w, scale, P.ref);
+                key = ji;
+            }
+        }
+        const uint32_t peers = __match_any_sync(0xffffffffu, key);
+        n = __reduce_add_sync(peers, n);
+        if (key != UINT32_MAX && n && lane == (uint32_t)__ffs(peers) - 1u)
+            atomicAdd(counts + (size_t)key * DXB_COVERAGE_STEPS + step, (unsigned long long)n);
+    }
+}
+// k_scale_alpha: every pixel of the levels >= 1 (the jobs after the P.items level-0 ones), src -> dst, at the result of its
+// job's search
+__global__ void __launch_bounds__(256) k_scale_alpha(const dxb_coverage_job* __restrict__ jobs, dxb_coverage_params P, const unsigned long long* counts)
+{
+    const dxb_coverage_job* levels = jobs + P.items;
+    uint32_t cached = UINT32_MAX; float scale = 1.0f;
+    for (uint32_t unit = blockIdx.x * blockDim.x + threadIdx.x; unit < P.scaledPixels; unit += gridDim.x * blockDim.x)
+    {
+        const dxb_coverage_job& j = dxb_find_job(levels, P.njobs - P.items, levels[0], unit, &dxb_coverage_job::firstPixel);
+        const uint32_t ji = (uint32_t)(&j - jobs);
+        if (ji != cached) { cached = ji; (void)dxb_job_scale(jobs, counts, ji, DXB_COVERAGE_STEPS, &scale); }
+        const uint32_t i = unit - j.firstPixel;
         const uint32_t y = i / j.width, x = i - y * j.width;
-        dxb_scale_alpha_pixel(fmt, j.src + (size_t)y * j.srcPitch, j.dst + (size_t)y * j.dstPitch, x, scale);
+        dxb_scale_alpha_pixel(P.format, j.src + (size_t)y * j.srcPitch, j.dst + (size_t)y * j.dstPitch, x, scale);
     }
 }
-const char* dxb_launch_alpha_coverage(unsigned grid, cudaStream_t stream, const dxb_job& j, uint32_t fmt, float scale, float ref, unsigned long long* count)
+const char* dxb_launch_alpha_coverage(unsigned grid, cudaStream_t stream, const dxb_coverage_job* jobs, const dxb_coverage_params& P,
+                                      unsigned long long* counts, uint32_t step)
 {
-    k_alpha_coverage<<<grid, 256, 0, stream>>>(j, fmt, scale, ref, count);
+    k_alpha_coverage<<<grid, 256, 0, stream>>>(jobs, P, counts, step);
     return "k_alpha_coverage";
 }
-const char* dxb_launch_scale_alpha(unsigned grid, cudaStream_t stream, const dxb_job& j, uint32_t fmt, float scale)
+const char* dxb_launch_scale_alpha(unsigned grid, cudaStream_t stream, const dxb_coverage_job* jobs, const dxb_coverage_params& P,
+                                   const unsigned long long* counts)
 {
-    k_scale_alpha<<<grid, 256, 0, stream>>>(j, fmt, scale);
+    k_scale_alpha<<<grid, 256, 0, stream>>>(jobs, P, counts);
     return "k_scale_alpha";
 }
 

@@ -42,8 +42,13 @@ int32_t dxb_launch_mip_chain(cudaStream_t stream, const dxb_mip_job* jobs, const
                              dxb_mip_params P, const dxb_tri_axis* tri, unsigned gridCap, bool genericOnly,
                              int32_t (*launched)(const char* kernel));
 const char* dxb_launch_convert_diffuse(cudaStream_t stream, const dxb_job* jobs, const dxb_job* hostJobs, const dxb_convert_params& P, void* errors, uint32_t errStride);
-const char* dxb_launch_alpha_coverage(unsigned grid, cudaStream_t stream, const dxb_job& j, uint32_t fmt, float scale, float ref, unsigned long long* count);
-const char* dxb_launch_scale_alpha(unsigned grid, cudaStream_t stream, const dxb_job& j, uint32_t fmt, float scale);
+// ScaleMipMapsAlphaForCoverage of a batch of chains (dxb_coverage_job): `jobs` is the device table, `counts` DXB_COVERAGE_STEPS
+// counters per job, zero before step 0.  dxb_launch_alpha_coverage enqueues search step `step` of every job; dxb_launch_scale_alpha,
+// after the last step, scales every level >= 1 by the result of its search.
+const char* dxb_launch_alpha_coverage(unsigned grid, cudaStream_t stream, const dxb_coverage_job* jobs, const dxb_coverage_params& P,
+                                      unsigned long long* counts, uint32_t step);
+const char* dxb_launch_scale_alpha(unsigned grid, cudaStream_t stream, const dxb_coverage_job* jobs, const dxb_coverage_params& P,
+                                   const unsigned long long* counts);
 const char* dxb_launch_pmalpha(unsigned grid, cudaStream_t stream, const dxb_job* jobs, const dxb_job* hostJobs, const dxb_convert_params& P);
 // resident CTAs per SM of each kernel at its block size
 int dxb_occupancy_bc15();
@@ -51,15 +56,16 @@ int dxb_occupancy_bc7();
 int dxb_occupancy_bc6h();
 
 #ifdef __CUDACC__
+// the job of work unit `unit`; `first` names the job's prefix sum of units when a table has more than one (dxb_coverage_job)
 template <typename J>
-__device__ __forceinline__ const J& dxb_find_job(const J* jobs, uint32_t njobs, const J& single, uint32_t unit)
+__device__ __forceinline__ const J& dxb_find_job(const J* jobs, uint32_t njobs, const J& single, uint32_t unit, uint32_t J::*first = &J::firstUnit)
 {
     if (jobs == nullptr) return single;
-    uint32_t lo = 0, hi = njobs;            // last job with firstUnit <= unit
+    uint32_t lo = 0, hi = njobs;            // last job with first <= unit
     while (hi - lo > 1)
     {
         const uint32_t mid = (lo + hi) >> 1;
-        if (jobs[mid].firstUnit <= unit) lo = mid; else hi = mid;
+        if (jobs[mid].*first <= unit) lo = mid; else hi = mid;
     }
     return jobs[lo];
 }

@@ -12,6 +12,7 @@
 #include "dxb_formats.h"
 #include "dxb_jobs.h"
 #include "dxb_host_tri.h"
+#include "dxb_coverage.h"
 
 namespace {
 
@@ -289,32 +290,98 @@ int32_t plan_alpha_coverage(const dxb200_image* src, size_t n, const dxb200_imag
     return DXB_S_OK;
 }
 
-// CalculateAlphaCoverage's result (DirectXTexMipmaps.cpp:300-304): `count` covered samples of the 8x8 samples in each of the
-// (w - 1)(h - 1) cells of 2x2 pixels; 0 for an image without a cell
-float alpha_coverage_fraction(uint64_t count, size_t w, size_t h)
-{
-    const float cscale = static_cast<float>((w - 1) * (h - 1) * 8 * 8);
-    return cscale > 0.0f ? static_cast<float>(count) / cscale : 0.0f;
-}
-
-// EstimateAlphaScaleForCoverage (:310-355): bisection on [0, 4], at most 10 coverage evaluations.  coverage(scale, &cov)
-// returns an HRESULT; anything but S_OK stops the search and is returned.
+// EstimateAlphaScaleForCoverage (:310-355) driven step by step: coverage(scale, &cov) measures one step and returns an HRESULT;
+// anything but S_OK stops the search and is returned.  The rule is dxb_coverage_replay's.
 template <typename CoverageFn>
 int32_t estimate_alpha_scale(float target, CoverageFn coverage, float* scale)
 {
-    float lo = 0.0f, hi = 4.0f, s = 1.0f;
-    for (int it = 0; it < 10; ++it)
+    float cov[DXB_COVERAGE_STEPS];
+    const auto seen = [&](uint32_t i) { return cov[i]; };
+    float s = 1.0f;
+    for (uint32_t k = 0; k < DXB_COVERAGE_STEPS; ++k)
     {
-        float cov = 0.0f;
-        const int32_t hr = coverage(s, &cov);
+        if (!dxb_coverage_replay(target, k, seen, &s)) break;
+        const int32_t hr = coverage(s, &cov[k]);
         if (hr != DXB_S_OK) return hr;
-        if (cov < target) lo = s;
-        else if (cov > target) hi = s;
-        else break;
-        s = (lo + hi) * 0.5f;
+        if (k + 1 == DXB_COVERAGE_STEPS) (void)dxb_coverage_replay(target, DXB_COVERAGE_STEPS, seen, &s);
     }
     *scale = s;
     return DXB_S_OK;
+}
+
+// The job table of a batched ScaleMipMapsAlphaForCoverage: chains[it * levels + l] = level l of item it (source), out[...] = where
+// its result goes (the same images in a chain that is scaled in place).  Level 0 of every item comes first (job it), then the
+// other levels item by item.  Every cell and scaled pixel of the batch must have a 32-bit index: E_INVALIDARG otherwise.
+struct CoveragePlan { dxb_coverage_params P; std::vector<dxb_coverage_job> jobs; };
+
+int32_t plan_coverage_jobs(const dxb200_image* chains, const dxb200_image* out, size_t items, size_t levels, float ref, CoveragePlan* cp)
+{
+    dxb_coverage_params& P = cp->P; memset(&P, 0, sizeof(P));
+    P.format = chains[0].format; P.items = (uint32_t)items; P.njobs = (uint32_t)(items * levels); P.ref = ref;
+    cp->jobs.assign(items * levels, dxb_coverage_job());
+    uint64_t cells = 0, pixels = 0;
+    for (size_t n = 0; n < items * levels; ++n)
+    {
+        const size_t it = n < items ? n : (n - items) / (levels - 1), l = n < items ? 0 : 1 + (n - items) % (levels - 1);
+        const dxb200_image& s = chains[it * levels + l]; const dxb200_image& d = out[it * levels + l];
+        dxb_coverage_job& j = cp->jobs[n];
+        j.src = s.pixels; j.dst = d.pixels; j.srcPitch = s.rowPitch; j.dstPitch = d.rowPitch;
+        j.width = (uint32_t)s.width; j.height = (uint32_t)s.height; j.item = (uint32_t)it; j.pad = 0;
+        j.firstUnit = (uint32_t)cells; j.firstPixel = (uint32_t)pixels;
+        cells += (uint64_t)(s.width - 1) * (s.height - 1);
+        if (l) pixels += (uint64_t)s.width * s.height;
+        if (cells > 0xFFFFFFFFull || pixels > 0xFFFFFFFFull) return DXB_E_INVALIDARG;
+        if (n + 1 == items) P.baseCells = (uint32_t)cells;
+    }
+    P.totalCells = (uint32_t)cells; P.scaledPixels = (uint32_t)pixels;
+    return DXB_S_OK;
+}
+
+// ---- GenerateMipMaps -> ScaleMipMapsAlphaForCoverage -> PremultiplyAlpha -> Compress in one call (mipmaps_compress) ----------
+// chain = the chain every item will have on the device (ScratchImage layout of the source format; level 0 at the caller's
+// pitch, its pixels the upload source; the other levels carry base[i].pixels only for validation).
+struct ChainPlan
+{
+    std::vector<dxb200_image> chain;
+    uint32_t mode;
+    bool coverage; float ref;
+    bool premultiply; dxb_convert_params pm;
+    CompressPlan compress;
+};
+
+// Every check of the four steps before anything is uploaded, each with the HRESULT the reference's four calls would return at
+// the first step that fails; steps == nullptr (or no step enabled) = GenerateMipMaps + Compress.
+int32_t plan_mipmaps_compress(const dxb200_image* base, size_t items, size_t levels, uint32_t filter, const dxb200_chain_steps* steps,
+                              uint32_t dstFormat, uint32_t flags, float threshold, const dxb200_image* dst, ChainPlan* cp)
+{
+    if (!base || !dst || !items || !levels) return DXB_E_INVALIDARG;
+    std::vector<dxb200_image>& chain = cp->chain;
+    chain.resize(items * levels);
+    for (size_t i = 0; i < items; ++i)
+    {
+        size_t w = base[i].width, h = base[i].height;
+        if (!base[i].pixels) return DXB_E_POINTER;
+        if (levels > count_mips(w, h)) return DXB_E_INVALIDARG;
+        for (size_t l = 0; l < levels; ++l)
+        {
+            dxb200_image& c = chain[i * levels + l];
+            c.width = w; c.height = h; c.format = base[i].format;
+            const int32_t hp = compute_pitch(c.format, w, h, &c.rowPitch, &c.slicePitch);
+            if (hp != DXB_S_OK) return hp;
+            c.pixels = const_cast<uint8_t*>(base[i].pixels);
+            if (h > 1) h >>= 1;
+            if (w > 1) w >>= 1;
+        }
+        chain[i * levels].rowPitch = base[i].rowPitch; chain[i * levels].slicePitch = base[i].slicePitch;
+    }
+    int32_t hr = plan_mips(chain.data(), items, levels, filter, &cp->mode);
+    if (hr != DXB_S_OK) return hr;
+    cp->ref = steps ? steps->alphaReference : 0.0f;
+    cp->coverage = cp->ref > 0.0f;                                                      // texconv -keepcoverage (:3304)
+    if (cp->coverage && (hr = plan_alpha_coverage(chain.data(), items * levels, chain.data())) != DXB_S_OK) return hr;
+    cp->premultiply = steps && steps->premultiply;
+    if (cp->premultiply && (hr = plan_pmalpha(chain.data(), items * levels, steps->pmalphaFlags, chain.data(), &cp->pm)) != DXB_S_OK) return hr;
+    return plan_compress(chain.data(), items * levels, dstFormat, flags, threshold, dst, &cp->compress);
 }
 
 } // namespace

@@ -138,6 +138,21 @@ DXB200_API int32_t  dxb200_generate_mipmaps_device(const dxb200_image* chain, si
  * to the source up and the blocks down.  filter as dxb200_generate_mipmaps, flags / threshold as dxb200_compress. */
 DXB200_API int32_t  dxb200_mipmaps_compress(const dxb200_image* base, size_t items, size_t levels, uint32_t filter, uint32_t dstFormat,
                                  uint32_t flags, float threshold, float alphaWeight, const dxb200_image* dst);
+/* The steps texconv runs between GenerateMipMaps and Compress, done in device memory by dxb200_mipmaps_compress_ex on every chain
+ * after its mips and before its compression, in this order (Texconv/texconv.cpp:3480, 3526). */
+typedef struct dxb200_chain_steps
+{
+    float    alphaReference;  /* > 0: ScaleMipMapsAlphaForCoverage of every item at this reference (texconv :3304, :3480); <= 0: skipped */
+    uint32_t premultiply;     /* nonzero: PremultiplyAlpha of every image of every chain with pmalphaFlags (texconv :3526) */
+    uint32_t pmalphaFlags;    /* TEX_PMALPHA_FLAGS, as dxb200_premultiply_alpha */
+} dxb200_chain_steps;
+/* dxb200_mipmaps_compress with `steps` (NULL: none, exactly dxb200_mipmaps_compress).  Results are identical to
+ * dxb200_generate_mipmaps, then dxb200_scale_mipmaps_alpha_for_coverage per item, then dxb200_premultiply_alpha, then
+ * dxb200_compress; every argument is checked before anything is uploaded, and the call returns the HRESULT of the first of those
+ * four calls that would fail.  Each chunk of items runs the coverage search of all its chains as 10 + 1 kernel launches. */
+DXB200_API int32_t  dxb200_mipmaps_compress_ex(const dxb200_image* base, size_t items, size_t levels, uint32_t filter,
+                                               const dxb200_chain_steps* steps, uint32_t dstFormat, uint32_t flags,
+                                               float threshold, float alphaWeight, const dxb200_image* dst);
 
 /* DirectX::Resize (DirectXTexResize.cpp:854-935 single image, :942-1120 arrays; custom filters ResizePointFilter /
  * ResizeBoxFilter / ResizeLinearFilter / ResizeCubicFilter / ResizeTriangleFilter :255-798, selection :805-837).
@@ -159,7 +174,8 @@ DXB200_API int32_t  dxb200_premultiply_alpha_device(const dxb200_image* src, siz
  * EstimateAlphaScaleForCoverage :310-355, ScaleAlpha :143-193) for ONE array item: src[0..nlevels) = its mip levels as
  * GenerateMipMaps produced them, dst[0..nlevels) = the same levels of the result.  Level 0 is copied; every other level's
  * alpha is scaled so that its alpha-test coverage at `alphaReference` matches level 0's (10-step bisection).
- * (SURVEY 8(f) rank 4.)  The _device variant synchronises `stream` internally (the bisection reads counts back). */
+ * (SURVEY 8(f) rank 4.)  The bisection runs on the device: 10 coverage launches and one scaling launch per call, with no
+ * host round trip in between.  The _device variant synchronises `stream` before it returns. */
 DXB200_API int32_t  dxb200_scale_mipmaps_alpha_for_coverage(const dxb200_image* src, size_t nlevels, float alphaReference, const dxb200_image* dst);
 DXB200_API int32_t  dxb200_scale_mipmaps_alpha_for_coverage_device(const dxb200_image* src, size_t nlevels, float alphaReference,
                                                                    const dxb200_image* dst, void* stream);
