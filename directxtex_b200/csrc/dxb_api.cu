@@ -566,6 +566,24 @@ int32_t launch_mips(const dxb200_image* chain, size_t items, size_t levels, uint
     return hr;
 }
 
+// ---- Decompress (DirectXTexCompress.cpp:852-979; DecompressBC :425-535) ---------------------------------
+int32_t launch_decompress(dxb_compress_params P, const dxb200_image* src, const dxb200_image* dst, size_t n, cudaStream_t stream)
+{
+    JobTable jt;
+    const int32_t hr = jt.build(src, dst, n, true, stream);
+    if (hr != DXB_S_OK) return hr;
+    P.totalUnits = jt.total; P.njobs = (uint32_t)n;
+    return check_launch(dxb_launch_decompress(grid_for(jt.total, 128, (uint32_t)t_v.dev->gridBC15 * 8u), stream, jt.dev.d, jt.host.data(), P));
+}
+
+// ---- Resize: a two-"level" chain per item whose second level has an arbitrary size ------------------------------------
+int32_t launch_resize(const dxb200_image* src, const dxb200_image* dst, size_t n, uint32_t filter, uint32_t mode, cudaStream_t stream)
+{
+    std::vector<dxb200_image> pairs(2 * n);
+    for (size_t i = 0; i < n; ++i) { pairs[2 * i] = src[i]; pairs[2 * i + 1] = dst[i]; }
+    return launch_mips(pairs.data(), n, 2, filter, mode, stream);
+}
+
 // ---- ScaleMipMapsAlphaForCoverage -------------------------------------------------------------------------------------
 // chains[it * levels + l] (DEVICE pointers) -> out[...]: levels >= 1 of every item scaled so that their alpha-test coverage at `ref`
 // matches level 0's; level 0 is not written.  Always DXB_COVERAGE_STEPS k_alpha_coverage launches and one k_scale_alpha, with
@@ -597,6 +615,54 @@ int32_t scale_alpha_for_coverage_device(const dxb200_image* src, size_t n, float
     DXB_CUDA(cudaMemcpy2DAsync(dst[0].pixels, dst[0].rowPitch, src[0].pixels, src[0].rowPitch, std::min(src[0].rowPitch, dst[0].rowPitch),
                                src[0].slicePitch / std::max<size_t>(src[0].rowPitch, 1), cudaMemcpyDeviceToDevice, st));
     return launch_coverage(src, dst, 1, n, ref, st);
+}
+
+// ---- [Decompress] -> [Resize] -> GenerateMipMaps -> [coverage] -> [premultiply] -> Compress, chunk by chunk ---------------------
+// texconv runs GenerateMipMaps and then Compress on the result (Texconv/texconv.cpp; SURVEY 3.5), after Decompress (:2316-2480) for
+// a BC input and Resize (:2576-2643) for a new size; with the host-pointer calls every intermediate travels device -> host ->
+// device.  Here each item's base goes up once, every step runs in device memory and only the packed blocks come back: 4 B/texel
+// up + 1.33 B/texel down for BC3 from RGBA8 instead of 4 + 5.33 + 5.33 + 1.33.  Chunks of whole items are pipelined over the
+// lane's NSLOT (stream, buffer) slots.  A chunk holds, per item and in plane order: the base as the caller laid it out (when a
+// front step reads it), the decompressed image (only when a resize follows), the chain (level 0 uploaded when no front step writes
+// it) and the blocks.  With no front step that is exactly the chain and the blocks.
+int32_t run_chains(const dxb200_image* base, size_t items, size_t levels, uint32_t filter, const FromPlan& fp, const dxb200_image* dst)
+{
+    const ChainPlan& cp = fp.chain;
+    const bool front = fp.decompress || fp.resize, mid = fp.decompress && fp.resize;
+    return run_sharded(items, [&](size_t i) { return cp.chain[i * levels].slicePitch; },
+        [&](size_t lo, size_t hi)
+        {
+            std::vector<Plane> planes;
+            if (front) planes.push_back({ base + lo, 1, Copy::Up, Copy::Up });
+            if (mid) planes.push_back({ fp.decompressed.data() + lo, 1, Copy::None, Copy::None });
+            planes.push_back({ cp.chain.data() + lo * levels, levels, front ? Copy::None : Copy::Up, Copy::None });
+            planes.push_back({ dst + lo * levels, levels, Copy::Down, Copy::Down });
+            return run_staged(planes.data(), planes.size(), hi - lo, ITEM_CHUNK,
+                [&](const std::vector<dxb200_image>* dev, size_t cnt, cudaStream_t st)
+                {
+                    const dxb200_image* src = front ? dev[0].data() : nullptr;
+                    const dxb200_image* decompressed = mid ? dev[1].data() : nullptr;
+                    const dxb200_image* chains = dev[planes.size() - 2].data();
+                    int32_t h2 = DXB_S_OK;
+                    std::vector<dxb200_image> level(cnt);
+                    if (front)
+                    {
+                        for (size_t it = 0; it < cnt; ++it) level[it] = chains[it * levels];
+                        if (fp.decompress) h2 = launch_decompress(fp.dp, src, mid ? decompressed : level.data(), cnt, st);
+                        if (h2 == DXB_S_OK && fp.resize) h2 = launch_resize(mid ? decompressed : src, level.data(), cnt, fp.resizeFilter, fp.resizeMode, st);
+                    }
+                    if (h2 == DXB_S_OK) h2 = launch_mips(chains, cnt, levels, filter, cp.mode, st);
+                    if (h2 == DXB_S_OK && cp.coverage) h2 = launch_coverage(chains, chains, cnt, levels, cp.ref, st);
+                    // one launch per level: the chunk's images of a level are equal, as the separate calls' images are, so they take the
+                    // same premultiply kernel
+                    for (size_t l = 0; l < levels && h2 == DXB_S_OK && cp.premultiply; ++l)
+                    {
+                        for (size_t it = 0; it < cnt; ++it) level[it] = chains[it * levels + l];
+                        h2 = launch_pmalpha(cp.pm, level.data(), level.data(), cnt, st);
+                    }
+                    return h2 != DXB_S_OK ? h2 : launch_compress(cp.compress, chains, dev[planes.size() - 1].data(), cnt * levels, st);
+                });
+        });
 }
 
 } // namespace
@@ -755,15 +821,6 @@ int32_t dxb200_compress(const dxb200_image* src, size_t nimages, uint32_t dstFor
 }
 
 // ---- Decompress (DirectXTexCompress.cpp:852-979; DecompressBC :425-535) ---------------------------------
-static int32_t launch_decompress(dxb_compress_params P, const dxb200_image* src, const dxb200_image* dst, size_t n, cudaStream_t stream)
-{
-    JobTable jt;
-    const int32_t hr = jt.build(src, dst, n, true, stream);
-    if (hr != DXB_S_OK) return hr;
-    P.totalUnits = jt.total; P.njobs = (uint32_t)n;
-    return check_launch(dxb_launch_decompress(grid_for(jt.total, 128, (uint32_t)t_v.dev->gridBC15 * 8u), stream, jt.dev.d, jt.host.data(), P));
-}
-
 int32_t dxb200_decompress_device(const dxb200_image* src, size_t nimages, uint32_t dstFormat, const dxb200_image* dst, void* stream)
 {
     dxb_compress_params P;
@@ -846,42 +903,25 @@ int32_t dxb200_generate_mipmaps(const dxb200_image* chain, size_t items, size_t 
         });
 }
 
-// ---- GenerateMipMaps + Compress in one call: the mip chain never leaves HBM --------------------------------------------
-// texconv runs GenerateMipMaps and then Compress on the result (Texconv/texconv.cpp; SURVEY 3.5); with the two host-pointer calls
-// the chain travels device -> host -> device in between.  Here level 0 of every item goes up once, the chain is built and
-// compressed in device memory, and only the packed blocks come back: 4 B/texel up + 1.33 B/texel down (BC3 from RGBA8)
-// instead of 4 + 5.33 + 5.33 + 1.33.  Per item: base[i] = level 0 (host), dst[i * levels + l] = the BC image of level l (host).
-// Chunks of whole items are pipelined over the lane's NSLOT (stream, buffer) slots: H2D, mip kernels, compress kernel, D2H.
-// dxb200_mipmaps_compress_ex adds texconv's two steps between the mips and the compression (-keepcoverage :3480, -pmalpha :3526),
-// both in place on the chunk's chains in device memory.
+// ---- GenerateMipMaps + Compress in one call: the mip chain never leaves HBM (run_chains) --------------------------------
+// Per item: base[i] = level 0 (host), dst[i * levels + l] = the BC image of level l (host).  dxb200_mipmaps_compress_ex adds
+// texconv's two steps between the mips and the compression (-keepcoverage :3480, -pmalpha :3526), both in place on the chunk's
+// chains in device memory; dxb200_mipmaps_compress_from adds Decompress and Resize in front of the mips.
+int32_t dxb200_mipmaps_compress_from(const dxb200_image* base, size_t items, const dxb200_chain_source* source, size_t levels, uint32_t filter,
+                                     const dxb200_chain_steps* steps, uint32_t dstFormat, uint32_t flags, float threshold, float alphaWeight,
+                                     const dxb200_image* dst)
+{
+    (void)alphaWeight;
+    FromPlan fp;
+    const int32_t hr = plan_mipmaps_compress_from(base, items, source, levels, filter, steps, dstFormat, flags, threshold, dst, &fp);
+    if (hr != DXB_S_OK) return hr;
+    return run_chains(base, items, levels, filter, fp, dst);
+}
+
 int32_t dxb200_mipmaps_compress_ex(const dxb200_image* base, size_t items, size_t levels, uint32_t filter, const dxb200_chain_steps* steps,
                                    uint32_t dstFormat, uint32_t flags, float threshold, float alphaWeight, const dxb200_image* dst)
 {
-    (void)alphaWeight;
-    ChainPlan cp;
-    const int32_t hr = plan_mipmaps_compress(base, items, levels, filter, steps, dstFormat, flags, threshold, dst, &cp);
-    if (hr != DXB_S_OK) return hr;
-    return run_sharded(items, [&](size_t i) { return base[i].slicePitch; },
-        [&](size_t lo, size_t hi)
-        {
-            const Plane planes[2] = { { cp.chain.data() + lo * levels, levels, Copy::Up, Copy::None }, { dst + lo * levels, levels, Copy::Down, Copy::Down } };
-            return run_staged(planes, 2, hi - lo, ITEM_CHUNK,
-                [&](const std::vector<dxb200_image>* dev, size_t cnt, cudaStream_t st)
-                {
-                    const dxb200_image* chains = dev[0].data();
-                    int32_t h2 = launch_mips(chains, cnt, levels, filter, cp.mode, st);
-                    if (h2 == DXB_S_OK && cp.coverage) h2 = launch_coverage(chains, chains, cnt, levels, cp.ref, st);
-                    // one launch per level: the chunk's images of a level are equal, as the separate calls' images are, so they take the
-                    // same premultiply kernel
-                    std::vector<dxb200_image> level(cnt);
-                    for (size_t l = 0; l < levels && h2 == DXB_S_OK && cp.premultiply; ++l)
-                    {
-                        for (size_t it = 0; it < cnt; ++it) level[it] = chains[it * levels + l];
-                        h2 = launch_pmalpha(cp.pm, level.data(), level.data(), cnt, st);
-                    }
-                    return h2 != DXB_S_OK ? h2 : launch_compress(cp.compress, chains, dev[1].data(), cnt * levels, st);
-                });
-        });
+    return dxb200_mipmaps_compress_from(base, items, nullptr, levels, filter, steps, dstFormat, flags, threshold, alphaWeight, dst);
 }
 
 int32_t dxb200_mipmaps_compress(const dxb200_image* base, size_t items, size_t levels, uint32_t filter, uint32_t dstFormat,
@@ -954,14 +994,6 @@ int32_t dxb200_scale_mipmaps_alpha_for_coverage(const dxb200_image* src, size_t 
                                        src[l].slicePitch / std::max<size_t>(src[l].rowPitch, 1), cudaMemcpyDeviceToHost, st), "D2H");
     if (hr == DXB_S_OK) hr = cuda_hr(cudaStreamSynchronize(st), "alpha coverage sync");
     return hr;
-}
-
-// a resize is a two-"level" chain per item whose second level has an arbitrary size
-static int32_t launch_resize(const dxb200_image* src, const dxb200_image* dst, size_t n, uint32_t filter, uint32_t mode, cudaStream_t stream)
-{
-    std::vector<dxb200_image> pairs(2 * n);
-    for (size_t i = 0; i < n; ++i) { pairs[2 * i] = src[i]; pairs[2 * i + 1] = dst[i]; }
-    return launch_mips(pairs.data(), n, 2, filter, mode, stream);
 }
 
 int32_t dxb200_resize_device(const dxb200_image* src, size_t nimages, uint32_t filter, const dxb200_image* dst, void* stream)

@@ -216,6 +216,24 @@ DXB_FMT_FN int dxb_is_srgb_format(uint32_t fmt)
     }
 }
 
+// The format Decompress writes when it is asked for DXGI_FORMAT_UNKNOWN (DefaultDecompress, DirectXTexCompress.cpp:377-421);
+// UNKNOWN for a format that is not BC.
+DXB_FMT_FN uint32_t dxb_default_decompress(uint32_t fmt)
+{
+    switch (fmt)
+    {
+    case DXB_FMT_BC1_UNORM: case DXB_FMT_BC2_UNORM: case DXB_FMT_BC3_UNORM: case DXB_FMT_BC7_UNORM: return DXB_FMT_R8G8B8A8_UNORM;
+    case DXB_FMT_BC1_UNORM_SRGB: case DXB_FMT_BC2_UNORM_SRGB: case DXB_FMT_BC3_UNORM_SRGB: case DXB_FMT_BC7_UNORM_SRGB:
+        return DXB_FMT_R8G8B8A8_UNORM_SRGB;
+    case DXB_FMT_BC4_UNORM: return DXB_FMT_R8_UNORM;
+    case DXB_FMT_BC4_SNORM: return DXB_FMT_R8_SNORM;
+    case DXB_FMT_BC5_UNORM: return DXB_FMT_R8G8_UNORM;
+    case DXB_FMT_BC5_SNORM: return DXB_FMT_R8G8_SNORM;
+    case DXB_FMT_BC6H_UF16: case DXB_FMT_BC6H_SF16: return DXB_FMT_R32G32B32A32_FLOAT;
+    default: return DXB_FMT_UNKNOWN;
+    }
+}
+
 // Resolve the sRGB bits exactly as ConvertScanline does (DirectXTexConvert.cpp:3121-3167).
 // conversion flags CompressBC passes for a BC1-5 target when the caller gives no sRGB flags and source/target agree
 // on sRGB-ness (DetermineEncoderSettings, DirectXTexCompress.cpp:46-68)

@@ -384,4 +384,64 @@ int32_t plan_mipmaps_compress(const dxb200_image* base, size_t items, size_t lev
     return plan_compress(chain.data(), items * levels, dstFormat, flags, threshold, dst, &cp->compress);
 }
 
+// ---- Decompress -> Resize -> mipmaps_compress_ex in one call (mipmaps_compress_from) -----------------------------------------
+// The per-item device images: base[i] (the caller's, BC or not, at its pitch), decompressed[i] (the base's size in the decompress
+// format at compute_pitch; in the buffer only when a resize follows, else it is level 0 of the chain), the chain (level 0 = W x H
+// at compute_pitch when a front step writes it) and the blocks.  Images the device makes carry base[i].pixels only for validation.
+struct FromPlan
+{
+    bool decompress, resize;
+    dxb_compress_params dp;                     // the Decompress
+    std::vector<dxb200_image> decompressed;
+    uint32_t resizeFilter, resizeMode;          // the Resize, into level 0 of the chain
+    ChainPlan chain;
+};
+
+// image i of `n` of format fmt, w x h, at compute_pitch, with the pixels of base[i]
+std::vector<dxb200_image> plan_images(const dxb200_image* base, size_t n, uint32_t fmt, size_t w, size_t h)
+{
+    std::vector<dxb200_image> out(n);
+    for (size_t i = 0; i < n; ++i)
+    {
+        dxb200_image& im = out[i];
+        im.width = w ? w : base[i].width; im.height = h ? h : base[i].height; im.format = fmt; im.rowPitch = im.slicePitch = 0;
+        (void)compute_pitch(fmt, im.width, im.height, &im.rowPitch, &im.slicePitch);      // a format no pitch exists for is refused below
+        im.pixels = base[i].pixels;
+    }
+    return out;
+}
+
+// Every check of Decompress, Resize and the four steps of plan_mipmaps_compress before anything is uploaded, each with the HRESULT of
+// the first of the separate calls that would fail.  source == nullptr, or a source that changes nothing = plan_mipmaps_compress.
+int32_t plan_mipmaps_compress_from(const dxb200_image* base, size_t items, const dxb200_chain_source* source, size_t levels, uint32_t filter,
+                                   const dxb200_chain_steps* steps, uint32_t dstFormat, uint32_t flags, float threshold, const dxb200_image* dst,
+                                   FromPlan* fp)
+{
+    fp->decompress = fp->resize = false;
+    fp->resizeFilter = fp->resizeMode = 0;
+    fp->decompressed.clear();
+    if (source && (!source->width) != (!source->height)) return DXB_E_INVALIDARG;
+    if (!source || !base || !items) return plan_mipmaps_compress(base, items, levels, filter, steps, dstFormat, flags, threshold, dst, &fp->chain);
+    const size_t w = source->width ? source->width : base[0].width, h = source->height ? source->height : base[0].height;
+    fp->decompress = is_compressed(base[0].format);
+    fp->resize = (w != base[0].width || h != base[0].height);
+    std::vector<dxb200_image> level0(base, base + items);
+    int32_t hr = DXB_S_OK;
+    if (fp->decompress)
+    {
+        const uint32_t fmt = source->decompressFormat ? source->decompressFormat : dxb_default_decompress(base[0].format);
+        fp->decompressed = plan_images(base, items, fmt, 0, 0);
+        if ((hr = plan_decompress(base, items, fmt, fp->decompressed.data(), &fp->dp)) != DXB_S_OK) return hr;
+        level0 = fp->decompressed;
+    }
+    if (fp->resize)
+    {
+        const std::vector<dxb200_image> resized = plan_images(base, items, level0[0].format, w, h);
+        if ((hr = plan_resize(level0.data(), items, source->resizeFilter, resized.data(), &fp->resizeMode)) != DXB_S_OK) return hr;
+        fp->resizeFilter = source->resizeFilter;
+        level0 = resized;
+    }
+    return plan_mipmaps_compress(level0.data(), items, levels, filter, steps, dstFormat, flags, threshold, dst, &fp->chain);
+}
+
 } // namespace

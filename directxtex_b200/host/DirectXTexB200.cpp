@@ -5,6 +5,7 @@
 // ScratchImage DirectXTexImage.cpp:300-455, TexMetadata::ComputeIndex DirectXTexUtil.cpp:1695-1741.
 #include "DirectXTexB200.h"
 #include "../../include/dxtex_b200.h"
+#include "../csrc/dxb_formats.h"
 
 #include <algorithm>
 #include <cstdio>
@@ -576,17 +577,7 @@ HRESULT Decompress(const Image& cImage, DXGI_FORMAT format, ScratchImage& image)
 {
     if (!IsCompressed(cImage.format) || IsCompressed(format)) return E_INVALIDARG;
     if (format == DXGI_FORMAT_UNKNOWN)
-    {
-        switch (cImage.format)         // DefaultDecompress, DirectXTexCompress.cpp:377-421
-        {
-        case DXGI_FORMAT_BC4_UNORM: format = DXGI_FORMAT_R8_UNORM; break;
-        case DXGI_FORMAT_BC4_SNORM: format = DXGI_FORMAT_R8_SNORM; break;
-        case DXGI_FORMAT_BC5_UNORM: format = DXGI_FORMAT_R8G8_UNORM; break;
-        case DXGI_FORMAT_BC5_SNORM: format = DXGI_FORMAT_R8G8_SNORM; break;
-        case DXGI_FORMAT_BC6H_UF16: case DXGI_FORMAT_BC6H_SF16: format = DXGI_FORMAT_R32G32B32A32_FLOAT; break;
-        default: format = IsSRGB(cImage.format) ? DXGI_FORMAT_R8G8B8A8_UNORM_SRGB : DXGI_FORMAT_R8G8B8A8_UNORM; break;
-        }
-    }
+        format = static_cast<DXGI_FORMAT>(dxb_default_decompress(static_cast<uint32_t>(cImage.format)));     // DefaultDecompress
     HRESULT hr = image.Initialize2D(format, cImage.width, cImage.height, 1, 1);
     if (FAILED(hr)) return hr;
     const dxb200_image s = to_c(cImage), d = to_c(*image.GetImage(0, 0, 0));

@@ -153,6 +153,25 @@ typedef struct dxb200_chain_steps
 DXB200_API int32_t  dxb200_mipmaps_compress_ex(const dxb200_image* base, size_t items, size_t levels, uint32_t filter,
                                                const dxb200_chain_steps* steps, uint32_t dstFormat, uint32_t flags,
                                                float threshold, float alphaWeight, const dxb200_image* dst);
+/* texconv's steps in front of GenerateMipMaps, run in device memory by dxb200_mipmaps_compress_from on every item before its
+ * mips, in this order: Decompress (Texconv/texconv.cpp:2316-2480), Resize (:2576-2643). */
+typedef struct dxb200_chain_source
+{
+    uint32_t decompressFormat;  /* base in a BC format: Decompress it to this DXGI format first; 0 (UNKNOWN) = DefaultDecompress
+                                   (DirectXTexCompress.cpp:377-421).  Ignored for an uncompressed base. */
+    size_t   width, height;     /* level 0 of every chain; both 0 = the base's size.  A base of another size is Resized to it. */
+    uint32_t resizeFilter;      /* TEX_FILTER_FLAGS of that Resize (texconv passes its mip filter flags) */
+} dxb200_chain_source;
+/* dxb200_mipmaps_compress_ex of items as they were loaded: base[i] = item i (host), BC or uncompressed, all items of one format
+ * and one size; dst[i * levels + l] laid out as ScratchImage::Initialize2D(dstFormat, W, H, items, levels) would, W x H = the
+ * chain's level 0.  Results are identical to dxb200_decompress (base -> decompressFormat, if the base is BC), then dxb200_resize
+ * (-> W x H with resizeFilter, if the size differs), then dxb200_mipmaps_compress_ex; the decompressed and resized images
+ * never leave device memory, so the base goes up and only the blocks come down.  Every argument of every step is checked before
+ * anything is uploaded, and the call returns the HRESULT of the first of those calls that would fail.  source == NULL, or a
+ * source that changes nothing, is exactly dxb200_mipmaps_compress_ex; only one of width / height 0 -> E_INVALIDARG. */
+DXB200_API int32_t  dxb200_mipmaps_compress_from(const dxb200_image* base, size_t items, const dxb200_chain_source* source,
+                                                 size_t levels, uint32_t filter, const dxb200_chain_steps* steps, uint32_t dstFormat,
+                                                 uint32_t flags, float threshold, float alphaWeight, const dxb200_image* dst);
 
 /* DirectX::Resize (DirectXTexResize.cpp:854-935 single image, :942-1120 arrays; custom filters ResizePointFilter /
  * ResizeBoxFilter / ResizeLinearFilter / ResizeCubicFilter / ResizeTriangleFilter :255-798, selection :805-837).
