@@ -11,10 +11,11 @@ LIB_PATH = os.environ.get("DXTEX_B200_LIB") or os.path.join(_HERE, "_lib", "libd
 SYMBOLS = [
     "dxb200_version", "dxb200_init", "dxb200_init_devices", "dxb200_initialized_devices", "dxb200_shutdown", "dxb200_device_count", "dxb200_launch_count", "dxb200_tma_launch_count", "dxb200_kernel_launch_count", "dxb200_set_option", "dxb200_get_option", "dxb200_last_error",
     "dxb200_host_alloc", "dxb200_host_free", "dxb200_compute_pitch", "dxb200_calculate_mip_levels",
-    "dxb200_compress", "dxb200_compress_ex", "dxb200_compress_device", "dxb200_convert_ex", "dxb200_mipmaps_compress", "dxb200_mipmaps_compress_ex", "dxb200_mipmaps_compress_from", "dxb200_decompress", "dxb200_decompress_device",
+    "dxb200_compress", "dxb200_compress_ex", "dxb200_compress_device", "dxb200_convert_ex", "dxb200_mipmaps_compress", "dxb200_mipmaps_compress_ex", "dxb200_mipmaps_compress_from", "dxb200_mipmaps_compress_from_ex", "dxb200_decompress", "dxb200_decompress_device",
     "dxb200_convert", "dxb200_convert_device", "dxb200_generate_mipmaps", "dxb200_generate_mipmaps_device",
     "dxb200_resize", "dxb200_resize_device", "dxb200_premultiply_alpha", "dxb200_premultiply_alpha_device",
     "dxb200_scale_mipmaps_alpha_for_coverage", "dxb200_scale_mipmaps_alpha_for_coverage_device",
+    "dxb200_is_alpha_all_opaque", "dxb200_is_alpha_all_opaque_device",
     "dxb200_dds_encode_header", "dxb200_dds_save_memory", "dxb200_dds_get_metadata", "dxb200_dds_load_memory",
 ]
 
@@ -80,6 +81,9 @@ def _load():
                                                C.c_float, IP]
     lib.dxb200_mipmaps_compress_from.argtypes = [IP, C.c_size_t, C.POINTER(ChainSource), C.c_size_t, C.c_uint32, C.POINTER(ChainSteps), C.c_uint32,
                                                  C.c_uint32, C.c_float, C.c_float, IP]
+    lib.dxb200_mipmaps_compress_from_ex.argtypes = lib.dxb200_mipmaps_compress_from.argtypes + [C.POINTER(C.c_int32)]
+    lib.dxb200_is_alpha_all_opaque.argtypes = [IP, C.c_size_t, C.POINTER(C.c_int32)]
+    lib.dxb200_is_alpha_all_opaque_device.argtypes = [IP, C.c_size_t, C.POINTER(C.c_int32), C.c_void_p]
     lib.dxb200_compute_pitch.argtypes = [C.c_uint32, C.c_size_t, C.c_size_t, C.POINTER(C.c_size_t), C.POINTER(C.c_size_t)]
     lib.dxb200_calculate_mip_levels.argtypes = [C.c_size_t, C.c_size_t, C.POINTER(C.c_size_t)]
     lib.dxb200_compress.argtypes = [IP, C.c_size_t, C.c_uint32, C.c_uint32, C.c_float, C.c_float, IP]
@@ -105,7 +109,7 @@ def _load():
     lib.dxb200_dds_load_memory.argtypes = [C.c_void_p, C.c_size_t, C.c_uint32, IP, C.c_size_t]
     for name in ("dxb200_dds_encode_header", "dxb200_dds_save_memory", "dxb200_dds_get_metadata", "dxb200_dds_load_memory"):
         getattr(lib, name).restype = C.c_int32
-    for name in ("dxb200_init", "dxb200_init_devices", "dxb200_initialized_devices", "dxb200_compress_ex", "dxb200_convert_ex", "dxb200_mipmaps_compress", "dxb200_mipmaps_compress_ex", "dxb200_mipmaps_compress_from", "dxb200_device_count", "dxb200_compute_pitch", "dxb200_calculate_mip_levels", "dxb200_compress",
+    for name in ("dxb200_init", "dxb200_init_devices", "dxb200_initialized_devices", "dxb200_compress_ex", "dxb200_convert_ex", "dxb200_mipmaps_compress", "dxb200_mipmaps_compress_ex", "dxb200_mipmaps_compress_from", "dxb200_mipmaps_compress_from_ex", "dxb200_is_alpha_all_opaque", "dxb200_is_alpha_all_opaque_device", "dxb200_device_count", "dxb200_compute_pitch", "dxb200_calculate_mip_levels", "dxb200_compress",
                  "dxb200_compress_device", "dxb200_decompress", "dxb200_decompress_device", "dxb200_convert",
                  "dxb200_convert_device", "dxb200_generate_mipmaps", "dxb200_generate_mipmaps_device", "dxb200_resize", "dxb200_resize_device", "dxb200_premultiply_alpha", "dxb200_premultiply_alpha_device"):
         getattr(lib, name).restype = C.c_int32
@@ -214,10 +218,8 @@ def chain_source(decompress_format=0, width=0, height=0, resize_filter=0):
     return ChainSource(decompress_format, width, height, resize_filter)
 
 
-def mipmaps_compress_from(bases, w, h, base_fmt, dst_fmt, source=None, filter=0, levels=0, flags=0, steps=None, row_pitch=0):
-    """dxb200_mipmaps_compress_from of an array of equally sized w x h host images of base_fmt (BC or not; rows row_pitch bytes
-    apart, 0 = tight) with the ChainSource `source` and the ChainSteps `steps` (None: none); returns one packed BC chain (bytes)
-    per image, of the chain's level 0 size (source's width x height, or w x h)"""
+def _from_args(bases, w, h, base_fmt, dst_fmt, source, filter, levels, flags, steps, row_pitch):
+    """(the arguments of dxb200_mipmaps_compress_from, the output arrays)"""
     bases = [np.ascontiguousarray(a).view(np.uint8).reshape(-1) for a in bases]
     cw, ch = (source.width, source.height) if source is not None and source.width else (w, h)
     levels = levels or F.count_mips(cw, ch)
@@ -225,11 +227,40 @@ def mipmaps_compress_from(bases, w, h, base_fmt, dst_fmt, source=None, filter=0,
     outs = [np.zeros(total, np.uint8) for _ in bases]
     s = images([make_image(_np_ptr(a), w, h, base_fmt, row_pitch) for a in bases])
     d = images([Image(lw, lh, dst_fmt, r, sp, _np_ptr(o) + off) for o in outs for (off, lw, lh, r, sp) in olayout])
-    hr = lib.dxb200_mipmaps_compress_from(s, len(bases), C.byref(source) if source is not None else None, levels, filter,
-                                          C.byref(steps) if steps is not None else None, dst_fmt, flags, 0.5, 1.0, d)
+    return (s, len(bases), C.byref(source) if source is not None else None, levels, filter, C.byref(steps) if steps is not None else None,
+            dst_fmt, flags, 0.5, 1.0, d), outs
+
+
+def mipmaps_compress_from(bases, w, h, base_fmt, dst_fmt, source=None, filter=0, levels=0, flags=0, steps=None, row_pitch=0):
+    """dxb200_mipmaps_compress_from of an array of equally sized w x h host images of base_fmt (BC or not; rows row_pitch bytes
+    apart, 0 = tight) with the ChainSource `source` and the ChainSteps `steps` (None: none); returns one packed BC chain (bytes)
+    per image, of the chain's level 0 size (source's width x height, or w x h)"""
+    args, outs = _from_args(bases, w, h, base_fmt, dst_fmt, source, filter, levels, flags, steps, row_pitch)
+    hr = lib.dxb200_mipmaps_compress_from(*args)
     if hr != 0:
         raise DxTexError(hr, "dxb200_mipmaps_compress_from")
     return outs
+
+
+def mipmaps_compress_from_ex(bases, w, h, base_fmt, dst_fmt, source=None, filter=0, levels=0, flags=0, steps=None, row_pitch=0):
+    """mipmaps_compress_from through dxb200_mipmaps_compress_from_ex: (the chains, IsAlphaAllOpaque of the output as a bool)"""
+    args, outs = _from_args(bases, w, h, base_fmt, dst_fmt, source, filter, levels, flags, steps, row_pitch)
+    opaque = C.c_int32(-1)
+    hr = lib.dxb200_mipmaps_compress_from_ex(*args, C.byref(opaque))
+    if hr != 0:
+        raise DxTexError(hr, "dxb200_mipmaps_compress_from_ex")
+    return outs, opaque.value == 1
+
+
+def is_alpha_all_opaque(arrays, w, h, fmt, row_pitch=0):
+    """dxb200_is_alpha_all_opaque of equally sized w x h host images of fmt (rows row_pitch bytes apart, 0 = tight): a bool"""
+    arrays = [np.ascontiguousarray(a) for a in arrays]
+    s = images([make_image(_np_ptr(a), w, h, fmt, row_pitch) for a in arrays])
+    opaque = C.c_int32(-1)
+    hr = lib.dxb200_is_alpha_all_opaque(s, len(arrays), C.byref(opaque))
+    if hr != 0:
+        raise DxTexError(hr, "dxb200_is_alpha_all_opaque")
+    return opaque.value == 1
 
 
 def compress_array(srcs, w, h, src_fmt, dst_fmt, flags=0, threshold=0.5):

@@ -617,6 +617,54 @@ int32_t scale_alpha_for_coverage_device(const dxb200_image* src, size_t n, float
     return launch_coverage(src, dst, 1, n, ref, st);
 }
 
+// ---- IsAlphaAllOpaque (DirectXTexImage.cpp:800-852; IsAlphaAllOpaqueBC, DirectXTexCompress.cpp:539-621) -------------------------
+// src (DEVICE pointers) scanned into words[i] (DEVICE, one 32-bit word per job, several jobs may share one; zero before the launch):
+// 1 when a texel of src[i] is not opaque, untouched otherwise.  One launch of the generic k_decompress (BC) or k_convert.
+int32_t launch_alpha_opaque(const AlphaOpaquePlan& ap, const dxb200_image* src, const dxb200_image* words, size_t n, cudaStream_t stream)
+{
+    JobTable jt;
+    const int32_t hr = jt.build(src, words, n, ap.blocks, stream);
+    if (hr != DXB_S_OK) return hr;
+    const Device& d = *t_v.dev;
+    if (ap.blocks)
+        return check_launch(dxb_launch_alpha_opaque_blocks(grid_for(jt.total, 128, (uint32_t)d.gridBC15 * 8u), stream, jt.dev.d, jt.host.data(),
+                                                          alpha_opaque_block_params(ap, jt.total, (uint32_t)n)));
+    return check_launch(dxb_launch_alpha_opaque_pixels(grid_for(jt.total, 256, (uint32_t)d.gridRow * 8u), stream, jt.dev.d, jt.host.data(),
+                                                      alpha_opaque_pixel_params(ap, jt.total, (uint32_t)n)));
+}
+
+// the result words of a staged plane: one per item, 256 bytes apart in the chunk's buffer with nothing in between, so one memset
+// clears them all
+int32_t clear_words(const std::vector<dxb200_image>& words, cudaStream_t stream)
+{
+    const size_t span = (size_t)(words.back().pixels - words.front().pixels) + sizeof(uint32_t);
+    return cuda_hr(cudaMemsetAsync(words.front().pixels, 0, span, stream), "cudaMemsetAsync(alpha words)");
+}
+
+// The host side of a scan's staged result plane: one 32-bit word per item, in pinned memory.  A download into pageable memory
+// returns only when the copy is done, i.e. when the chunk's kernels are, so it would hold back the uploads of the next chunks
+// (64 x 1024^2 BC3 -> BC7 chains through mipmaps_compress_from_ex on an H100: 31.7 ms with pageable words, 28.7 ms pinned).
+struct ResultWords
+{
+    uint32_t* w = nullptr; size_t n = 0;
+    ~ResultWords() { if (w) cudaFreeHost(w); }
+    int32_t alloc(size_t count)
+    {
+        DXB_CUDA(cudaHostAlloc(reinterpret_cast<void**>(&w), std::max<size_t>(count, 1) * sizeof(uint32_t), cudaHostAllocPortable));
+        n = count;
+        memset(w, 0, n * sizeof(uint32_t));
+        return DXB_S_OK;
+    }
+    // the plane's host images: word i as a 1 x 1 image of 4 bytes
+    std::vector<dxb200_image> images() const
+    {
+        std::vector<dxb200_image> out(n);
+        for (size_t i = 0; i < n; ++i) out[i] = { 1, 1, DXB_FMT_UNKNOWN, sizeof(uint32_t), sizeof(uint32_t), reinterpret_cast<uint8_t*>(w + i) };
+        return out;
+    }
+    bool all_zero() const { return std::all_of(w, w + n, [](uint32_t v) { return v == 0; }); }
+};
+
 // ---- [Decompress] -> [Resize] -> GenerateMipMaps -> [coverage] -> [premultiply] -> Compress, chunk by chunk ---------------------
 // texconv runs GenerateMipMaps and then Compress on the result (Texconv/texconv.cpp; SURVEY 3.5), after Decompress (:2316-2480) for
 // a BC input and Resize (:2576-2643) for a new size; with the host-pointer calls every intermediate travels device -> host ->
@@ -624,25 +672,32 @@ int32_t scale_alpha_for_coverage_device(const dxb200_image* src, size_t n, float
 // up + 1.33 B/texel down for BC3 from RGBA8 instead of 4 + 5.33 + 5.33 + 1.33.  Chunks of whole items are pipelined over the
 // lane's NSLOT (stream, buffer) slots.  A chunk holds, per item and in plane order: the base as the caller laid it out (when a
 // front step reads it), the decompressed image (only when a resize follows), the chain (level 0 uploaded when no front step writes
-// it) and the blocks.  With no front step that is exactly the chain and the blocks.
-int32_t run_chains(const dxb200_image* base, size_t items, size_t levels, uint32_t filter, const FromPlan& fp, const dxb200_image* dst)
+// it) and the blocks.  With no front step that is exactly the chain and the blocks.  With a scan (words != nullptr: one result word
+// per item, see dxb200_mipmaps_compress_from_ex) one more plane holds the items' words; they are cleared, set by one scan launch
+// over all the chunk's blocks after the compression, and come back with the blocks.
+int32_t run_chains(const dxb200_image* base, size_t items, size_t levels, uint32_t filter, const FromPlan& fp, const dxb200_image* dst,
+                   const AlphaOpaquePlan& scan, const ResultWords* words)
 {
     const ChainPlan& cp = fp.chain;
     const bool front = fp.decompress || fp.resize, mid = fp.decompress && fp.resize;
+    const std::vector<dxb200_image> wimg = words ? words->images() : std::vector<dxb200_image>();
     return run_sharded(items, [&](size_t i) { return cp.chain[i * levels].slicePitch; },
         [&](size_t lo, size_t hi)
         {
             std::vector<Plane> planes;
             if (front) planes.push_back({ base + lo, 1, Copy::Up, Copy::Up });
             if (mid) planes.push_back({ fp.decompressed.data() + lo, 1, Copy::None, Copy::None });
+            const size_t pc = planes.size();                    // the chains' plane, then the blocks' and the words'
             planes.push_back({ cp.chain.data() + lo * levels, levels, front ? Copy::None : Copy::Up, Copy::None });
             planes.push_back({ dst + lo * levels, levels, Copy::Down, Copy::Down });
+            if (words) planes.push_back({ wimg.data() + lo, 1, Copy::Down, Copy::Down });
             return run_staged(planes.data(), planes.size(), hi - lo, ITEM_CHUNK,
                 [&](const std::vector<dxb200_image>* dev, size_t cnt, cudaStream_t st)
                 {
                     const dxb200_image* src = front ? dev[0].data() : nullptr;
                     const dxb200_image* decompressed = mid ? dev[1].data() : nullptr;
-                    const dxb200_image* chains = dev[planes.size() - 2].data();
+                    const dxb200_image* chains = dev[pc].data();
+                    const dxb200_image* blocks = dev[pc + 1].data();
                     int32_t h2 = DXB_S_OK;
                     std::vector<dxb200_image> level(cnt);
                     if (front)
@@ -660,7 +715,16 @@ int32_t run_chains(const dxb200_image* base, size_t items, size_t levels, uint32
                         for (size_t it = 0; it < cnt; ++it) level[it] = chains[it * levels + l];
                         h2 = launch_pmalpha(cp.pm, level.data(), level.data(), cnt, st);
                     }
-                    return h2 != DXB_S_OK ? h2 : launch_compress(cp.compress, chains, dev[planes.size() - 1].data(), cnt * levels, st);
+                    if (h2 == DXB_S_OK) h2 = launch_compress(cp.compress, chains, blocks, cnt * levels, st);
+                    if (h2 == DXB_S_OK && words)
+                    {
+                        const std::vector<dxb200_image>& w = dev[pc + 2];
+                        std::vector<dxb200_image> jobWords(cnt * levels);      // every level of an item sets the item's word
+                        for (size_t i = 0; i < jobWords.size(); ++i) jobWords[i] = w[i / levels];
+                        h2 = clear_words(w, st);
+                        if (h2 == DXB_S_OK) h2 = launch_alpha_opaque(scan, blocks, jobWords.data(), jobWords.size(), st);
+                    }
+                    return h2;
                 });
         });
 }
@@ -907,15 +971,30 @@ int32_t dxb200_generate_mipmaps(const dxb200_image* chain, size_t items, size_t 
 // Per item: base[i] = level 0 (host), dst[i * levels + l] = the BC image of level l (host).  dxb200_mipmaps_compress_ex adds
 // texconv's two steps between the mips and the compression (-keepcoverage :3480, -pmalpha :3526), both in place on the chunk's
 // chains in device memory; dxb200_mipmaps_compress_from adds Decompress and Resize in front of the mips.
+// dxb200_mipmaps_compress_from_ex adds texconv's "set alpha mode" test of the output (:3738-3766): IsAlphaAllOpaque of the blocks,
+// scanned where they were made.
+int32_t dxb200_mipmaps_compress_from_ex(const dxb200_image* base, size_t items, const dxb200_chain_source* source, size_t levels, uint32_t filter,
+                                        const dxb200_chain_steps* steps, uint32_t dstFormat, uint32_t flags, float threshold, float alphaWeight,
+                                        const dxb200_image* dst, int32_t* alphaAllOpaque)
+{
+    (void)alphaWeight;
+    FromPlan fp;
+    int32_t hr = plan_mipmaps_compress_from(base, items, source, levels, filter, steps, dstFormat, flags, threshold, dst, &fp);
+    if (hr != DXB_S_OK) return hr;
+    AlphaOpaquePlan ap = {};
+    if (alphaAllOpaque && (hr = plan_alpha_opaque(dst, items * levels, alphaAllOpaque, &ap)) != DXB_S_OK) return hr;
+    ResultWords words;
+    if (ap.scan && (hr = words.alloc(items)) != DXB_S_OK) return hr;
+    hr = run_chains(base, items, levels, filter, fp, dst, ap, ap.scan ? &words : nullptr);
+    if (hr == DXB_S_OK && alphaAllOpaque) *alphaAllOpaque = (!ap.scan || words.all_zero()) ? 1 : 0;
+    return hr;
+}
+
 int32_t dxb200_mipmaps_compress_from(const dxb200_image* base, size_t items, const dxb200_chain_source* source, size_t levels, uint32_t filter,
                                      const dxb200_chain_steps* steps, uint32_t dstFormat, uint32_t flags, float threshold, float alphaWeight,
                                      const dxb200_image* dst)
 {
-    (void)alphaWeight;
-    FromPlan fp;
-    const int32_t hr = plan_mipmaps_compress_from(base, items, source, levels, filter, steps, dstFormat, flags, threshold, dst, &fp);
-    if (hr != DXB_S_OK) return hr;
-    return run_chains(base, items, levels, filter, fp, dst);
+    return dxb200_mipmaps_compress_from_ex(base, items, source, levels, filter, steps, dstFormat, flags, threshold, alphaWeight, dst, nullptr);
 }
 
 int32_t dxb200_mipmaps_compress_ex(const dxb200_image* base, size_t items, size_t levels, uint32_t filter, const dxb200_chain_steps* steps,
@@ -993,6 +1072,61 @@ int32_t dxb200_scale_mipmaps_alpha_for_coverage(const dxb200_image* src, size_t 
         hr = cuda_hr(cudaMemcpy2DAsync(dst[l].pixels, dst[l].rowPitch, dd[l].pixels, dd[l].rowPitch, std::min(dst[l].rowPitch, dd[l].rowPitch),
                                        src[l].slicePitch / std::max<size_t>(src[l].rowPitch, 1), cudaMemcpyDeviceToHost, st), "D2H");
     if (hr == DXB_S_OK) hr = cuda_hr(cudaStreamSynchronize(st), "alpha coverage sync");
+    return hr;
+}
+
+// ---- IsAlphaAllOpaque ----------------------------------------------------------------------------
+int32_t dxb200_is_alpha_all_opaque_device(const dxb200_image* images, size_t nimages, int32_t* opaque, void* stream)
+{
+    AlphaOpaquePlan ap;
+    int32_t hr = plan_alpha_opaque(images, nimages, opaque, &ap);
+    if (hr != DXB_S_OK) return hr;
+    if (!ap.scan) { *opaque = 1; return DXB_S_OK; }
+    if (!bc_pointers_ok(images, nimages)) return DXB_E_INVALIDARG;
+    DevScope scope;
+    hr = scope.enter(images[0].pixels);
+    if (hr != DXB_S_OK) return hr;
+    const cudaStream_t st = static_cast<cudaStream_t>(stream);
+    uint8_t* word = nullptr;                            // one word for the whole call: every job may set it
+    DXB_CUDA(cudaMallocAsync(reinterpret_cast<void**>(&word), sizeof(uint32_t), st));
+    const std::vector<dxb200_image> words(nimages, dxb200_image{ 1, 1, DXB_FMT_UNKNOWN, sizeof(uint32_t), sizeof(uint32_t), word });
+    uint32_t result = 0;
+    hr = cuda_hr(cudaMemsetAsync(word, 0, sizeof(uint32_t), st), "cudaMemsetAsync(alpha word)");
+    if (hr == DXB_S_OK) hr = launch_alpha_opaque(ap, images, words.data(), nimages, st);
+    if (hr == DXB_S_OK) hr = cuda_hr(cudaMemcpyAsync(&result, word, sizeof(uint32_t), cudaMemcpyDeviceToHost, st), "D2H");
+    cudaFreeAsync(word, st);
+    const int32_t hs = cuda_hr(cudaStreamSynchronize(st), "alpha opaque sync");        // the answer is a host value
+    if (hr == DXB_S_OK && hs == DXB_S_OK) *opaque = result ? 0 : 1;
+    return hr != DXB_S_OK ? hr : hs;
+}
+
+// Bands of whole (block) rows, as the band calls cut them, sharded over the devices by bytes; the images go up, one result word
+// per band comes back, and the answer is the AND of the bands'.
+int32_t dxb200_is_alpha_all_opaque(const dxb200_image* images, size_t nimages, int32_t* opaque)
+{
+    AlphaOpaquePlan ap;
+    int32_t hr = plan_alpha_opaque(images, nimages, opaque, &ap);
+    if (hr != DXB_S_OK) return hr;
+    if (!ap.scan) { *opaque = 1; return DXB_S_OK; }
+    std::vector<dxb200_image> none(images, images + nimages);          // no destination: bands count the source's bytes only
+    for (dxb200_image& im : none) im.rowPitch = im.slicePitch = 0;
+    BandSplit bands;
+    split_bands(images, none.data(), nimages, 1, 0, ap.blocks, false, bands);
+    ResultWords words;
+    if ((hr = words.alloc(bands.src.size())) != DXB_S_OK) return hr;
+    const std::vector<dxb200_image> wimg = words.images();
+    hr = run_sharded(bands.src.size(), [&](size_t i) { return bands.src[i].slicePitch; },
+        [&](size_t lo, size_t hi)
+        {
+            const Plane planes[2] = { { bands.src.data() + lo, 1, Copy::Up, Copy::Up }, { wimg.data() + lo, 1, Copy::Down, Copy::Down } };
+            return run_staged(planes, 2, hi - lo, BAND_CHUNK,
+                [&](const std::vector<dxb200_image>* dev, size_t cnt, cudaStream_t st)
+                {
+                    const int32_t h2 = clear_words(dev[1], st);
+                    return h2 != DXB_S_OK ? h2 : launch_alpha_opaque(ap, dev[0].data(), dev[1].data(), cnt, st);
+                });
+        });
+    if (hr == DXB_S_OK) *opaque = words.all_zero() ? 1 : 0;
     return hr;
 }
 

@@ -234,6 +234,29 @@ DXB_FMT_FN uint32_t dxb_default_decompress(uint32_t fmt)
     }
 }
 
+// HasAlpha (DirectXTexUtil.cpp:530-584) for every DXGI value, implemented by this backend or not: IsAlphaAllOpaque answers true
+// for a format without alpha before it reads a pixel, so that answer needs no implementation of the format.  BC4, BC5 and BC6H
+// have no alpha even though their conversion flags carry CONVF_A.
+DXB_FMT_FN int dxb_has_alpha(uint32_t fmt)
+{
+    switch (fmt)
+    {
+    case 1: case 2: case 3: case 4:                         // R32G32B32A32_TYPELESS .. _SINT
+    case 9: case 10: case 11: case 12: case 13: case 14:    // R16G16B16A16_TYPELESS .. _SINT
+    case 23: case 24: case 25:                              // R10G10B10A2_TYPELESS .. _UINT
+    case 27: case 28: case 29: case 30: case 31: case 32:   // R8G8B8A8_TYPELESS .. _SINT
+    case 65:                                                // A8_UNORM
+    case 70: case 71: case 72: case 73: case 74: case 75: case 76: case 77: case 78:      // BC1 .. BC3, TYPELESS / UNORM / SRGB
+    case 86: case 87: case 89: case 90: case 91:            // B5G5R5A1, B8G8R8A8, R10G10B10_XR_BIAS_A2, B8G8R8A8_TYPELESS / _SRGB
+    case 97: case 98: case 99:                              // BC7
+    case 100: case 101: case 102: case 111: case 112: case 114: case 115:                 // AYUV, Y410, Y416, AI44, IA44, A8P8, B4G4R4A4
+    case 116: case 117: case 189: case 191:                 // the Xbox R10G10B10_{7E3,6E4,SNORM}_A2 formats, A4B4G4R4_UNORM
+        return 1;
+    default:
+        return 0;
+    }
+}
+
 // Resolve the sRGB bits exactly as ConvertScanline does (DirectXTexConvert.cpp:3121-3167).
 // conversion flags CompressBC passes for a BC1-5 target when the caller gives no sRGB flags and source/target agree
 // on sRGB-ness (DetermineEncoderSettings, DirectXTexCompress.cpp:46-68)

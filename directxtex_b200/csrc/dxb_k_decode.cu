@@ -1,12 +1,14 @@
 // dxb_k_decode.cu — DecompressBC (DirectXTexCompress.cpp:425-535) for a batch of images: one THREAD per 4x4 block:
 // decode (dxb_decode.cuh) -> ConvertScanline -> StoreScanline.
-//   k_decompress            generic: any BC source, any implemented target format
+//   k_decompress            generic: any BC source, any implemented target format; with the target DXB_SCAN_ALPHA_OPAQUE it
+//                           runs IsAlphaAllOpaqueBC's test instead (dxb_alpha_opaque.h) and stores nothing but the result word
 //   k_decompress_t<SF,DF>   the default (source, target) pairs with no sRGB step: compile-time formats (one decoder, one
 //                           store path per kernel) and one vector store per block row.  No pair names an sRGB format:
 //                           an sRGB call matches its twins' pair (dxb_make_linear).
 #include "dxb_launch.h"
 #include "dxb_dispatch.h"
 #include "dxb_decode.cuh"
+#include "dxb_alpha_opaque.h"
 
 // ---- table-driven fast paths -------------------------------------------------------------------------------------------
 // BC1 / BC3 / BC4 / BC5 blocks hold at most 4 colours and 8 values per channel; ConvertScanline + StoreScanline of the default target
@@ -129,6 +131,7 @@ __device__ __forceinline__ void decode_body(const dxb_job* __restrict__ jobs, co
     for (uint32_t unit = blockIdx.x * blockDim.x + threadIdx.x; unit < P.totalUnits; unit += stride)
     {
         const dxb_job& j = dxb_find_job(jobs, P.njobs, single, unit);
+        if (GENERIC && dstFormat == DXB_SCAN_ALPHA_OPAQUE && dxb_alpha_word_set(j.dst)) continue;
         const uint32_t local = unit - j.firstUnit;
         const uint32_t by = local / j.nbx, bx = local - by * j.nbx;
         __align__(16) uint8_t blk[16];
@@ -148,6 +151,11 @@ __device__ __forceinline__ void decode_body(const dxb_job* __restrict__ jobs, co
         }
         dxb_px px[16];
         dxb_decode_block(srcFormat, blk, px);
+        if (GENERIC && dstFormat == DXB_SCAN_ALPHA_OPAQUE)
+        {
+            if (dxb_block_not_opaque(px, pw, ph)) dxb_alpha_word_store(j.dst);
+            continue;
+        }
         if (!GENERIC)
         {
             constexpr uint32_t B = dxb_bytes_per_pixel(GENERIC ? 2u : DF), ROWB = 4u * B, V = (ROWB >= 16u) ? 16u : ROWB;
@@ -204,6 +212,12 @@ const char* dxb_launch_decompress(unsigned grid, cudaStream_t stream, const dxb_
     if (P.cflags == 0 && dxb_on_pair<71, 28, 74, 28, 77, 28, 98, 28, 80, 61, 81, 63, 83, 49, 84, 51, 95, 2, 96, 2>(sf, df, hot))
         return "k_decompress_t";
 #endif
+    k_decompress<<<grid, 128, 0, stream>>>(jobs, hostJobs[0], P);
+    return "k_decompress";
+}
+
+const char* dxb_launch_alpha_opaque_blocks(unsigned grid, cudaStream_t stream, const dxb_job* jobs, const dxb_job* hostJobs, const dxb_compress_params& P)
+{
     k_decompress<<<grid, 128, 0, stream>>>(jobs, hostJobs[0], P);
     return "k_decompress";
 }

@@ -1,5 +1,6 @@
 // dxb_k_rows.cu — row kernels (HBM-bound side of the path):
-//   k_convert            generic: one thread per pixel, any implemented format pair, heterogeneous batches
+//   k_convert            generic: one thread per pixel, any implemented format pair, heterogeneous batches; with the destination
+//                        DXB_SCAN_ALPHA_OPAQUE it runs IsAlphaAllOpaque's test instead (dxb_alpha_opaque.h)
 //   k_convert_vec<SF,DF> hot pairs: compile-time formats, 16-byte vector access on the wider side, uniform batches
 //   k_mip_level          generic: one thread per destination pixel, any format / filter
 //   k_mip_tile<FMT,MODE,SRGB>  hot formats x {BOX,LINEAR,CUBIC}: compile-time format and filter, 2D thread tiles,
@@ -16,6 +17,7 @@
 #include "dxb_pixel.cuh"
 #include "dxb_mips.cuh"
 #include "dxb_coverage.h"
+#include "dxb_alpha_opaque.h"
 
 // ------------------------------------------------------------------------------------------------ generic
 __global__ void __launch_bounds__(256) k_convert(const dxb_job* __restrict__ jobs, dxb_job single, dxb_convert_params P)
@@ -26,6 +28,12 @@ __global__ void __launch_bounds__(256) k_convert(const dxb_job* __restrict__ job
         const dxb_job& j = dxb_find_job(jobs, P.njobs, single, unit);
         const uint32_t local = unit - j.firstUnit;
         const uint32_t y = local / j.width, x = local - y * j.width;
+        if (P.dstFormat == DXB_SCAN_ALPHA_OPAQUE)
+        {
+            if (!dxb_alpha_word_set(j.dst) && dxb_alpha_not_opaque(dxb_load_pixel(P.srcFormat, j.src + (size_t)y * j.srcPitch, x).w, DXB_OPAQUE_PIXEL))
+                dxb_alpha_word_store(j.dst);
+            continue;
+        }
         dxb_px v = dxb_load_pixel(P.srcFormat, j.src + (size_t)y * j.srcPitch, x);
         v = dxb_convert_pixel(v, P.inF, P.outF, P.flags);
         if (P.flags & DXB_FILTER_DITHER) dxb_store_pixel_dither(P.dstFormat, j.dst + (size_t)y * j.dstPitch, x, y, v);     // ordered dither (:4861-4879)
@@ -177,6 +185,12 @@ const char* dxb_launch_convert(unsigned grid, cudaStream_t stream, const dxb_job
                         61, 28, 28, 61, 11, 2, 2, 11, 41, 2, 2, 41, 29, 2, 2, 29, 29, 28, 28, 29>(P.srcFormat, P.dstFormat, hot))
             return "k_convert_vec";
     }
+    k_convert<<<grid, 256, 0, stream>>>(jobs, hostJobs[0], P);
+    return "k_convert";
+}
+
+const char* dxb_launch_alpha_opaque_pixels(unsigned grid, cudaStream_t stream, const dxb_job* jobs, const dxb_job* hostJobs, const dxb_convert_params& P)
+{
     k_convert<<<grid, 256, 0, stream>>>(jobs, hostJobs[0], P);
     return "k_convert";
 }

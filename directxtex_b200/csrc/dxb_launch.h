@@ -49,6 +49,11 @@ const char* dxb_launch_alpha_coverage(unsigned grid, cudaStream_t stream, const 
                                       unsigned long long* counts, uint32_t step);
 const char* dxb_launch_scale_alpha(unsigned grid, cudaStream_t stream, const dxb_coverage_job* jobs, const dxb_coverage_params& P,
                                    const unsigned long long* counts);
+// IsAlphaAllOpaque of a batch (dxb_alpha_opaque.h): P.dstFormat = DXB_SCAN_ALPHA_OPAQUE and every job's dst = its result word, zero
+// before the launch.  BC1 / BC2 / BC3 / BC7 sources run on the generic k_decompress, one thread per block; uncompressed sources on
+// the generic k_convert, one thread per pixel.
+const char* dxb_launch_alpha_opaque_blocks(unsigned grid, cudaStream_t stream, const dxb_job* jobs, const dxb_job* hostJobs, const dxb_compress_params& P);
+const char* dxb_launch_alpha_opaque_pixels(unsigned grid, cudaStream_t stream, const dxb_job* jobs, const dxb_job* hostJobs, const dxb_convert_params& P);
 const char* dxb_launch_pmalpha(unsigned grid, cudaStream_t stream, const dxb_job* jobs, const dxb_job* hostJobs, const dxb_convert_params& P);
 // resident CTAs per SM of each kernel at its block size
 int dxb_occupancy_bc15();

@@ -13,6 +13,7 @@
 #include "dxb_jobs.h"
 #include "dxb_host_tri.h"
 #include "dxb_coverage.h"
+#include "dxb_alpha_opaque.h"
 
 namespace {
 
@@ -442,6 +443,51 @@ int32_t plan_mipmaps_compress_from(const dxb200_image* base, size_t items, const
         level0 = resized;
     }
     return plan_mipmaps_compress(level0.data(), items, levels, filter, steps, dstFormat, flags, threshold, dst, &fp->chain);
+}
+
+// ---- IsAlphaAllOpaque (DirectXTexImage.cpp:800-852; IsAlphaAllOpaqueBC, DirectXTexCompress.cpp:539-621) ---------------------
+// The reference's answer comes without a device when scan == false: a format without alpha is opaque, nothing is read.  Otherwise
+// every texel of every image has to be scanned: BC1 / BC2 / BC3 / BC7 blocks on k_decompress (blocks), any other implemented
+// format with alpha on k_convert.  Images of one call share one format; a null pixel pointer is E_POINTER whatever the format.
+struct AlphaOpaquePlan { bool scan, blocks; uint32_t format; };
+
+int32_t plan_alpha_opaque(const dxb200_image* images, size_t n, const int32_t* opaque, AlphaOpaquePlan* ap)
+{
+    ap->scan = ap->blocks = false; ap->format = 0;
+    if (!images || !opaque || !n) return DXB_E_INVALIDARG;
+    const uint32_t fmt = images[0].format;
+    for (size_t i = 0; i < n; ++i)
+    {
+        if (images[i].format != fmt) return DXB_E_INVALIDARG;
+        if (!images[i].pixels) return DXB_E_POINTER;
+    }
+    if (!dxb_has_alpha(fmt)) return DXB_S_OK;                                            // :805-806, no pixel is read
+    const bool blocks = is_compressed(fmt);
+    if (blocks ? !dxb_alpha_scan_blocks(fmt) : !is_supported_pixel_format(fmt)) return DXB_E_NOT_SUPPORTED;
+    for (size_t i = 0; i < n; ++i)
+    {
+        const dxb200_image& im = images[i];
+        if (!im.width || !im.height || im.width > 0xFFFFFFFFull || im.height > 0xFFFFFFFFull) return DXB_E_INVALIDARG;
+        if (!bc_pitch_ok(im)) return DXB_E_INVALIDARG;                                  // the rules of Decompress
+    }
+    ap->scan = true; ap->blocks = blocks; ap->format = fmt;
+    return DXB_S_OK;
+}
+
+// the parameters of the scan's launch over `units` work units of `njobs` jobs (dxb_alpha_opaque.h)
+dxb_compress_params alpha_opaque_block_params(const AlphaOpaquePlan& ap, uint32_t units, uint32_t njobs)
+{
+    dxb_compress_params P; memset(&P, 0, sizeof(P));
+    P.srcFormat = ap.format; P.dstFormat = DXB_SCAN_ALPHA_OPAQUE; P.inF = dxb_convert_flags(ap.format);
+    P.totalUnits = units; P.njobs = njobs;
+    return P;
+}
+dxb_convert_params alpha_opaque_pixel_params(const AlphaOpaquePlan& ap, uint32_t units, uint32_t njobs)
+{
+    dxb_convert_params P; memset(&P, 0, sizeof(P));
+    P.srcFormat = ap.format; P.dstFormat = DXB_SCAN_ALPHA_OPAQUE; P.inF = dxb_convert_flags(ap.format);
+    P.totalUnits = units; P.njobs = njobs;
+    return P;
 }
 
 } // namespace

@@ -503,6 +503,20 @@ const Image* ScratchImage::GetImage(size_t mip, size_t item, size_t slice) const
     return (i < m_nimages) ? &m_image[i] : nullptr;
 }
 
+bool ScratchImage::IsAlphaAllOpaque() const noexcept
+{
+    if (!m_image) return false;
+    if (!HasAlpha(m_metadata.format)) return true;
+    try
+    {
+        std::vector<dxb200_image> imgs(m_nimages);
+        for (size_t i = 0; i < m_nimages; ++i) imgs[i] = to_c(m_image[i]);
+        int32_t opaque = 0;
+        return dxb200_is_alpha_all_opaque(imgs.data(), imgs.size(), &opaque) == 0 && opaque == 1;
+    }
+    catch (...) { return false; }
+}
+
 // ---------------------------------------------------------------------------------------------------
 // Compress
 namespace

@@ -180,6 +180,9 @@ namespace DirectX
         size_t GetImageCount() const noexcept { return m_nimages; }
         uint8_t* GetPixels() const noexcept { return m_memory; }
         size_t GetPixelsSize() const noexcept { return m_size; }
+        // every texel of every image opaque (DirectXTexImage.cpp:800-852): true for a format without alpha, false when empty or when
+        // the scan fails (a format with alpha this library does not implement, no device)
+        bool IsAlphaAllOpaque() const noexcept;
 
     private:
         size_t m_nimages, m_size;

@@ -172,6 +172,27 @@ typedef struct dxb200_chain_source
 DXB200_API int32_t  dxb200_mipmaps_compress_from(const dxb200_image* base, size_t items, const dxb200_chain_source* source,
                                                  size_t levels, uint32_t filter, const dxb200_chain_steps* steps, uint32_t dstFormat,
                                                  uint32_t flags, float threshold, float alphaWeight, const dxb200_image* dst);
+/* dxb200_mipmaps_compress_from that also answers texconv's next step, "set alpha mode" (Texconv/texconv.cpp:3738-3766):
+ * alphaAllOpaque == NULL is exactly dxb200_mipmaps_compress_from; otherwise *alphaAllOpaque = 1 or 0, what
+ * ScratchImage::IsAlphaAllOpaque() returns for the output (Initialize2D(dstFormat, W, H, items, levels) holding dst).  The blocks
+ * are scanned where they were made, one launch per chunk after its compression, and the answer comes back with the blocks;
+ * the blocks are identical to dxb200_mipmaps_compress_from's.  BC4, BC5 and BC6H outputs have no alpha: no scan, 1. */
+DXB200_API int32_t  dxb200_mipmaps_compress_from_ex(const dxb200_image* base, size_t items, const dxb200_chain_source* source,
+                                                    size_t levels, uint32_t filter, const dxb200_chain_steps* steps, uint32_t dstFormat,
+                                                    uint32_t flags, float threshold, float alphaWeight, const dxb200_image* dst,
+                                                    int32_t* alphaAllOpaque);
+
+/* ScratchImage::IsAlphaAllOpaque (DirectXTexImage.cpp:800-852; IsAlphaAllOpaqueBC, DirectXTexCompress.cpp:539-621) of
+ * `nimages` images of one format: *opaque = 1 when every texel inside every image has alpha >= 0.997 (uncompressed, as
+ * LoadScanline reads it) or >= 0.99 (decoded BC1 / BC2 / BC3 / BC7 blocks; the padding texels of partial blocks do not count),
+ * else 0.  A NaN alpha counts as opaque.  A format without alpha (HasAlpha: BC4, BC5, BC6H, B8G8R8X8, R32_FLOAT, ...) answers 1
+ * without a pixel being read and without a device.  HRESULTs: images / opaque NULL or nimages == 0, images of different formats,
+ * a zero or over-32-bit size, a BC row pitch that is not a multiple of the block size -> E_INVALIDARG; a NULL pixel pointer ->
+ * E_POINTER; a format with alpha this library does not implement -> E_NOT_SUPPORTED (0x80070032).
+ * The host call stages the images in bands of whole (block) rows, sharded over the initialised devices; only one result word per
+ * band comes back.  The _device call runs on the device that owns the pointers and synchronises `stream` before it returns. */
+DXB200_API int32_t  dxb200_is_alpha_all_opaque(const dxb200_image* images, size_t nimages, int32_t* opaque);
+DXB200_API int32_t  dxb200_is_alpha_all_opaque_device(const dxb200_image* images, size_t nimages, int32_t* opaque, void* stream);
 
 /* DirectX::Resize (DirectXTexResize.cpp:854-935 single image, :942-1120 arrays; custom filters ResizePointFilter /
  * ResizeBoxFilter / ResizeLinearFilter / ResizeCubicFilter / ResizeTriangleFilter :255-798, selection :805-837).
