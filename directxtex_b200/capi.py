@@ -16,6 +16,7 @@ SYMBOLS = [
     "dxb200_resize", "dxb200_resize_device", "dxb200_premultiply_alpha", "dxb200_premultiply_alpha_device",
     "dxb200_scale_mipmaps_alpha_for_coverage", "dxb200_scale_mipmaps_alpha_for_coverage_device",
     "dxb200_is_alpha_all_opaque", "dxb200_is_alpha_all_opaque_device",
+    "dxb200_apply_channel_steps", "dxb200_apply_channel_steps_device", "dxb200_mipmaps_compress_from_channels",
     "dxb200_dds_encode_header", "dxb200_dds_save_memory", "dxb200_dds_get_metadata", "dxb200_dds_load_memory",
 ]
 
@@ -40,6 +41,12 @@ class ChainSteps(C.Structure):
 class ChainSource(C.Structure):
     """dxb200_chain_source: the Decompress and Resize dxb200_mipmaps_compress_from runs in front of the mips."""
     _fields_ = [("decompressFormat", C.c_uint32), ("width", C.c_size_t), ("height", C.c_size_t), ("resizeFilter", C.c_uint32)]
+
+
+class ChannelSteps(C.Structure):
+    """dxb200_channel_steps: texconv's swizzle, colour key, invert-Y and reconstruct-Z steps."""
+    _fields_ = [("swizzle", C.c_uint8 * 4), ("zeroMask", C.c_uint8), ("oneMask", C.c_uint8), ("colorKey", C.c_uint8),
+                ("invertY", C.c_uint8), ("reconstructZ", C.c_uint8), ("colorKeyValue", C.c_uint32)]
 
 
 STATUS_FN = C.CFUNCTYPE(C.c_int, C.c_size_t, C.c_size_t, C.c_void_p)      # dxb200_status_fn
@@ -82,6 +89,11 @@ def _load():
     lib.dxb200_mipmaps_compress_from.argtypes = [IP, C.c_size_t, C.POINTER(ChainSource), C.c_size_t, C.c_uint32, C.POINTER(ChainSteps), C.c_uint32,
                                                  C.c_uint32, C.c_float, C.c_float, IP]
     lib.dxb200_mipmaps_compress_from_ex.argtypes = lib.dxb200_mipmaps_compress_from.argtypes + [C.POINTER(C.c_int32)]
+    lib.dxb200_mipmaps_compress_from_channels.argtypes = [IP, C.c_size_t, C.POINTER(ChainSource), C.POINTER(ChannelSteps), C.c_size_t, C.c_uint32,
+                                                          C.POINTER(ChainSteps), C.c_uint32, C.c_uint32, C.c_float, C.c_float, IP,
+                                                          C.POINTER(C.c_int32)]
+    lib.dxb200_apply_channel_steps.argtypes = [IP, C.c_size_t, C.POINTER(ChannelSteps), IP]
+    lib.dxb200_apply_channel_steps_device.argtypes = [IP, C.c_size_t, C.POINTER(ChannelSteps), IP, C.c_void_p]
     lib.dxb200_is_alpha_all_opaque.argtypes = [IP, C.c_size_t, C.POINTER(C.c_int32)]
     lib.dxb200_is_alpha_all_opaque_device.argtypes = [IP, C.c_size_t, C.POINTER(C.c_int32), C.c_void_p]
     lib.dxb200_compute_pitch.argtypes = [C.c_uint32, C.c_size_t, C.c_size_t, C.POINTER(C.c_size_t), C.POINTER(C.c_size_t)]
@@ -109,7 +121,7 @@ def _load():
     lib.dxb200_dds_load_memory.argtypes = [C.c_void_p, C.c_size_t, C.c_uint32, IP, C.c_size_t]
     for name in ("dxb200_dds_encode_header", "dxb200_dds_save_memory", "dxb200_dds_get_metadata", "dxb200_dds_load_memory"):
         getattr(lib, name).restype = C.c_int32
-    for name in ("dxb200_init", "dxb200_init_devices", "dxb200_initialized_devices", "dxb200_compress_ex", "dxb200_convert_ex", "dxb200_mipmaps_compress", "dxb200_mipmaps_compress_ex", "dxb200_mipmaps_compress_from", "dxb200_mipmaps_compress_from_ex", "dxb200_is_alpha_all_opaque", "dxb200_is_alpha_all_opaque_device", "dxb200_device_count", "dxb200_compute_pitch", "dxb200_calculate_mip_levels", "dxb200_compress",
+    for name in ("dxb200_init", "dxb200_init_devices", "dxb200_initialized_devices", "dxb200_compress_ex", "dxb200_convert_ex", "dxb200_mipmaps_compress", "dxb200_mipmaps_compress_ex", "dxb200_mipmaps_compress_from", "dxb200_mipmaps_compress_from_ex", "dxb200_is_alpha_all_opaque", "dxb200_is_alpha_all_opaque_device", "dxb200_apply_channel_steps", "dxb200_apply_channel_steps_device", "dxb200_mipmaps_compress_from_channels", "dxb200_device_count", "dxb200_compute_pitch", "dxb200_calculate_mip_levels", "dxb200_compress",
                  "dxb200_compress_device", "dxb200_decompress", "dxb200_decompress_device", "dxb200_convert",
                  "dxb200_convert_device", "dxb200_generate_mipmaps", "dxb200_generate_mipmaps_device", "dxb200_resize", "dxb200_resize_device", "dxb200_premultiply_alpha", "dxb200_premultiply_alpha_device"):
         getattr(lib, name).restype = C.c_int32
@@ -250,6 +262,38 @@ def mipmaps_compress_from_ex(bases, w, h, base_fmt, dst_fmt, source=None, filter
     if hr != 0:
         raise DxTexError(hr, "dxb200_mipmaps_compress_from_ex")
     return outs, opaque.value == 1
+
+
+def channel_steps(swizzle=(0, 1, 2, 3), zero_mask=0, one_mask=0, color_key=None, invert_y=False, reconstruct_z=False):
+    """the dxb200_channel_steps of texconv's -swizzle (output channel c takes source channel swizzle[c]; bit c of zero_mask /
+    one_mask forces channel c to 0 / 1), -c (color_key = 0xRRGGBB, None = off), -inverty and -reconstructz"""
+    return ChannelSteps((C.c_uint8 * 4)(*swizzle), zero_mask, one_mask, 0 if color_key is None else 1, 1 if invert_y else 0,
+                        1 if reconstruct_z else 0, 0 if color_key is None else color_key)
+
+
+def mipmaps_compress_from_channels(bases, w, h, base_fmt, dst_fmt, source=None, channels=None, filter=0, levels=0, flags=0, steps=None,
+                                   row_pitch=0):
+    """mipmaps_compress_from_ex through dxb200_mipmaps_compress_from_channels with the ChannelSteps `channels` (None: none): (the
+    chains, IsAlphaAllOpaque of the output as a bool)"""
+    args, outs = _from_args(bases, w, h, base_fmt, dst_fmt, source, filter, levels, flags, steps, row_pitch)
+    opaque = C.c_int32(-1)
+    hr = lib.dxb200_mipmaps_compress_from_channels(*args[:3], C.byref(channels) if channels is not None else None, *args[3:], C.byref(opaque))
+    if hr != 0:
+        raise DxTexError(hr, "dxb200_mipmaps_compress_from_channels")
+    return outs, opaque.value == 1
+
+
+def apply_channel_steps(arrays, w, h, fmt, channels, row_pitch=0):
+    """dxb200_apply_channel_steps of equally sized w x h host images of fmt (rows row_pitch bytes apart, 0 = tight) with the
+    ChannelSteps `channels`: one output array per image, of the input's layout"""
+    arrays = [np.ascontiguousarray(a).view(np.uint8).reshape(-1) for a in arrays]
+    outs = [np.zeros_like(a) for a in arrays]
+    s = images([make_image(_np_ptr(a), w, h, fmt, row_pitch) for a in arrays])
+    d = images([make_image(_np_ptr(o), w, h, fmt, row_pitch) for o in outs])
+    hr = lib.dxb200_apply_channel_steps(s, len(arrays), C.byref(channels), d)
+    if hr != 0:
+        raise DxTexError(hr, "dxb200_apply_channel_steps")
+    return outs
 
 
 def is_alpha_all_opaque(arrays, w, h, fmt, row_pitch=0):

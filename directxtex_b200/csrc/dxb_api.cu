@@ -531,6 +531,16 @@ int32_t launch_pmalpha(dxb_convert_params P, const dxb200_image* src, const dxb2
     return check_launch(dxb_launch_pmalpha(grid_for(jt.total, 256, (uint32_t)t_v.dev->gridRow * 8u), stream, jt.dev.d, jt.host.data(), P));
 }
 
+// ---- texconv's channel steps (dxb_channel_steps.h) ------------------------------------------------------------------------
+int32_t launch_channel_steps(dxb_convert_params P, const dxb200_image* src, const dxb200_image* dst, size_t n, cudaStream_t stream)
+{
+    JobTable jt;
+    const int32_t hr = jt.build(src, dst, n, false, stream);
+    if (hr != DXB_S_OK) return hr;
+    P.totalUnits = jt.total; P.njobs = (uint32_t)n;
+    return check_launch(dxb_launch_channel_steps(grid_for(jt.total, 256, (uint32_t)t_v.dev->gridRow * 8u), stream, jt.dev.d, jt.host.data(), P));
+}
+
 // ---- GenerateMipMaps ----------------------------------------------------------------------------
 // chain[] holds DEVICE pointers; level 0 of each item is populated
 int32_t launch_mips(const dxb200_image* chain, size_t items, size_t levels, uint32_t filter, uint32_t mode, cudaStream_t stream)
@@ -672,9 +682,10 @@ struct ResultWords
 // up + 1.33 B/texel down for BC3 from RGBA8 instead of 4 + 5.33 + 5.33 + 1.33.  Chunks of whole items are pipelined over the
 // lane's NSLOT (stream, buffer) slots.  A chunk holds, per item and in plane order: the base as the caller laid it out (when a
 // front step reads it), the decompressed image (only when a resize follows), the chain (level 0 uploaded when no front step writes
-// it) and the blocks.  With no front step that is exactly the chain and the blocks.  With a scan (words != nullptr: one result word
-// per item, see dxb200_mipmaps_compress_from_ex) one more plane holds the items' words; they are cleared, set by one scan launch
-// over all the chunk's blocks after the compression, and come back with the blocks.
+// it) and the blocks.  With no front step that is exactly the chain and the blocks.  Channel steps (fp.channels) run in place on
+// every item's level 0 after the front steps or the upload, one launch per chunk and no plane of their own.  With a scan (words !=
+// nullptr: one result word per item, see dxb200_mipmaps_compress_from_ex) one more plane holds the items' words; they are cleared,
+// set by one scan launch over all the chunk's blocks after the compression, and come back with the blocks.
 int32_t run_chains(const dxb200_image* base, size_t items, size_t levels, uint32_t filter, const FromPlan& fp, const dxb200_image* dst,
                    const AlphaOpaquePlan& scan, const ResultWords* words)
 {
@@ -700,12 +711,13 @@ int32_t run_chains(const dxb200_image* base, size_t items, size_t levels, uint32
                     const dxb200_image* blocks = dev[pc + 1].data();
                     int32_t h2 = DXB_S_OK;
                     std::vector<dxb200_image> level(cnt);
+                    for (size_t it = 0; it < cnt; ++it) level[it] = chains[it * levels];
                     if (front)
                     {
-                        for (size_t it = 0; it < cnt; ++it) level[it] = chains[it * levels];
                         if (fp.decompress) h2 = launch_decompress(fp.dp, src, mid ? decompressed : level.data(), cnt, st);
                         if (h2 == DXB_S_OK && fp.resize) h2 = launch_resize(mid ? decompressed : src, level.data(), cnt, fp.resizeFilter, fp.resizeMode, st);
                     }
+                    if (h2 == DXB_S_OK && fp.channels) h2 = launch_channel_steps(fp.cp, level.data(), level.data(), cnt, st);
                     if (h2 == DXB_S_OK) h2 = launch_mips(chains, cnt, levels, filter, cp.mode, st);
                     if (h2 == DXB_S_OK && cp.coverage) h2 = launch_coverage(chains, chains, cnt, levels, cp.ref, st);
                     // one launch per level: the chunk's images of a level are equal, as the separate calls' images are, so they take the
@@ -972,14 +984,15 @@ int32_t dxb200_generate_mipmaps(const dxb200_image* chain, size_t items, size_t 
 // texconv's two steps between the mips and the compression (-keepcoverage :3480, -pmalpha :3526), both in place on the chunk's
 // chains in device memory; dxb200_mipmaps_compress_from adds Decompress and Resize in front of the mips.
 // dxb200_mipmaps_compress_from_ex adds texconv's "set alpha mode" test of the output (:3738-3766): IsAlphaAllOpaque of the blocks,
-// scanned where they were made.
-int32_t dxb200_mipmaps_compress_from_ex(const dxb200_image* base, size_t items, const dxb200_chain_source* source, size_t levels, uint32_t filter,
-                                        const dxb200_chain_steps* steps, uint32_t dstFormat, uint32_t flags, float threshold, float alphaWeight,
-                                        const dxb200_image* dst, int32_t* alphaAllOpaque)
+// scanned where they were made.  dxb200_mipmaps_compress_from_channels adds texconv's channel steps after Resize (:2645-3300).
+int32_t dxb200_mipmaps_compress_from_channels(const dxb200_image* base, size_t items, const dxb200_chain_source* source,
+                                              const dxb200_channel_steps* channels, size_t levels, uint32_t filter, const dxb200_chain_steps* steps,
+                                              uint32_t dstFormat, uint32_t flags, float threshold, float alphaWeight, const dxb200_image* dst,
+                                              int32_t* alphaAllOpaque)
 {
     (void)alphaWeight;
     FromPlan fp;
-    int32_t hr = plan_mipmaps_compress_from(base, items, source, levels, filter, steps, dstFormat, flags, threshold, dst, &fp);
+    int32_t hr = plan_mipmaps_compress_channels(base, items, source, channels, levels, filter, steps, dstFormat, flags, threshold, dst, &fp);
     if (hr != DXB_S_OK) return hr;
     AlphaOpaquePlan ap = {};
     if (alphaAllOpaque && (hr = plan_alpha_opaque(dst, items * levels, alphaAllOpaque, &ap)) != DXB_S_OK) return hr;
@@ -988,6 +1001,14 @@ int32_t dxb200_mipmaps_compress_from_ex(const dxb200_image* base, size_t items, 
     hr = run_chains(base, items, levels, filter, fp, dst, ap, ap.scan ? &words : nullptr);
     if (hr == DXB_S_OK && alphaAllOpaque) *alphaAllOpaque = (!ap.scan || words.all_zero()) ? 1 : 0;
     return hr;
+}
+
+int32_t dxb200_mipmaps_compress_from_ex(const dxb200_image* base, size_t items, const dxb200_chain_source* source, size_t levels, uint32_t filter,
+                                        const dxb200_chain_steps* steps, uint32_t dstFormat, uint32_t flags, float threshold, float alphaWeight,
+                                        const dxb200_image* dst, int32_t* alphaAllOpaque)
+{
+    return dxb200_mipmaps_compress_from_channels(base, items, source, nullptr, levels, filter, steps, dstFormat, flags, threshold, alphaWeight,
+                                                 dst, alphaAllOpaque);
 }
 
 int32_t dxb200_mipmaps_compress_from(const dxb200_image* base, size_t items, const dxb200_chain_source* source, size_t levels, uint32_t filter,
@@ -1027,6 +1048,27 @@ int32_t dxb200_premultiply_alpha(const dxb200_image* src, size_t nimages, uint32
     if (hr != DXB_S_OK) return hr;
     return run_bands(src, dst, nimages, 1, 1, false, false, nullptr, nullptr,
         [&](const dxb200_image* ds, const dxb200_image* dd, size_t cnt, cudaStream_t st) { return launch_pmalpha(P, ds, dd, cnt, st); });
+}
+
+// ---- texconv's channel steps (TransformImage with texconv's lambdas) --------------------------------------------------------
+int32_t dxb200_apply_channel_steps_device(const dxb200_image* src, size_t n, const dxb200_channel_steps* steps, const dxb200_image* dst, void* stream)
+{
+    dxb_convert_params P;
+    int32_t hr = plan_channel_steps(src, n, steps, dst, &P);
+    if (hr != DXB_S_OK) return hr;
+    DevScope scope;
+    hr = scope.enter(src[0].pixels);
+    if (hr != DXB_S_OK) return hr;
+    return launch_channel_steps(P, src, dst, n, static_cast<cudaStream_t>(stream));
+}
+
+int32_t dxb200_apply_channel_steps(const dxb200_image* src, size_t n, const dxb200_channel_steps* steps, const dxb200_image* dst)
+{
+    dxb_convert_params P;
+    int32_t hr = plan_channel_steps(src, n, steps, dst, &P);
+    if (hr != DXB_S_OK) return hr;
+    return run_bands(src, dst, n, 1, 1, false, false, nullptr, nullptr,
+        [&](const dxb200_image* ds, const dxb200_image* dd, size_t cnt, cudaStream_t st) { return launch_channel_steps(P, ds, dd, cnt, st); });
 }
 
 // ---- ScaleMipMapsAlphaForCoverage ----------------------------------------------------------------

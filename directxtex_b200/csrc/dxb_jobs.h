@@ -27,6 +27,8 @@ struct dxb_convert_params
     uint32_t srcFormat, dstFormat, inF, outF, flags;
     uint32_t totalUnits, njobs;
     float threshold;               // alpha threshold of 1-bit alpha destinations (B5G5R5A1)
+    uint32_t steps;                // texconv's channel steps when srcFormat == dstFormat (dxb_channel_steps.h), else 0
+    float key[3];                  // the colour key of those steps, as floats
 };
 
 struct dxb_mip_job

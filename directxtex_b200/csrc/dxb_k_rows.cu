@@ -1,6 +1,7 @@
 // dxb_k_rows.cu — row kernels (HBM-bound side of the path):
 //   k_convert            generic: one thread per pixel, any implemented format pair, heterogeneous batches; with the destination
-//                        DXB_SCAN_ALPHA_OPAQUE it runs IsAlphaAllOpaque's test instead (dxb_alpha_opaque.h)
+//                        DXB_SCAN_ALPHA_OPAQUE it runs IsAlphaAllOpaque's test instead (dxb_alpha_opaque.h); with the
+//                        destination format equal to the source format it runs texconv's channel steps (dxb_channel_steps.h)
 //   k_convert_vec<SF,DF> hot pairs: compile-time formats, 16-byte vector access on the wider side, uniform batches
 //   k_mip_level          generic: one thread per destination pixel, any format / filter
 //   k_mip_tile<FMT,MODE,SRGB>  hot formats x {BOX,LINEAR,CUBIC}: compile-time format and filter, 2D thread tiles,
@@ -18,6 +19,7 @@
 #include "dxb_mips.cuh"
 #include "dxb_coverage.h"
 #include "dxb_alpha_opaque.h"
+#include "dxb_channel_steps.h"
 
 // ------------------------------------------------------------------------------------------------ generic
 __global__ void __launch_bounds__(256) k_convert(const dxb_job* __restrict__ jobs, dxb_job single, dxb_convert_params P)
@@ -32,6 +34,11 @@ __global__ void __launch_bounds__(256) k_convert(const dxb_job* __restrict__ job
         {
             if (!dxb_alpha_word_set(j.dst) && dxb_alpha_not_opaque(dxb_load_pixel(P.srcFormat, j.src + (size_t)y * j.srcPitch, x).w, DXB_OPAQUE_PIXEL))
                 dxb_alpha_word_store(j.dst);
+            continue;
+        }
+        if (P.dstFormat == P.srcFormat)
+        {
+            dxb_channel_steps_pixel(P.srcFormat, j.src + (size_t)y * j.srcPitch, j.dst + (size_t)y * j.dstPitch, x, P.steps, P.key[0], P.key[1], P.key[2]);
             continue;
         }
         dxb_px v = dxb_load_pixel(P.srcFormat, j.src + (size_t)y * j.srcPitch, x);
@@ -190,6 +197,12 @@ const char* dxb_launch_convert(unsigned grid, cudaStream_t stream, const dxb_job
 }
 
 const char* dxb_launch_alpha_opaque_pixels(unsigned grid, cudaStream_t stream, const dxb_job* jobs, const dxb_job* hostJobs, const dxb_convert_params& P)
+{
+    k_convert<<<grid, 256, 0, stream>>>(jobs, hostJobs[0], P);
+    return "k_convert";
+}
+
+const char* dxb_launch_channel_steps(unsigned grid, cudaStream_t stream, const dxb_job* jobs, const dxb_job* hostJobs, const dxb_convert_params& P)
 {
     k_convert<<<grid, 256, 0, stream>>>(jobs, hostJobs[0], P);
     return "k_convert";

@@ -54,6 +54,9 @@ const char* dxb_launch_scale_alpha(unsigned grid, cudaStream_t stream, const dxb
 // the generic k_convert, one thread per pixel.
 const char* dxb_launch_alpha_opaque_blocks(unsigned grid, cudaStream_t stream, const dxb_job* jobs, const dxb_job* hostJobs, const dxb_compress_params& P);
 const char* dxb_launch_alpha_opaque_pixels(unsigned grid, cudaStream_t stream, const dxb_job* jobs, const dxb_job* hostJobs, const dxb_convert_params& P);
+// texconv's channel steps (dxb_channel_steps.h) on the generic k_convert, one thread per pixel: P.srcFormat == P.dstFormat, P.steps
+// and P.key; a job's dst may be its src (same pointer and pitch)
+const char* dxb_launch_channel_steps(unsigned grid, cudaStream_t stream, const dxb_job* jobs, const dxb_job* hostJobs, const dxb_convert_params& P);
 const char* dxb_launch_pmalpha(unsigned grid, cudaStream_t stream, const dxb_job* jobs, const dxb_job* hostJobs, const dxb_convert_params& P);
 // resident CTAs per SM of each kernel at its block size
 int dxb_occupancy_bc15();

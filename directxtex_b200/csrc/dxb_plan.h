@@ -14,6 +14,7 @@
 #include "dxb_host_tri.h"
 #include "dxb_coverage.h"
 #include "dxb_alpha_opaque.h"
+#include "dxb_channel_steps.h"
 
 namespace {
 
@@ -385,16 +386,71 @@ int32_t plan_mipmaps_compress(const dxb200_image* base, size_t items, size_t lev
     return plan_compress(chain.data(), items * levels, dstFormat, flags, threshold, dst, &cp->compress);
 }
 
-// ---- Decompress -> Resize -> mipmaps_compress_ex in one call (mipmaps_compress_from) -----------------------------------------
+// ---- texconv's channel steps (TransformImage, DirectXTexMisc.cpp:606-760; the rule in dxb_channel_steps.h) ------------------------
+// the step word of `s`: 0 when no step is enabled (the swizzle is enabled unless it is the identity with both masks 0)
+uint32_t channel_steps_word(const dxb200_channel_steps& s)
+{
+    uint32_t w = 0;
+    for (uint32_t c = 0; c < 4; ++c) w |= (uint32_t)(s.swizzle[c] & 3u) << (DXB_CH_SWIZZLE_SHIFT + 2u * c);
+    w |= (uint32_t)(s.zeroMask & 0xFu) << DXB_CH_ZERO_SHIFT | (uint32_t)(s.oneMask & 0xFu) << DXB_CH_ONE_SHIFT;
+    if (s.swizzle[0] != 0 || s.swizzle[1] != 1 || s.swizzle[2] != 2 || s.swizzle[3] != 3 || s.zeroMask || s.oneMask) w |= DXB_CH_SWIZZLE;
+    if (s.colorKey) w |= DXB_CH_COLOR_KEY;
+    if (s.invertY) w |= DXB_CH_INVERT_Y;
+    if (s.reconstructZ) w |= DXB_CH_RECONSTRUCT_Z;
+    return (w & DXB_CH_STEPS) ? w : 0u;
+}
+
+// TransformImage's checks in its order (:646-701, TransformImage_ :220-227), then this library's: the steps stand in for the
+// reference's pixelFunc, so none enabled is its null function (E_INVALIDARG, checked where TransformImage_ checks it, on image 0).
+// P = the k_convert launch that runs them (srcFormat == dstFormat selects the steps).
+int32_t plan_channel_steps(const dxb200_image* src, size_t n, const dxb200_channel_steps* steps, const dxb200_image* dst, dxb_convert_params* P)
+{
+    if (!src || !dst || !steps || !n) return DXB_E_INVALIDARG;
+    const uint32_t fmt = src[0].format;
+    if (!is_supported_pixel_format(fmt)) return DXB_E_NOT_SUPPORTED;            // compressed, typeless, planar, palettized, other (:649)
+    if (src[0].width > 0xFFFFFFFFull || src[0].height > 0xFFFFFFFFull) return DXB_E_INVALIDARG;
+    const uint32_t word = channel_steps_word(*steps);
+    const bool valid = word && steps->swizzle[0] < 4 && steps->swizzle[1] < 4 && steps->swizzle[2] < 4 && steps->swizzle[3] < 4
+                    && !(steps->zeroMask & 0xF0u) && !(steps->oneMask & 0xF0u);
+    for (size_t i = 0; i < n; ++i)
+    {
+        if (src[i].format != fmt || src[i].width > 0xFFFFFFFFull || src[i].height > 0xFFFFFFFFull) return DXB_E_FAIL;     // :683-693
+        if (dst[i].format != fmt || dst[i].width != src[i].width || dst[i].height != src[i].height) return DXB_E_FAIL;  // :697, :226
+        if (i == 0 && !valid) return DXB_E_INVALIDARG;                                                                 // :220
+        if (!src[i].pixels || !dst[i].pixels) return DXB_E_POINTER;                                                     // :223
+    }
+    memset(P, 0, sizeof(*P));
+    P->srcFormat = P->dstFormat = fmt; P->inF = P->outF = dxb_convert_flags(fmt);
+    P->steps = word | ((dxb_convert_flags(fmt) & DXB_CONVF_UNORM) ? DXB_CH_UNORM : 0u);         // isunorm (:3252)
+    dxb_color_key_vector(steps->colorKeyValue, P->key);
+    return DXB_S_OK;
+}
+
+// The format texconv decompresses a BC base to when channel steps follow (:2393-2447): BC4 and BC5 hold one and two channels, so a
+// step that reads or writes another channel needs R8G8B8A8 (UNORM or SNORM as the BC format); otherwise DefaultDecompress.
+uint32_t channel_decompress_format(uint32_t bcFormat, const dxb200_channel_steps* s)
+{
+    const uint32_t def = dxb_default_decompress(bcFormat);
+    const bool bc4 = bcFormat == DXB_FMT_BC4_UNORM || bcFormat == DXB_FMT_BC4_SNORM, bc5 = bcFormat == DXB_FMT_BC5_UNORM || bcFormat == DXB_FMT_BC5_SNORM;
+    if (!s || !channel_steps_word(*s) || (!bc4 && !bc5)) return def;
+    bool wide = s->reconstructZ || (bc4 && s->invertY);
+    for (uint32_t c = bc4 ? 1u : 2u; c < 4; ++c) wide |= s->swizzle[c] != c || ((s->zeroMask | s->oneMask) >> c & 1u);
+    if (!wide) return def;
+    return (bcFormat == DXB_FMT_BC4_SNORM || bcFormat == DXB_FMT_BC5_SNORM) ? DXB_FMT_R8G8B8A8_SNORM : DXB_FMT_R8G8B8A8_UNORM;
+}
+
+// ---- Decompress -> Resize -> [channel steps] -> mipmaps_compress_ex in one call (mipmaps_compress_from) ------------------------
 // The per-item device images: base[i] (the caller's, BC or not, at its pitch), decompressed[i] (the base's size in the decompress
 // format at compute_pitch; in the buffer only when a resize follows, else it is level 0 of the chain), the chain (level 0 = W x H
 // at compute_pitch when a front step writes it) and the blocks.  Images the device makes carry base[i].pixels only for validation.
+// The channel steps run in place on level 0 of the chain.
 struct FromPlan
 {
-    bool decompress, resize;
+    bool decompress, resize, channels;
     dxb_compress_params dp;                     // the Decompress
     std::vector<dxb200_image> decompressed;
     uint32_t resizeFilter, resizeMode;          // the Resize, into level 0 of the chain
+    dxb_convert_params cp;                      // the channel steps
     ChainPlan chain;
 };
 
@@ -412,25 +468,28 @@ std::vector<dxb200_image> plan_images(const dxb200_image* base, size_t n, uint32
     return out;
 }
 
-// Every check of Decompress, Resize and the four steps of plan_mipmaps_compress before anything is uploaded, each with the HRESULT of
-// the first of the separate calls that would fail.  source == nullptr, or a source that changes nothing = plan_mipmaps_compress.
-int32_t plan_mipmaps_compress_from(const dxb200_image* base, size_t items, const dxb200_chain_source* source, size_t levels, uint32_t filter,
-                                   const dxb200_chain_steps* steps, uint32_t dstFormat, uint32_t flags, float threshold, const dxb200_image* dst,
-                                   FromPlan* fp)
+// Every check of Decompress, Resize, the channel steps and the four steps of plan_mipmaps_compress before anything is uploaded, each
+// with the HRESULT of the first of the separate calls that would fail.  source == nullptr, or a source that changes nothing, and
+// channels == nullptr, or no channel step enabled = plan_mipmaps_compress.
+int32_t plan_mipmaps_compress_channels(const dxb200_image* base, size_t items, const dxb200_chain_source* source, const dxb200_channel_steps* channels,
+                                       size_t levels, uint32_t filter, const dxb200_chain_steps* steps, uint32_t dstFormat, uint32_t flags,
+                                       float threshold, const dxb200_image* dst, FromPlan* fp)
 {
-    fp->decompress = fp->resize = false;
+    fp->decompress = fp->resize = fp->channels = false;
     fp->resizeFilter = fp->resizeMode = 0;
     fp->decompressed.clear();
     if (source && (!source->width) != (!source->height)) return DXB_E_INVALIDARG;
-    if (!source || !base || !items) return plan_mipmaps_compress(base, items, levels, filter, steps, dstFormat, flags, threshold, dst, &fp->chain);
-    const size_t w = source->width ? source->width : base[0].width, h = source->height ? source->height : base[0].height;
-    fp->decompress = is_compressed(base[0].format);
+    const bool ch = channels && channel_steps_word(*channels);
+    if ((!source && !ch) || !base || !items) return plan_mipmaps_compress(base, items, levels, filter, steps, dstFormat, flags, threshold, dst, &fp->chain);
+    const size_t w = source && source->width ? source->width : base[0].width, h = source && source->height ? source->height : base[0].height;
+    fp->decompress = source && is_compressed(base[0].format);
     fp->resize = (w != base[0].width || h != base[0].height);
     std::vector<dxb200_image> level0(base, base + items);
     int32_t hr = DXB_S_OK;
     if (fp->decompress)
     {
-        const uint32_t fmt = source->decompressFormat ? source->decompressFormat : dxb_default_decompress(base[0].format);
+        const uint32_t fmt = source->decompressFormat ? source->decompressFormat : ch ? channel_decompress_format(base[0].format, channels)
+                                                                                      : dxb_default_decompress(base[0].format);
         fp->decompressed = plan_images(base, items, fmt, 0, 0);
         if ((hr = plan_decompress(base, items, fmt, fp->decompressed.data(), &fp->dp)) != DXB_S_OK) return hr;
         level0 = fp->decompressed;
@@ -442,7 +501,16 @@ int32_t plan_mipmaps_compress_from(const dxb200_image* base, size_t items, const
         fp->resizeFilter = source->resizeFilter;
         level0 = resized;
     }
+    if (ch && (hr = plan_channel_steps(level0.data(), items, channels, level0.data(), &fp->cp)) != DXB_S_OK) return hr;
+    fp->channels = ch;
     return plan_mipmaps_compress(level0.data(), items, levels, filter, steps, dstFormat, flags, threshold, dst, &fp->chain);
+}
+
+int32_t plan_mipmaps_compress_from(const dxb200_image* base, size_t items, const dxb200_chain_source* source, size_t levels, uint32_t filter,
+                                   const dxb200_chain_steps* steps, uint32_t dstFormat, uint32_t flags, float threshold, const dxb200_image* dst,
+                                   FromPlan* fp)
+{
+    return plan_mipmaps_compress_channels(base, items, source, nullptr, levels, filter, steps, dstFormat, flags, threshold, dst, fp);
 }
 
 // ---- IsAlphaAllOpaque (DirectXTexImage.cpp:800-852; IsAlphaAllOpaqueBC, DirectXTexCompress.cpp:539-621) ---------------------

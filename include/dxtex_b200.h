@@ -182,6 +182,52 @@ DXB200_API int32_t  dxb200_mipmaps_compress_from_ex(const dxb200_image* base, si
                                                     uint32_t flags, float threshold, float alphaWeight, const dxb200_image* dst,
                                                     int32_t* alphaAllOpaque);
 
+/* texconv's four channel steps between Resize and GenerateMipMaps, each a DirectX::TransformImage (DirectXTexMisc.cpp:606-760) of
+ * the image in its own format, run in this order when enabled:
+ *   swizzle        (-swizzle, Texconv/texconv.cpp:2645-2694): out[c] = in[swizzle[c]], then the channels of zeroMask (bit c =
+ *                  channel c) become 0 and those of oneMask 1.  Enabled unless swizzle == {0, 1, 2, 3} and both masks are 0.
+ *   colour key     (-c, :3134-3191): a pixel whose x, y and z each lie within 0.2 of the key colorKeyValue & 0xFFFFFF (0xRRGGBB,
+ *                  loaded as an XMCOLOR) becomes (0, 0, 0, 0), every other pixel gets alpha 1.  texconv enables it only for a
+ *                  format with alpha.
+ *   invert Y       (-inverty, :3193-3240): y = 1 - y.
+ *   reconstruct Z  (-reconstructz, :3242-3300): z = sqrt(1 - (x*x + y*y)), on x*2 - 1 and y*2 - 1 and mapped back by z*0.5 + 0.5
+ *                  for a UNORM (or sRGB) format; x*x + y*y > 1 gives a NaN z, stored as the format stores a NaN.
+ * Each step loads the pixel without an sRGB step and stores it at alpha threshold 0, so a step sees the previous one's stored
+ * result (an 8-bit format is quantised between steps). */
+typedef struct dxb200_channel_steps
+{
+    uint8_t  swizzle[4];        /* source channel (0..3) of each output channel */
+    uint8_t  zeroMask, oneMask; /* bits 0..3: channels forced to 0, then channels forced to 1 */
+    uint8_t  colorKey;          /* nonzero: the colour key step */
+    uint8_t  invertY;           /* nonzero: the invert Y step */
+    uint8_t  reconstructZ;      /* nonzero: the reconstruct Z step */
+    uint32_t colorKeyValue;     /* the key, 0xRRGGBB (higher bits are ignored) */
+} dxb200_channel_steps;
+/* The enabled steps of `steps` on src[i] -> dst[i], i < n: every source has src[0]'s format, every destination its source's
+ * format and size; dst may be src (same pixels and pitch).  HRESULTs, in TransformImage's order: src / dst / steps NULL or n == 0
+ * -> E_INVALIDARG; a compressed, typeless, planar or palettized format, or one this library does not implement ->
+ * E_NOT_SUPPORTED (0x80070032); src[0] wider or higher than 2^32 - 1 -> E_INVALIDARG; then per image a source of another format or
+ * over 32 bits, or a destination of another format or size -> E_FAIL; no step enabled (image 0), a swizzle element above 3 or a
+ * mask bit above bit 3 -> E_INVALIDARG; a NULL pixel pointer -> E_POINTER.  The host call stages the images in bands, sharded over
+ * the initialised devices, as dxb200_convert does; the _device call enqueues on `stream` and returns. */
+DXB200_API int32_t  dxb200_apply_channel_steps(const dxb200_image* src, size_t n, const dxb200_channel_steps* steps, const dxb200_image* dst);
+DXB200_API int32_t  dxb200_apply_channel_steps_device(const dxb200_image* src, size_t n, const dxb200_channel_steps* steps,
+                                                      const dxb200_image* dst, void* stream);
+/* dxb200_mipmaps_compress_from_ex with texconv's channel steps between Resize and GenerateMipMaps (Texconv/texconv.cpp:2645-3300):
+ * results identical to dxb200_decompress, dxb200_resize, dxb200_apply_channel_steps on level 0 and
+ * dxb200_mipmaps_compress_from_ex.  The steps run in device memory, in place on every chain's level 0: one more k_convert launch
+ * per chunk, no more memory.  With steps enabled and decompressFormat == 0, a BC4 / BC5 base decompresses to the format texconv
+ * picks (:2393-2447): R8G8B8A8_UNORM (BC4_UNORM, BC5_UNORM) or R8G8B8A8_SNORM (the SNORM twins) when a step needs more channels
+ * than R8 / R8G8 hold (BC4: invert Y, reconstruct Z, a swizzle or mask of channels 1-3; BC5: reconstruct Z, a swizzle or mask of
+ * channels 2-3), else DefaultDecompress.  A failing call returns the HRESULT of the first of those calls that would fail, the
+ * channel steps checked on level 0's format and size.  channels == NULL, or no step enabled, is exactly
+ * dxb200_mipmaps_compress_from_ex. */
+DXB200_API int32_t  dxb200_mipmaps_compress_from_channels(const dxb200_image* base, size_t items, const dxb200_chain_source* source,
+                                                          const dxb200_channel_steps* channels, size_t levels, uint32_t filter,
+                                                          const dxb200_chain_steps* steps, uint32_t dstFormat, uint32_t flags,
+                                                          float threshold, float alphaWeight, const dxb200_image* dst,
+                                                          int32_t* alphaAllOpaque);
+
 /* ScratchImage::IsAlphaAllOpaque (DirectXTexImage.cpp:800-852; IsAlphaAllOpaqueBC, DirectXTexCompress.cpp:539-621) of
  * `nimages` images of one format: *opaque = 1 when every texel inside every image has alpha >= 0.997 (uncompressed, as
  * LoadScanline reads it) or >= 0.99 (decoded BC1 / BC2 / BC3 / BC7 blocks; the padding texels of partial blocks do not count),
