@@ -170,19 +170,26 @@ DXB_DEV dxb_px dxb_mip_cubic(uint32_t fmt, const dxb_mip_job& j, uint32_t x, uin
     return dxb_cubic4(ty.x, C[0], C[1], C[2], C[3]);
 }
 
-// ---- TRIANGLE: acc = row[x] * (wy*wx) + acc, rows ascending then x ascending (:1516-1538)
+// ---- TRIANGLE: acc = row[x] * (wy*wx) + acc in the reference's order (:1516-1538): source rows ascending, then source x
+// ascending, then that row's entries for this destination row, then that column's entries for this destination column.  A row
+// (column) has two entries for one destination when wrap brings it back around a short axis; the entries of one source row
+// (column) are adjacent in the gather lists.
 DXB_DEV dxb_px dxb_mip_triangle(uint32_t fmt, const dxb_mip_job& j, uint32_t x, uint32_t y, uint32_t lflags,
                                 const dxb_tri_axis& ax, const dxb_tri_axis& ay)
 {
     dxb_px acc = dxb_make_px(0.0f, 0.0f, 0.0f, 0.0f);
-    for (uint32_t iy = ay.off[y]; iy < ay.off[y + 1]; ++iy)
+    const uint32_t yEnd = ay.off[y + 1], xEnd = ax.off[x + 1];
+    for (uint32_t iy = ay.off[y], ny; iy < yEnd; iy = ny)
     {
-        const uint32_t sy = ay.src[iy]; const float wy = ay.w[iy];
-        for (uint32_t ix = ax.off[x]; ix < ax.off[x + 1]; ++ix)
+        const uint32_t sy = ay.src[iy];
+        for (ny = iy + 1; ny < yEnd && ay.src[ny] == sy; ++ny) {}
+        for (uint32_t ix = ax.off[x], nx; ix < xEnd; ix = nx)
         {
-            const float wgt = wy * ax.w[ix];
-            const dxb_px p = dxb_load_linear(fmt, j.src, j.srcPitch, ax.src[ix], sy, lflags);
-            acc = dxb_px_add(dxb_px_scale(p, wgt), acc);
+            const uint32_t sx = ax.src[ix];
+            for (nx = ix + 1; nx < xEnd && ax.src[nx] == sx; ++nx) {}
+            const dxb_px p = dxb_load_linear(fmt, j.src, j.srcPitch, sx, sy, lflags);
+            for (uint32_t ey = iy; ey < ny; ++ey)
+                for (uint32_t ex = ix; ex < nx; ++ex) acc = dxb_px_add(dxb_px_scale(p, ay.w[ey] * ax.w[ex]), acc);
         }
     }
     if (fmt == DXB_FMT_R10G10B10A2_UNORM) acc.w = acc.w + 0.1f;      // Bias {0,0,0,0.1} (:1560-1575)

@@ -150,13 +150,9 @@ static std::vector<dxb200_image> emul_chain(const uint8_t* base, const size_t* o
     return chain;
 }
 
-extern "C" int32_t emul_generate_mipmaps(uint8_t* chainBase, const size_t* offsets, const size_t* widths, const size_t* heights,
-                                         const size_t* pitches, size_t levels, uint32_t fmt, uint32_t filter)
+// levels 1 .. levels-1 of one chain planned by build_mip_plan, every pixel through dxb_mip_pixel
+static void emul_run_mip_plan(const std::vector<dxb200_image>& chain, size_t levels, uint32_t filter, uint32_t mode)
 {
-    const std::vector<dxb200_image> chain = emul_chain(chainBase, offsets, widths, heights, pitches, levels, fmt);
-    uint32_t mode = 0;
-    const int32_t hr = plan_mips(chain.data(), 1, levels, filter, &mode);
-    if (hr != DXB_S_OK) return hr;
     const MipPlan mp = build_mip_plan(chain.data(), 1, levels, filter, mode);
     for (size_t l = 1; l < levels; ++l)
     {
@@ -171,6 +167,27 @@ extern "C" int32_t emul_generate_mipmaps(uint8_t* chainBase, const size_t* offse
         for (uint32_t y = 0; y < j.dh; ++y)
             for (uint32_t x = 0; x < j.dw; ++x) dxb_mip_pixel(mp.P.format, mp.P.mode, j, x, y, mp.P.filter, mp.P.lflags, ax, ay);
     }
+}
+
+extern "C" int32_t emul_generate_mipmaps(uint8_t* chainBase, const size_t* offsets, const size_t* widths, const size_t* heights,
+                                         const size_t* pitches, size_t levels, uint32_t fmt, uint32_t filter)
+{
+    const std::vector<dxb200_image> chain = emul_chain(chainBase, offsets, widths, heights, pitches, levels, fmt);
+    uint32_t mode = 0;
+    const int32_t hr = plan_mips(chain.data(), 1, levels, filter, &mode);
+    if (hr != DXB_S_OK) return hr;
+    emul_run_mip_plan(chain, levels, filter, mode);
+    return DXB_S_OK;
+}
+
+// Resize of one tight w x h image to width x height: the library plans it as a chain of two levels (plan_resize)
+extern "C" int32_t emul_resize(const uint8_t* src, size_t w, size_t h, uint32_t fmt, size_t width, size_t height, uint32_t filter, uint8_t* dst)
+{
+    const std::vector<dxb200_image> chain = { emul_image(src, w, h, fmt, 0), emul_image(dst, width, height, fmt, 0) };
+    uint32_t mode = 0;
+    const int32_t hr = plan_resize(&chain[0], 1, filter, &chain[1], &mode);
+    if (hr != DXB_S_OK) return hr;
+    emul_run_mip_plan(chain, 2, filter, mode);
     return DXB_S_OK;
 }
 

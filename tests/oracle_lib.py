@@ -161,6 +161,7 @@ class Emul:
         L.emul_compress.argtypes = [vp, sz, sz, u32, sz, u32, u32, f32, vp]
         L.emul_convert.argtypes = [vp, sz, sz, u32, sz, u32, sz, u32, vp]
         L.emul_generate_mipmaps.argtypes = [vp] + [C.POINTER(sz)] * 4 + [sz, u32, u32]
+        L.emul_resize.argtypes = [vp, sz, sz, u32, sz, sz, u32, vp]
         L.emul_scale_mips_alpha.argtypes = [vp, vp] + [C.POINTER(sz)] * 4 + [sz, u32, C.c_float]
         L.emul_decompress.argtypes = [vp, sz, sz, u32, u32, vp]
 
@@ -192,6 +193,12 @@ class Emul:
         off, ws, hs, ps = A(*[l[0] for l in layout]), A(*[l[1] for l in layout]), A(*[l[2] for l in layout]), A(*[l[3] for l in layout])
         hr = self.L.emul_generate_mipmaps(chain.ctypes.data, off, ws, hs, ps, len(layout), fmt, filter)
         return F.hr_u32(hr), chain
+
+    def resize(self, src, w, h, fmt, width, height, filter=0):
+        src = np.ascontiguousarray(src)
+        out = np.zeros(width * height * F.BYTES_PER_PIXEL[fmt], np.uint8)
+        hr = self.L.emul_resize(src.ctypes.data, w, h, fmt, width, height, filter, out.ctypes.data)
+        return F.hr_u32(hr), out
 
     def scale_mips_alpha(self, chain, w, h, fmt, alpha_ref):
         layout, total = F.mip_chain_layout(fmt, w, h, 0)
