@@ -17,6 +17,7 @@ SYMBOLS = [
     "dxb200_scale_mipmaps_alpha_for_coverage", "dxb200_scale_mipmaps_alpha_for_coverage_device",
     "dxb200_is_alpha_all_opaque", "dxb200_is_alpha_all_opaque_device",
     "dxb200_apply_channel_steps", "dxb200_apply_channel_steps_device", "dxb200_mipmaps_compress_from_channels",
+    "dxb200_mipmaps_convert_from",
     "dxb200_dds_encode_header", "dxb200_dds_save_memory", "dxb200_dds_get_metadata", "dxb200_dds_load_memory",
 ]
 
@@ -92,6 +93,8 @@ def _load():
     lib.dxb200_mipmaps_compress_from_channels.argtypes = [IP, C.c_size_t, C.POINTER(ChainSource), C.POINTER(ChannelSteps), C.c_size_t, C.c_uint32,
                                                           C.POINTER(ChainSteps), C.c_uint32, C.c_uint32, C.c_float, C.c_float, IP,
                                                           C.POINTER(C.c_int32)]
+    lib.dxb200_mipmaps_convert_from.argtypes = [IP, C.c_size_t, C.POINTER(ChainSource), C.POINTER(ChannelSteps), C.c_uint32, C.c_uint32,
+                                                C.c_float, C.c_size_t, C.c_uint32, C.POINTER(ChainSteps), IP, C.POINTER(C.c_int32)]
     lib.dxb200_apply_channel_steps.argtypes = [IP, C.c_size_t, C.POINTER(ChannelSteps), IP]
     lib.dxb200_apply_channel_steps_device.argtypes = [IP, C.c_size_t, C.POINTER(ChannelSteps), IP, C.c_void_p]
     lib.dxb200_is_alpha_all_opaque.argtypes = [IP, C.c_size_t, C.POINTER(C.c_int32)]
@@ -121,7 +124,7 @@ def _load():
     lib.dxb200_dds_load_memory.argtypes = [C.c_void_p, C.c_size_t, C.c_uint32, IP, C.c_size_t]
     for name in ("dxb200_dds_encode_header", "dxb200_dds_save_memory", "dxb200_dds_get_metadata", "dxb200_dds_load_memory"):
         getattr(lib, name).restype = C.c_int32
-    for name in ("dxb200_init", "dxb200_init_devices", "dxb200_initialized_devices", "dxb200_compress_ex", "dxb200_convert_ex", "dxb200_mipmaps_compress", "dxb200_mipmaps_compress_ex", "dxb200_mipmaps_compress_from", "dxb200_mipmaps_compress_from_ex", "dxb200_is_alpha_all_opaque", "dxb200_is_alpha_all_opaque_device", "dxb200_apply_channel_steps", "dxb200_apply_channel_steps_device", "dxb200_mipmaps_compress_from_channels", "dxb200_device_count", "dxb200_compute_pitch", "dxb200_calculate_mip_levels", "dxb200_compress",
+    for name in ("dxb200_init", "dxb200_init_devices", "dxb200_initialized_devices", "dxb200_compress_ex", "dxb200_convert_ex", "dxb200_mipmaps_compress", "dxb200_mipmaps_compress_ex", "dxb200_mipmaps_compress_from", "dxb200_mipmaps_compress_from_ex", "dxb200_is_alpha_all_opaque", "dxb200_is_alpha_all_opaque_device", "dxb200_apply_channel_steps", "dxb200_apply_channel_steps_device", "dxb200_mipmaps_compress_from_channels", "dxb200_mipmaps_convert_from", "dxb200_device_count", "dxb200_compute_pitch", "dxb200_calculate_mip_levels", "dxb200_compress",
                  "dxb200_compress_device", "dxb200_decompress", "dxb200_decompress_device", "dxb200_convert",
                  "dxb200_convert_device", "dxb200_generate_mipmaps", "dxb200_generate_mipmaps_device", "dxb200_resize", "dxb200_resize_device", "dxb200_premultiply_alpha", "dxb200_premultiply_alpha_device"):
         getattr(lib, name).restype = C.c_int32
@@ -280,6 +283,27 @@ def mipmaps_compress_from_channels(bases, w, h, base_fmt, dst_fmt, source=None, 
     hr = lib.dxb200_mipmaps_compress_from_channels(*args[:3], C.byref(channels) if channels is not None else None, *args[3:], C.byref(opaque))
     if hr != 0:
         raise DxTexError(hr, "dxb200_mipmaps_compress_from_channels")
+    return outs, opaque.value == 1
+
+
+def mipmaps_convert_from(bases, w, h, base_fmt, dst_fmt, source=None, channels=None, convert_filter=0, threshold=0.5, filter=0, levels=0,
+                         steps=None):
+    """dxb200_mipmaps_convert_from of an array of equally sized w x h host images of base_fmt (BC or not) into dst_fmt chains, with
+    the ChainSource `source`, the ChannelSteps `channels` and the ChainSteps `steps` (None: none): (one chain per image, laid out as
+    texture_layout(dst_fmt, W, H, 1, levels), IsAlphaAllOpaque of the output as a bool)"""
+    bases = [np.ascontiguousarray(a).view(np.uint8).reshape(-1) for a in bases]
+    cw, ch = (source.width, source.height) if source is not None and source.width else (w, h)
+    levels = levels or F.count_mips(cw, ch)
+    olayout, total = texture_layout(dst_fmt, cw, ch, 1, levels)
+    outs = [np.zeros(total, np.uint8) for _ in bases]
+    s = images([make_image(_np_ptr(a), w, h, base_fmt) for a in bases])
+    d = images([Image(lw, lh, dst_fmt, r, sp, _np_ptr(o) + off) for o in outs for (off, lw, lh, r, sp) in olayout])
+    opaque = C.c_int32(-1)
+    hr = lib.dxb200_mipmaps_convert_from(s, len(bases), C.byref(source) if source is not None else None,
+                                         C.byref(channels) if channels is not None else None, dst_fmt, convert_filter, threshold, levels,
+                                         filter, C.byref(steps) if steps is not None else None, d, C.byref(opaque))
+    if hr != 0:
+        raise DxTexError(hr, "dxb200_mipmaps_convert_from")
     return outs, opaque.value == 1
 
 

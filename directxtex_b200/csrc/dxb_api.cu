@@ -675,49 +675,61 @@ struct ResultWords
     bool all_zero() const { return std::all_of(w, w + n, [](uint32_t v) { return v == 0; }); }
 };
 
-// ---- [Decompress] -> [Resize] -> GenerateMipMaps -> [coverage] -> [premultiply] -> Compress, chunk by chunk ---------------------
+// ---- [Decompress] -> [Resize] -> [channel steps] -> [Convert] -> [channel steps] -> GenerateMipMaps -> [coverage] -> [premultiply]
+// -> [Compress], chunk by chunk ---------------------------------------------------------------------------------------------------
 // texconv runs GenerateMipMaps and then Compress on the result (Texconv/texconv.cpp; SURVEY 3.5), after Decompress (:2316-2480) for
 // a BC input and Resize (:2576-2643) for a new size; with the host-pointer calls every intermediate travels device -> host ->
 // device.  Here each item's base goes up once, every step runs in device memory and only the packed blocks come back: 4 B/texel
 // up + 1.33 B/texel down for BC3 from RGBA8 instead of 4 + 5.33 + 5.33 + 1.33.  Chunks of whole items are pipelined over the
 // lane's NSLOT (stream, buffer) slots.  A chunk holds, per item and in plane order: the base as the caller laid it out (when a
-// front step reads it), the decompressed image (only when a resize follows), the chain (level 0 uploaded when no front step writes
-// it) and the blocks.  With no front step that is exactly the chain and the blocks.  Channel steps (fp.channels) run in place on
-// every item's level 0 after the front steps or the upload, one launch per chunk and no plane of their own.  With a scan (words !=
-// nullptr: one result word per item, see dxb200_mipmaps_compress_from_ex) one more plane holds the items' words; they are cleared,
-// set by one scan launch over all the chunk's blocks after the compression, and come back with the blocks.
+// device step reads it), the decompressed image (only when a resize follows), the pre-Convert level 0 (when a front step writes
+// it and a Convert follows), the chain (level 0 uploaded when no front step writes it and the output is compressed) and the blocks.
+// With no front step that is exactly the chain and the blocks.  Channel steps (fp.channels) run in place on every item's level 0
+// after the front steps or the upload, one launch per chunk and no plane of their own.  For an uncompressed output (mipmaps_
+// convert_from) the chain is the caller's dst, at its pitches, and every level comes back; the Convert writes its level 0 and the
+// later channel steps (fp.post) run in place there.  When no step writes that level 0 (no front step, no Convert), the uploaded
+// base is copied into it device to device.  With a scan (words != nullptr: one result word per item, see
+// dxb200_mipmaps_compress_from_ex) one more plane holds the items' words; they are cleared, set by one scan launch over all the
+// chunk's output after its last step, and come back with it.
 int32_t run_chains(const dxb200_image* base, size_t items, size_t levels, uint32_t filter, const FromPlan& fp, const dxb200_image* dst,
                    const AlphaOpaquePlan& scan, const ResultWords* words)
 {
     const ChainPlan& cp = fp.chain;
-    const bool front = fp.decompress || fp.resize, mid = fp.decompress && fp.resize;
+    const bool front = fp.decompress || fp.resize, mid = fp.decompress && fp.resize, pre = front && fp.convert;
+    const bool up = !front && cp.compressed;                   // the chain's level 0 is uploaded; otherwise the base is
     const std::vector<dxb200_image> wimg = words ? words->images() : std::vector<dxb200_image>();
     return run_sharded(items, [&](size_t i) { return cp.chain[i * levels].slicePitch; },
         [&](size_t lo, size_t hi)
         {
             std::vector<Plane> planes;
-            if (front) planes.push_back({ base + lo, 1, Copy::Up, Copy::Up });
+            if (!up) planes.push_back({ base + lo, 1, Copy::Up, Copy::Up });
             if (mid) planes.push_back({ fp.decompressed.data() + lo, 1, Copy::None, Copy::None });
+            if (pre) planes.push_back({ fp.level0.data() + lo, 1, Copy::None, Copy::None });
             const size_t pc = planes.size();                    // the chains' plane, then the blocks' and the words'
-            planes.push_back({ cp.chain.data() + lo * levels, levels, front ? Copy::None : Copy::Up, Copy::None });
+            if (cp.compressed) planes.push_back({ cp.chain.data() + lo * levels, levels, up ? Copy::Up : Copy::None, Copy::None });
             planes.push_back({ dst + lo * levels, levels, Copy::Down, Copy::Down });
             if (words) planes.push_back({ wimg.data() + lo, 1, Copy::Down, Copy::Down });
             return run_staged(planes.data(), planes.size(), hi - lo, ITEM_CHUNK,
                 [&](const std::vector<dxb200_image>* dev, size_t cnt, cudaStream_t st)
                 {
-                    const dxb200_image* src = front ? dev[0].data() : nullptr;
+                    const dxb200_image* src = up ? nullptr : dev[0].data();
                     const dxb200_image* decompressed = mid ? dev[1].data() : nullptr;
                     const dxb200_image* chains = dev[pc].data();
-                    const dxb200_image* blocks = dev[pc + 1].data();
+                    const dxb200_image* out = dev[cp.compressed ? pc + 1 : pc].data();
                     int32_t h2 = DXB_S_OK;
                     std::vector<dxb200_image> level(cnt);
                     for (size_t it = 0; it < cnt; ++it) level[it] = chains[it * levels];
-                    if (front)
-                    {
-                        if (fp.decompress) h2 = launch_decompress(fp.dp, src, mid ? decompressed : level.data(), cnt, st);
-                        if (h2 == DXB_S_OK && fp.resize) h2 = launch_resize(mid ? decompressed : src, level.data(), cnt, fp.resizeFilter, fp.resizeMode, st);
-                    }
-                    if (h2 == DXB_S_OK && fp.channels) h2 = launch_channel_steps(fp.cp, level.data(), level.data(), cnt, st);
+                    // the image the front steps write and the channel steps (the swizzle, with a Convert) run on
+                    const dxb200_image* first = pre ? dev[pc - 1].data() : fp.convert && !front ? src : level.data();
+                    if (fp.decompress) h2 = launch_decompress(fp.dp, src, mid ? decompressed : first, cnt, st);
+                    if (h2 == DXB_S_OK && fp.resize) h2 = launch_resize(mid ? decompressed : src, first, cnt, fp.resizeFilter, fp.resizeMode, st);
+                    for (size_t it = 0; it < cnt && h2 == DXB_S_OK && !up && !front && !fp.convert; ++it)
+                        h2 = cuda_hr(cudaMemcpy2DAsync(level[it].pixels, level[it].rowPitch, src[it].pixels, src[it].rowPitch,
+                                                       level[it].width * dxb_bytes_per_pixel(level[it].format), level[it].height,
+                                                       cudaMemcpyDeviceToDevice, st), "base -> level 0");
+                    if (h2 == DXB_S_OK && fp.channels) h2 = launch_channel_steps(fp.cp, first, first, cnt, st);
+                    if (h2 == DXB_S_OK && fp.convert) h2 = launch_convert(fp.cv, first, level.data(), cnt, st);
+                    if (h2 == DXB_S_OK && fp.post) h2 = launch_channel_steps(fp.pp, level.data(), level.data(), cnt, st);
                     if (h2 == DXB_S_OK) h2 = launch_mips(chains, cnt, levels, filter, cp.mode, st);
                     if (h2 == DXB_S_OK && cp.coverage) h2 = launch_coverage(chains, chains, cnt, levels, cp.ref, st);
                     // one launch per level: the chunk's images of a level are equal, as the separate calls' images are, so they take the
@@ -727,14 +739,14 @@ int32_t run_chains(const dxb200_image* base, size_t items, size_t levels, uint32
                         for (size_t it = 0; it < cnt; ++it) level[it] = chains[it * levels + l];
                         h2 = launch_pmalpha(cp.pm, level.data(), level.data(), cnt, st);
                     }
-                    if (h2 == DXB_S_OK) h2 = launch_compress(cp.compress, chains, blocks, cnt * levels, st);
+                    if (h2 == DXB_S_OK && cp.compressed) h2 = launch_compress(cp.compress, chains, out, cnt * levels, st);
                     if (h2 == DXB_S_OK && words)
                     {
-                        const std::vector<dxb200_image>& w = dev[pc + 2];
+                        const std::vector<dxb200_image>& w = dev[planes.size() - 1];
                         std::vector<dxb200_image> jobWords(cnt * levels);      // every level of an item sets the item's word
                         for (size_t i = 0; i < jobWords.size(); ++i) jobWords[i] = w[i / levels];
                         h2 = clear_words(w, st);
-                        if (h2 == DXB_S_OK) h2 = launch_alpha_opaque(scan, blocks, jobWords.data(), jobWords.size(), st);
+                        if (h2 == DXB_S_OK) h2 = launch_alpha_opaque(scan, out, jobWords.data(), jobWords.size(), st);
                     }
                     return h2;
                 });
@@ -1028,6 +1040,23 @@ int32_t dxb200_mipmaps_compress(const dxb200_image* base, size_t items, size_t l
                                 uint32_t flags, float threshold, float alphaWeight, const dxb200_image* dst)
 {
     return dxb200_mipmaps_compress_ex(base, items, levels, filter, nullptr, dstFormat, flags, threshold, alphaWeight, dst);
+}
+
+// ---- texconv's path to an uncompressed target in one call: the chain never leaves HBM until it is done (run_chains) ------------
+int32_t dxb200_mipmaps_convert_from(const dxb200_image* base, size_t items, const dxb200_chain_source* source, const dxb200_channel_steps* channels,
+                                    uint32_t dstFormat, uint32_t convertFilter, float threshold, size_t levels, uint32_t filter,
+                                    const dxb200_chain_steps* steps, const dxb200_image* dst, int32_t* alphaAllOpaque)
+{
+    FromPlan fp;
+    AlphaOpaquePlan ap;
+    int32_t hr = plan_mipmaps_convert_from(base, items, source, channels, dstFormat, convertFilter, threshold, levels, filter, steps, dst,
+                                           alphaAllOpaque, &fp, &ap);
+    if (hr != DXB_S_OK) return hr;
+    ResultWords words;
+    if (ap.scan && (hr = words.alloc(items)) != DXB_S_OK) return hr;
+    hr = run_chains(base, items, levels, filter, fp, dst, ap, ap.scan ? &words : nullptr);
+    if (hr == DXB_S_OK && alphaAllOpaque) *alphaAllOpaque = (!ap.scan || words.all_zero()) ? 1 : 0;
+    return hr;
 }
 
 int32_t dxb200_premultiply_alpha_device(const dxb200_image* src, size_t nimages, uint32_t flags, const dxb200_image* dst, void* stream)

@@ -339,17 +339,33 @@ int32_t plan_coverage_jobs(const dxb200_image* chains, const dxb200_image* out, 
     return DXB_S_OK;
 }
 
-// ---- GenerateMipMaps -> ScaleMipMapsAlphaForCoverage -> PremultiplyAlpha -> Compress in one call (mipmaps_compress) ----------
-// chain = the chain every item will have on the device (ScratchImage layout of the source format; level 0 at the caller's
-// pitch, its pixels the upload source; the other levels carry base[i].pixels only for validation).
+// ---- GenerateMipMaps -> ScaleMipMapsAlphaForCoverage -> PremultiplyAlpha -> [Compress] in one call (mipmaps_compress) ------------
+// chain = the chain every item will have on the device: for a compressed output, the ScratchImage layout of the source format (level
+// 0 at the caller's pitch, its pixels the upload source; the other levels carry base[i].pixels only for validation); for an
+// uncompressed output (compressed == false), the caller's dst itself.
 struct ChainPlan
 {
     std::vector<dxb200_image> chain;
     uint32_t mode;
     bool coverage; float ref;
     bool premultiply; dxb_convert_params pm;
-    CompressPlan compress;
+    bool compressed; CompressPlan compress;
 };
+
+// GenerateMipMaps, then the optional coverage and premultiply steps of `steps`, on cp->chain, with the HRESULT of the first of those
+// calls that would fail
+int32_t plan_chain_steps(size_t items, size_t levels, uint32_t filter, const dxb200_chain_steps* steps, ChainPlan* cp)
+{
+    const dxb200_image* chain = cp->chain.data();
+    int32_t hr = plan_mips(chain, items, levels, filter, &cp->mode);
+    if (hr != DXB_S_OK) return hr;
+    cp->ref = steps ? steps->alphaReference : 0.0f;
+    cp->coverage = cp->ref > 0.0f;                                                      // texconv -keepcoverage (:3304)
+    if (cp->coverage && (hr = plan_alpha_coverage(chain, items * levels, chain)) != DXB_S_OK) return hr;
+    cp->premultiply = steps && steps->premultiply;
+    if (cp->premultiply && (hr = plan_pmalpha(chain, items * levels, steps->pmalphaFlags, chain, &cp->pm)) != DXB_S_OK) return hr;
+    return DXB_S_OK;
+}
 
 // Every check of the four steps before anything is uploaded, each with the HRESULT the reference's four calls would return at
 // the first step that fails; steps == nullptr (or no step enabled) = GenerateMipMaps + Compress.
@@ -376,13 +392,9 @@ int32_t plan_mipmaps_compress(const dxb200_image* base, size_t items, size_t lev
         }
         chain[i * levels].rowPitch = base[i].rowPitch; chain[i * levels].slicePitch = base[i].slicePitch;
     }
-    int32_t hr = plan_mips(chain.data(), items, levels, filter, &cp->mode);
+    const int32_t hr = plan_chain_steps(items, levels, filter, steps, cp);
     if (hr != DXB_S_OK) return hr;
-    cp->ref = steps ? steps->alphaReference : 0.0f;
-    cp->coverage = cp->ref > 0.0f;                                                      // texconv -keepcoverage (:3304)
-    if (cp->coverage && (hr = plan_alpha_coverage(chain.data(), items * levels, chain.data())) != DXB_S_OK) return hr;
-    cp->premultiply = steps && steps->premultiply;
-    if (cp->premultiply && (hr = plan_pmalpha(chain.data(), items * levels, steps->pmalphaFlags, chain.data(), &cp->pm)) != DXB_S_OK) return hr;
+    cp->compressed = true;
     return plan_compress(chain.data(), items * levels, dstFormat, flags, threshold, dst, &cp->compress);
 }
 
@@ -439,18 +451,23 @@ uint32_t channel_decompress_format(uint32_t bcFormat, const dxb200_channel_steps
     return (bcFormat == DXB_FMT_BC4_SNORM || bcFormat == DXB_FMT_BC5_SNORM) ? DXB_FMT_R8G8B8A8_SNORM : DXB_FMT_R8G8B8A8_UNORM;
 }
 
-// ---- Decompress -> Resize -> [channel steps] -> mipmaps_compress_ex in one call (mipmaps_compress_from) ------------------------
+// ---- Decompress -> Resize -> [channel steps] -> [Convert] -> [channel steps] -> mips ... [Compress] in one call ----------------
 // The per-item device images: base[i] (the caller's, BC or not, at its pitch), decompressed[i] (the base's size in the decompress
-// format at compute_pitch; in the buffer only when a resize follows, else it is level 0 of the chain), the chain (level 0 = W x H
-// at compute_pitch when a front step writes it) and the blocks.  Images the device makes carry base[i].pixels only for validation.
-// The channel steps run in place on level 0 of the chain.
+// format at compute_pitch; in the buffer only when a resize follows, else it is level0[i]), level0[i] (what the front steps leave,
+// W x H at compute_pitch; the base when no front step runs), the chain and, for a compressed output, the blocks.  Images the device
+// makes carry base[i].pixels only for validation.  Without a Convert, level0[i] is level 0 of the chain: the channel steps run in
+// place on it.  With a Convert (mipmaps_convert_from), the swizzle runs in place on level0[i], the Convert writes level 0 of the
+// chain in the target format and the later steps (post) run in place there.
 struct FromPlan
 {
-    bool decompress, resize, channels;
+    bool decompress, resize, channels, convert, post;
     dxb_compress_params dp;                     // the Decompress
     std::vector<dxb200_image> decompressed;
-    uint32_t resizeFilter, resizeMode;          // the Resize, into level 0 of the chain
-    dxb_convert_params cp;                      // the channel steps
+    uint32_t resizeFilter, resizeMode;          // the Resize
+    std::vector<dxb200_image> level0;
+    dxb_convert_params cp;                      // the channel steps (with a Convert: the swizzle and masks)
+    dxb_convert_params cv;                      // the Convert
+    dxb_convert_params pp;                      // colour key, invert Y and reconstruct Z after the Convert
     ChainPlan chain;
 };
 
@@ -468,23 +485,21 @@ std::vector<dxb200_image> plan_images(const dxb200_image* base, size_t n, uint32
     return out;
 }
 
-// Every check of Decompress, Resize, the channel steps and the four steps of plan_mipmaps_compress before anything is uploaded, each
-// with the HRESULT of the first of the separate calls that would fail.  source == nullptr, or a source that changes nothing, and
-// channels == nullptr, or no channel step enabled = plan_mipmaps_compress.
-int32_t plan_mipmaps_compress_channels(const dxb200_image* base, size_t items, const dxb200_chain_source* source, const dxb200_channel_steps* channels,
-                                       size_t levels, uint32_t filter, const dxb200_chain_steps* steps, uint32_t dstFormat, uint32_t flags,
-                                       float threshold, const dxb200_image* dst, FromPlan* fp)
+// Decompress (a BC base, when source != nullptr) and Resize (when the source's size differs) of the base, with the HRESULT of the
+// first that would fail; fp->level0 = the images they leave.  With channel steps and no decompress format, a BC4 / BC5 base
+// decompresses to channel_decompress_format.
+int32_t plan_front(const dxb200_image* base, size_t items, const dxb200_chain_source* source, const dxb200_channel_steps* channels, FromPlan* fp)
 {
-    fp->decompress = fp->resize = fp->channels = false;
+    fp->decompress = fp->resize = fp->channels = fp->convert = fp->post = false;
     fp->resizeFilter = fp->resizeMode = 0;
     fp->decompressed.clear();
+    fp->level0.clear();
     if (source && (!source->width) != (!source->height)) return DXB_E_INVALIDARG;
     const bool ch = channels && channel_steps_word(*channels);
-    if ((!source && !ch) || !base || !items) return plan_mipmaps_compress(base, items, levels, filter, steps, dstFormat, flags, threshold, dst, &fp->chain);
     const size_t w = source && source->width ? source->width : base[0].width, h = source && source->height ? source->height : base[0].height;
     fp->decompress = source && is_compressed(base[0].format);
     fp->resize = (w != base[0].width || h != base[0].height);
-    std::vector<dxb200_image> level0(base, base + items);
+    fp->level0.assign(base, base + items);
     int32_t hr = DXB_S_OK;
     if (fp->decompress)
     {
@@ -492,18 +507,39 @@ int32_t plan_mipmaps_compress_channels(const dxb200_image* base, size_t items, c
                                                                                       : dxb_default_decompress(base[0].format);
         fp->decompressed = plan_images(base, items, fmt, 0, 0);
         if ((hr = plan_decompress(base, items, fmt, fp->decompressed.data(), &fp->dp)) != DXB_S_OK) return hr;
-        level0 = fp->decompressed;
+        fp->level0 = fp->decompressed;
     }
     if (fp->resize)
     {
-        const std::vector<dxb200_image> resized = plan_images(base, items, level0[0].format, w, h);
-        if ((hr = plan_resize(level0.data(), items, source->resizeFilter, resized.data(), &fp->resizeMode)) != DXB_S_OK) return hr;
+        const std::vector<dxb200_image> resized = plan_images(base, items, fp->level0[0].format, w, h);
+        if ((hr = plan_resize(fp->level0.data(), items, source->resizeFilter, resized.data(), &fp->resizeMode)) != DXB_S_OK) return hr;
         fp->resizeFilter = source->resizeFilter;
-        level0 = resized;
+        fp->level0 = resized;
     }
-    if (ch && (hr = plan_channel_steps(level0.data(), items, channels, level0.data(), &fp->cp)) != DXB_S_OK) return hr;
+    return DXB_S_OK;
+}
+
+// Every check of Decompress, Resize, the channel steps and the four steps of plan_mipmaps_compress before anything is uploaded, each
+// with the HRESULT of the first of the separate calls that would fail.  source == nullptr, or a source that changes nothing, and
+// channels == nullptr, or no channel step enabled = plan_mipmaps_compress.
+int32_t plan_mipmaps_compress_channels(const dxb200_image* base, size_t items, const dxb200_chain_source* source, const dxb200_channel_steps* channels,
+                                       size_t levels, uint32_t filter, const dxb200_chain_steps* steps, uint32_t dstFormat, uint32_t flags,
+                                       float threshold, const dxb200_image* dst, FromPlan* fp)
+{
+    fp->decompress = fp->resize = fp->channels = fp->convert = fp->post = false;
+    fp->resizeFilter = fp->resizeMode = 0;
+    fp->decompressed.clear();
+    const bool ch = channels && channel_steps_word(*channels);
+    if ((!source && !ch) || !base || !items)
+    {
+        fp->level0.clear();
+        return plan_mipmaps_compress(base, items, levels, filter, steps, dstFormat, flags, threshold, dst, &fp->chain);
+    }
+    int32_t hr = plan_front(base, items, source, channels, fp);
+    if (hr != DXB_S_OK) return hr;
+    if (ch && (hr = plan_channel_steps(fp->level0.data(), items, channels, fp->level0.data(), &fp->cp)) != DXB_S_OK) return hr;
     fp->channels = ch;
-    return plan_mipmaps_compress(level0.data(), items, levels, filter, steps, dstFormat, flags, threshold, dst, &fp->chain);
+    return plan_mipmaps_compress(fp->level0.data(), items, levels, filter, steps, dstFormat, flags, threshold, dst, &fp->chain);
 }
 
 int32_t plan_mipmaps_compress_from(const dxb200_image* base, size_t items, const dxb200_chain_source* source, size_t levels, uint32_t filter,
@@ -556,6 +592,71 @@ dxb_convert_params alpha_opaque_pixel_params(const AlphaOpaquePlan& ap, uint32_t
     P.srcFormat = ap.format; P.dstFormat = DXB_SCAN_ALPHA_OPAQUE; P.inF = dxb_convert_flags(ap.format);
     P.totalUnits = units; P.njobs = njobs;
     return P;
+}
+
+// ---- Decompress -> Resize -> swizzle -> Convert -> later channel steps -> mips -> coverage -> premultiply in one call --------------
+// (mipmaps_convert_from) texconv's path to an uncompressed target (Texconv/texconv.cpp:2316-3560).  Every check of the nine
+// separate calls before anything is uploaded, each with the HRESULT of the first that would fail: plan_front; the swizzle and
+// masks of `channels` on level 0's format; Convert to dstFormat into level 0 of dst, only when level 0's format differs (texconv
+// tests info.format != tformat; a BC dstFormat always goes through Convert's checks, E_INVALIDARG); colour key, invert Y and
+// reconstruct Z on dst's level 0; GenerateMipMaps, coverage and premultiply on dst (plan_chain_steps); IsAlphaAllOpaque of dst
+// when alphaAllOpaque != nullptr.  Without a Convert, dst's level 0 must have level 0's format and size (E_INVALIDARG), the later
+// steps are checked from level 0 into dst's level 0, GenerateMipMaps on a chain whose level 0 is level 0 (every base's pixels and
+// format, when no front step runs), and the two groups of channel steps run as one launch, as dxb200_mipmaps_compress_from_channels
+// runs them.  levels < 2 is GenerateMipMaps' E_INVALIDARG, after the Convert's checks.
+int32_t plan_mipmaps_convert_from(const dxb200_image* base, size_t items, const dxb200_chain_source* source, const dxb200_channel_steps* channels,
+                                  uint32_t dstFormat, uint32_t convertFilter, float threshold, size_t levels, uint32_t filter,
+                                  const dxb200_chain_steps* steps, const dxb200_image* dst, const int32_t* alphaAllOpaque, FromPlan* fp,
+                                  AlphaOpaquePlan* ap)
+{
+    ap->scan = ap->blocks = false; ap->format = 0;
+    if (!base || !items) return DXB_E_INVALIDARG;
+    int32_t hr = plan_front(base, items, source, channels, fp);
+    if (hr != DXB_S_OK) return hr;
+    dxb200_channel_steps swizzle = { { 0, 1, 2, 3 }, 0, 0, 0, 0, 0, 0 }, later = swizzle;        // nothing enabled
+    if (channels)
+    {
+        memcpy(swizzle.swizzle, channels->swizzle, 4); swizzle.zeroMask = channels->zeroMask; swizzle.oneMask = channels->oneMask;
+        later.colorKey = channels->colorKey; later.colorKeyValue = channels->colorKeyValue;
+        later.invertY = channels->invertY; later.reconstructZ = channels->reconstructZ;
+    }
+    fp->channels = channel_steps_word(swizzle) != 0;
+    if (fp->channels && (hr = plan_channel_steps(fp->level0.data(), items, &swizzle, fp->level0.data(), &fp->cp)) != DXB_S_OK) return hr;
+    if (!dst) return DXB_E_INVALIDARG;
+    std::vector<dxb200_image>& chain = fp->chain.chain;
+    chain.assign(dst, dst + items * levels);
+    std::vector<dxb200_image> out0(items);
+    for (size_t i = 0; i < items; ++i) out0[i] = dst[i * levels];         // levels == 0: dst[0], refused by GenerateMipMaps below
+    fp->convert = fp->level0[0].format != dstFormat || is_compressed(dstFormat);
+    if (fp->convert)
+    {
+        if ((hr = plan_convert(fp->level0.data(), items, dstFormat, convertFilter, out0.data(), &fp->cv)) != DXB_S_OK) return hr;
+        fp->cv.threshold = threshold;
+    }
+    else
+        for (size_t i = 0; i < items; ++i)
+        {
+            if (out0[i].format != dstFormat || out0[i].width != fp->level0[i].width || out0[i].height != fp->level0[i].height) return DXB_E_INVALIDARG;
+            if (!out0[i].pixels) return DXB_E_POINTER;
+        }
+    // without a Convert the later steps read level 0 as the front steps leave it (the base when none runs) and write dst's level 0
+    fp->post = channel_steps_word(later) != 0;
+    if (fp->post && (hr = plan_channel_steps(fp->convert ? out0.data() : fp->level0.data(), items, &later, out0.data(), &fp->pp)) != DXB_S_OK)
+        return hr;
+    if (!fp->convert && fp->post)
+    {
+        // one launch: the step word's flags say which steps run, each in texconv's order on the previous one's stored result
+        const uint32_t sw = fp->channels ? fp->cp.steps & (0xFFFFu | DXB_CH_SWIZZLE) : 0u;
+        fp->cp = fp->pp;
+        fp->cp.steps = (fp->pp.steps & ~0xFFFFu) | sw;
+        fp->channels = true; fp->post = false;
+    }
+    // without a Convert, GenerateMipMaps meets a chain whose level 0 is that image: its pixels and format are checked there
+    for (size_t i = 0; i < items && levels && !fp->convert; ++i) chain[i * levels] = fp->level0[i];
+    if ((hr = plan_chain_steps(items, levels, filter, steps, &fp->chain)) != DXB_S_OK) return hr;
+    for (size_t i = 0; i < items && levels; ++i) chain[i * levels] = dst[i * levels];
+    fp->chain.compressed = false;
+    return alphaAllOpaque ? plan_alpha_opaque(dst, items * levels, alphaAllOpaque, ap) : DXB_S_OK;
 }
 
 } // namespace

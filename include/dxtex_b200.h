@@ -227,6 +227,35 @@ DXB200_API int32_t  dxb200_mipmaps_compress_from_channels(const dxb200_image* ba
                                                           const dxb200_chain_steps* steps, uint32_t dstFormat, uint32_t flags,
                                                           float threshold, float alphaWeight, const dxb200_image* dst,
                                                           int32_t* alphaAllOpaque);
+/* texconv's path to an uncompressed target (-f R16G16B16A16_FLOAT, B8G8R8A8_UNORM, R8G8_SNORM, ...; Texconv/texconv.cpp:2316-3560)
+ * in one call: base, source, channels, levels, filter, steps and alphaAllOpaque mean what they mean for
+ * dxb200_mipmaps_compress_from_channels; dst[i * levels + l] = level l of item i in dstFormat, laid out as
+ * ScratchImage::Initialize2D(dstFormat, W, H, items, levels) would; convertFilter and threshold are dxb200_convert's filter and
+ * threshold.  Results are identical to this sequence of calls, each run only when it does something:
+ *   1. dxb200_decompress of a BC base (when source != NULL), to the format dxb200_mipmaps_compress_from_channels picks;
+ *   2. dxb200_resize, when the size changes;
+ *   3. dxb200_apply_channel_steps with the swizzle and masks of channels, when they are enabled;
+ *   4. dxb200_convert to dstFormat with convertFilter and threshold, when level 0's format differs from dstFormat (texconv tests
+ *      info.format != tformat, :3100-3132);
+ *   5. dxb200_apply_channel_steps with the colour key, invert Y and reconstruct Z of channels, now in dstFormat, when enabled;
+ *   6. dxb200_generate_mipmaps of dst;
+ *   7. dxb200_scale_mipmaps_alpha_for_coverage per item, when steps->alphaReference > 0;
+ *   8. dxb200_premultiply_alpha of every level, when steps->premultiply;
+ *   9. dxb200_is_alpha_all_opaque of dst, when alphaAllOpaque != NULL.
+ * Every argument is checked before anything is uploaded, and a failing call returns the HRESULT of the first of those calls that
+ * would fail, each checked on the format and size the image has at that point.  dst is met first by the Convert (its level 0:
+ * another format -> E_INVALIDARG, another size -> E_FAIL), then by GenerateMipMaps (every level).  Without a Convert, dst's level 0
+ * must have level 0's format and size (E_INVALIDARG) and non-NULL pixels (E_POINTER), the later channel steps are checked from
+ * level 0 (the base itself when no front step runs) into dst's level 0, and GenerateMipMaps is checked on a chain whose level 0 is
+ * that image, so a base of another format is E_INVALIDARG and NULL base pixels are E_POINTER there.  A BC dstFormat -> E_INVALIDARG
+ * (Convert's answer); a dithered store to B5G6R5, B5G5R5A1 or B4G4R4A4 -> HRESULT_E_NOT_SUPPORTED, as dxb200_convert; levels < 2
+ * -> E_INVALIDARG, GenerateMipMaps' answer, after the Convert's checks (levels == 0: the Convert is checked on dst[0]).  The intermediate images
+ * never leave device memory: the base goes up and only the finished chain (every level) comes down.  Without a Convert, steps 3
+ * and 5 run as one launch, with the same result. */
+DXB200_API int32_t  dxb200_mipmaps_convert_from(const dxb200_image* base, size_t items, const dxb200_chain_source* source,
+                                                const dxb200_channel_steps* channels, uint32_t dstFormat, uint32_t convertFilter,
+                                                float threshold, size_t levels, uint32_t filter, const dxb200_chain_steps* steps,
+                                                const dxb200_image* dst, int32_t* alphaAllOpaque);
 
 /* ScratchImage::IsAlphaAllOpaque (DirectXTexImage.cpp:800-852; IsAlphaAllOpaqueBC, DirectXTexCompress.cpp:539-621) of
  * `nimages` images of one format: *opaque = 1 when every texel inside every image has alpha >= 0.997 (uncompressed, as
