@@ -17,7 +17,7 @@ SYMBOLS = [
     "dxb200_scale_mipmaps_alpha_for_coverage", "dxb200_scale_mipmaps_alpha_for_coverage_device",
     "dxb200_is_alpha_all_opaque", "dxb200_is_alpha_all_opaque_device",
     "dxb200_apply_channel_steps", "dxb200_apply_channel_steps_device", "dxb200_mipmaps_compress_from_channels",
-    "dxb200_mipmaps_convert_from",
+    "dxb200_mipmaps_convert_from", "dxb200_levels_from",
     "dxb200_dds_encode_header", "dxb200_dds_save_memory", "dxb200_dds_get_metadata", "dxb200_dds_load_memory",
 ]
 
@@ -95,6 +95,8 @@ def _load():
                                                           C.POINTER(C.c_int32)]
     lib.dxb200_mipmaps_convert_from.argtypes = [IP, C.c_size_t, C.POINTER(ChainSource), C.POINTER(ChannelSteps), C.c_uint32, C.c_uint32,
                                                 C.c_float, C.c_size_t, C.c_uint32, C.POINTER(ChainSteps), IP, C.POINTER(C.c_int32)]
+    lib.dxb200_levels_from.argtypes = [IP, C.c_size_t, C.c_size_t, C.POINTER(ChainSource), C.POINTER(ChannelSteps), C.c_uint32, C.c_uint32,
+                                       C.c_uint32, C.c_float, C.POINTER(ChainSteps), IP, C.POINTER(C.c_int32)]
     lib.dxb200_apply_channel_steps.argtypes = [IP, C.c_size_t, C.POINTER(ChannelSteps), IP]
     lib.dxb200_apply_channel_steps_device.argtypes = [IP, C.c_size_t, C.POINTER(ChannelSteps), IP, C.c_void_p]
     lib.dxb200_is_alpha_all_opaque.argtypes = [IP, C.c_size_t, C.POINTER(C.c_int32)]
@@ -124,7 +126,7 @@ def _load():
     lib.dxb200_dds_load_memory.argtypes = [C.c_void_p, C.c_size_t, C.c_uint32, IP, C.c_size_t]
     for name in ("dxb200_dds_encode_header", "dxb200_dds_save_memory", "dxb200_dds_get_metadata", "dxb200_dds_load_memory"):
         getattr(lib, name).restype = C.c_int32
-    for name in ("dxb200_init", "dxb200_init_devices", "dxb200_initialized_devices", "dxb200_compress_ex", "dxb200_convert_ex", "dxb200_mipmaps_compress", "dxb200_mipmaps_compress_ex", "dxb200_mipmaps_compress_from", "dxb200_mipmaps_compress_from_ex", "dxb200_is_alpha_all_opaque", "dxb200_is_alpha_all_opaque_device", "dxb200_apply_channel_steps", "dxb200_apply_channel_steps_device", "dxb200_mipmaps_compress_from_channels", "dxb200_mipmaps_convert_from", "dxb200_device_count", "dxb200_compute_pitch", "dxb200_calculate_mip_levels", "dxb200_compress",
+    for name in ("dxb200_init", "dxb200_init_devices", "dxb200_initialized_devices", "dxb200_compress_ex", "dxb200_convert_ex", "dxb200_mipmaps_compress", "dxb200_mipmaps_compress_ex", "dxb200_mipmaps_compress_from", "dxb200_mipmaps_compress_from_ex", "dxb200_is_alpha_all_opaque", "dxb200_is_alpha_all_opaque_device", "dxb200_apply_channel_steps", "dxb200_apply_channel_steps_device", "dxb200_mipmaps_compress_from_channels", "dxb200_mipmaps_convert_from", "dxb200_levels_from", "dxb200_device_count", "dxb200_compute_pitch", "dxb200_calculate_mip_levels", "dxb200_compress",
                  "dxb200_compress_device", "dxb200_decompress", "dxb200_decompress_device", "dxb200_convert",
                  "dxb200_convert_device", "dxb200_generate_mipmaps", "dxb200_generate_mipmaps_device", "dxb200_resize", "dxb200_resize_device", "dxb200_premultiply_alpha", "dxb200_premultiply_alpha_device"):
         getattr(lib, name).restype = C.c_int32
@@ -304,6 +306,26 @@ def mipmaps_convert_from(bases, w, h, base_fmt, dst_fmt, source=None, channels=N
                                          filter, C.byref(steps) if steps is not None else None, d, C.byref(opaque))
     if hr != 0:
         raise DxTexError(hr, "dxb200_mipmaps_convert_from")
+    return outs, opaque.value == 1
+
+
+def levels_from(bases, sizes, base_fmt, dst_fmt, source=None, channels=None, convert_filter=0, compress_flags=0, threshold=0.5,
+                steps=None):
+    """dxb200_levels_from of items that keep their own levels: bases[i][l] = level l of item i (host, tight, of base_fmt, BC or
+    not), (w, h) = sizes[l] for every item; the ChainSource `source`, the ChannelSteps `channels` and the ChainSteps `steps`
+    (None: none).  Returns (outs[i][l] = that level in dst_fmt, tight; IsAlphaAllOpaque of the output as a bool)."""
+    levels = len(sizes)
+    osizes = [(source.width, source.height)] if levels == 1 and source is not None and source.width else list(sizes)
+    bases = [[np.ascontiguousarray(a).view(np.uint8).reshape(-1) for a in item] for item in bases]
+    outs = [[np.zeros(F.compute_pitch(dst_fmt, w, h)[1], np.uint8) for (w, h) in osizes] for _ in bases]
+    s = images([make_image(_np_ptr(a), w, h, base_fmt) for item in bases for a, (w, h) in zip(item, sizes)])
+    d = images([make_image(_np_ptr(o), w, h, dst_fmt) for item in outs for o, (w, h) in zip(item, osizes)])
+    opaque = C.c_int32(-1)
+    hr = lib.dxb200_levels_from(s, len(bases), levels, C.byref(source) if source is not None else None,
+                                C.byref(channels) if channels is not None else None, dst_fmt, convert_filter, compress_flags, threshold,
+                                C.byref(steps) if steps is not None else None, d, C.byref(opaque))
+    if hr != 0:
+        raise DxTexError(hr, "dxb200_levels_from")
     return outs, opaque.value == 1
 
 

@@ -690,23 +690,30 @@ struct ResultWords
 // later channel steps (fp.post) run in place there.  When no step writes that level 0 (no front step, no Convert), the uploaded
 // base is copied into it device to device.  With a scan (words != nullptr: one result word per item, see
 // dxb200_mipmaps_compress_from_ex) one more plane holds the items' words; they are cleared, set by one scan launch over all the
-// chunk's output after its last step, and come back with it.
+// chunk's output after its last step, and come back with it.  Items that keep their own levels (cp.generate == false, levels_from)
+// stage the same planes with every level where the others hold level 0: every level of the base goes up, the front, channel and
+// Convert steps run on all of them, and no mip or coverage launch runs.  Each step is one launch per chunk over all its levels:
+// the kernels take mixed-size batches through the job tables.  That keeps a premultiply or a Convert off its vector kernel, which
+// needs equal jobs, yet per-level launches measured no faster (DESIGN.md §4).  A BC base that passes through is copied into dst like an
+// uncompressed one, row of blocks by row of blocks.
 int32_t run_chains(const dxb200_image* base, size_t items, size_t levels, uint32_t filter, const FromPlan& fp, const dxb200_image* dst,
                    const AlphaOpaquePlan& scan, const ResultWords* words)
 {
     const ChainPlan& cp = fp.chain;
     const bool front = fp.decompress || fp.resize, mid = fp.decompress && fp.resize, pre = front && fp.convert;
     const bool up = !front && cp.compressed;                   // the chain's level 0 is uploaded; otherwise the base is
+    const size_t per = cp.generate ? 1 : levels;               // images per item that the steps in front of the mips act on
+    const Copy chainUp = up ? Copy::Up : Copy::None;
     const std::vector<dxb200_image> wimg = words ? words->images() : std::vector<dxb200_image>();
     return run_sharded(items, [&](size_t i) { return cp.chain[i * levels].slicePitch; },
         [&](size_t lo, size_t hi)
         {
             std::vector<Plane> planes;
-            if (!up) planes.push_back({ base + lo, 1, Copy::Up, Copy::Up });
-            if (mid) planes.push_back({ fp.decompressed.data() + lo, 1, Copy::None, Copy::None });
-            if (pre) planes.push_back({ fp.level0.data() + lo, 1, Copy::None, Copy::None });
+            if (!up) planes.push_back({ base + lo * per, per, Copy::Up, Copy::Up });
+            if (mid) planes.push_back({ fp.decompressed.data() + lo * per, per, Copy::None, Copy::None });
+            if (pre) planes.push_back({ fp.level0.data() + lo * per, per, Copy::None, Copy::None });
             const size_t pc = planes.size();                    // the chains' plane, then the blocks' and the words'
-            if (cp.compressed) planes.push_back({ cp.chain.data() + lo * levels, levels, up ? Copy::Up : Copy::None, Copy::None });
+            if (cp.compressed) planes.push_back({ cp.chain.data() + lo * levels, levels, chainUp, cp.generate ? Copy::None : chainUp });
             planes.push_back({ dst + lo * levels, levels, Copy::Down, Copy::Down });
             if (words) planes.push_back({ wimg.data() + lo, 1, Copy::Down, Copy::Down });
             return run_staged(planes.data(), planes.size(), hi - lo, ITEM_CHUNK,
@@ -717,27 +724,33 @@ int32_t run_chains(const dxb200_image* base, size_t items, size_t levels, uint32
                     const dxb200_image* chains = dev[pc].data();
                     const dxb200_image* out = dev[cp.compressed ? pc + 1 : pc].data();
                     int32_t h2 = DXB_S_OK;
-                    std::vector<dxb200_image> level(cnt);
-                    for (size_t it = 0; it < cnt; ++it) level[it] = chains[it * levels];
+                    const size_t m = cnt * per;
+                    std::vector<dxb200_image> level(m);
+                    for (size_t k = 0; k < m; ++k) level[k] = chains[k / per * levels + k % per];
                     // the image the front steps write and the channel steps (the swizzle, with a Convert) run on
                     const dxb200_image* first = pre ? dev[pc - 1].data() : fp.convert && !front ? src : level.data();
-                    if (fp.decompress) h2 = launch_decompress(fp.dp, src, mid ? decompressed : first, cnt, st);
-                    if (h2 == DXB_S_OK && fp.resize) h2 = launch_resize(mid ? decompressed : src, first, cnt, fp.resizeFilter, fp.resizeMode, st);
-                    for (size_t it = 0; it < cnt && h2 == DXB_S_OK && !up && !front && !fp.convert; ++it)
-                        h2 = cuda_hr(cudaMemcpy2DAsync(level[it].pixels, level[it].rowPitch, src[it].pixels, src[it].rowPitch,
-                                                       level[it].width * dxb_bytes_per_pixel(level[it].format), level[it].height,
-                                                       cudaMemcpyDeviceToDevice, st), "base -> level 0");
-                    if (h2 == DXB_S_OK && fp.channels) h2 = launch_channel_steps(fp.cp, first, first, cnt, st);
-                    if (h2 == DXB_S_OK && fp.convert) h2 = launch_convert(fp.cv, first, level.data(), cnt, st);
-                    if (h2 == DXB_S_OK && fp.post) h2 = launch_channel_steps(fp.pp, level.data(), level.data(), cnt, st);
-                    if (h2 == DXB_S_OK) h2 = launch_mips(chains, cnt, levels, filter, cp.mode, st);
-                    if (h2 == DXB_S_OK && cp.coverage) h2 = launch_coverage(chains, chains, cnt, levels, cp.ref, st);
-                    // one launch per level: the chunk's images of a level are equal, as the separate calls' images are, so they take the
-                    // same premultiply kernel
-                    for (size_t l = 0; l < levels && h2 == DXB_S_OK && cp.premultiply; ++l)
+                    if (fp.decompress) h2 = launch_decompress(fp.dp, src, mid ? decompressed : first, m, st);
+                    if (h2 == DXB_S_OK && fp.resize) h2 = launch_resize(mid ? decompressed : src, first, m, fp.resizeFilter, fp.resizeMode, st);
+                    for (size_t k = 0; k < m && h2 == DXB_S_OK && !up && !front && !fp.convert; ++k)
                     {
-                        for (size_t it = 0; it < cnt; ++it) level[it] = chains[it * levels + l];
-                        h2 = launch_pmalpha(cp.pm, level.data(), level.data(), cnt, st);
+                        // the planned formats are implemented ones, so compute_pitch succeeds; rows of pixels or of blocks
+                        size_t row = 0, slice = 0;
+                        (void)compute_pitch(level[k].format, level[k].width, level[k].height, &row, &slice);
+                        const size_t rows = is_compressed(level[k].format) ? std::max<size_t>(1, (level[k].height + 3) / 4) : level[k].height;
+                        h2 = cuda_hr(cudaMemcpy2DAsync(level[k].pixels, level[k].rowPitch, src[k].pixels, src[k].rowPitch, row, rows,
+                                                       cudaMemcpyDeviceToDevice, st), "base -> level 0");
+                    }
+                    if (h2 == DXB_S_OK && fp.channels) h2 = launch_channel_steps(fp.cp, first, first, m, st);
+                    if (h2 == DXB_S_OK && fp.convert) h2 = launch_convert(fp.cv, first, level.data(), m, st);
+                    if (h2 == DXB_S_OK && fp.post) h2 = launch_channel_steps(fp.pp, level.data(), level.data(), m, st);
+                    if (h2 == DXB_S_OK && cp.generate) h2 = launch_mips(chains, cnt, levels, filter, cp.mode, st);
+                    if (h2 == DXB_S_OK && cp.coverage) h2 = launch_coverage(chains, chains, cnt, levels, cp.ref, st);
+                    // a generated chain premultiplies one launch per level: the chunk's images of a level are equal, as the separate
+                    // calls' images are, so they take the same premultiply kernel; kept levels already sit in `level`, one launch
+                    for (size_t l = 0; l < levels / per && h2 == DXB_S_OK && cp.premultiply; ++l)
+                    {
+                        for (size_t it = 0; it < cnt && cp.generate; ++it) level[it] = chains[it * levels + l];
+                        h2 = launch_pmalpha(cp.pm, level.data(), level.data(), m, st);
                     }
                     if (h2 == DXB_S_OK && cp.compressed) h2 = launch_compress(cp.compress, chains, out, cnt * levels, st);
                     if (h2 == DXB_S_OK && words)
@@ -1055,6 +1068,23 @@ int32_t dxb200_mipmaps_convert_from(const dxb200_image* base, size_t items, cons
     ResultWords words;
     if (ap.scan && (hr = words.alloc(items)) != DXB_S_OK) return hr;
     hr = run_chains(base, items, levels, filter, fp, dst, ap, ap.scan ? &words : nullptr);
+    if (hr == DXB_S_OK && alphaAllOpaque) *alphaAllOpaque = (!ap.scan || words.all_zero()) ? 1 : 0;
+    return hr;
+}
+
+// ---- texconv on items that keep their own levels: every level stays in device memory until it is done (run_chains) -------------
+int32_t dxb200_levels_from(const dxb200_image* base, size_t items, size_t levels, const dxb200_chain_source* source,
+                           const dxb200_channel_steps* channels, uint32_t dstFormat, uint32_t convertFilter, uint32_t compressFlags,
+                           float threshold, const dxb200_chain_steps* steps, const dxb200_image* dst, int32_t* alphaAllOpaque)
+{
+    FromPlan fp;
+    AlphaOpaquePlan ap;
+    int32_t hr = plan_levels_from(base, items, levels, source, channels, dstFormat, convertFilter, compressFlags, threshold, steps, dst,
+                                  alphaAllOpaque, &fp, &ap);
+    if (hr != DXB_S_OK) return hr;
+    ResultWords words;
+    if (ap.scan && (hr = words.alloc(items)) != DXB_S_OK) return hr;
+    hr = run_chains(base, items, levels, 0, fp, dst, ap, ap.scan ? &words : nullptr);
     if (hr == DXB_S_OK && alphaAllOpaque) *alphaAllOpaque = (!ap.scan || words.all_zero()) ? 1 : 0;
     return hr;
 }

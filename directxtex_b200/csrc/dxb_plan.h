@@ -342,23 +342,24 @@ int32_t plan_coverage_jobs(const dxb200_image* chains, const dxb200_image* out, 
 // ---- GenerateMipMaps -> ScaleMipMapsAlphaForCoverage -> PremultiplyAlpha -> [Compress] in one call (mipmaps_compress) ------------
 // chain = the chain every item will have on the device: for a compressed output, the ScratchImage layout of the source format (level
 // 0 at the caller's pitch, its pixels the upload source; the other levels carry base[i].pixels only for validation); for an
-// uncompressed output (compressed == false), the caller's dst itself.
+// uncompressed output (compressed == false), the caller's dst itself.  generate == false (levels_from): the items keep the levels
+// they came with, so GenerateMipMaps and coverage do not run and every level goes through the steps in front of them.
 struct ChainPlan
 {
     std::vector<dxb200_image> chain;
-    uint32_t mode;
+    bool generate = true; uint32_t mode;
     bool coverage; float ref;
     bool premultiply; dxb_convert_params pm;
     bool compressed; CompressPlan compress;
 };
 
-// GenerateMipMaps, then the optional coverage and premultiply steps of `steps`, on cp->chain, with the HRESULT of the first of those
-// calls that would fail
+// GenerateMipMaps (when cp->generate), then the optional coverage and premultiply steps of `steps`, on cp->chain, with the HRESULT
+// of the first of those calls that would fail
 int32_t plan_chain_steps(size_t items, size_t levels, uint32_t filter, const dxb200_chain_steps* steps, ChainPlan* cp)
 {
     const dxb200_image* chain = cp->chain.data();
-    int32_t hr = plan_mips(chain, items, levels, filter, &cp->mode);
-    if (hr != DXB_S_OK) return hr;
+    int32_t hr = DXB_S_OK;
+    if (cp->generate && (hr = plan_mips(chain, items, levels, filter, &cp->mode)) != DXB_S_OK) return hr;
     cp->ref = steps ? steps->alphaReference : 0.0f;
     cp->coverage = cp->ref > 0.0f;                                                      // texconv -keepcoverage (:3304)
     if (cp->coverage && (hr = plan_alpha_coverage(chain, items * levels, chain)) != DXB_S_OK) return hr;
@@ -594,6 +595,60 @@ dxb_convert_params alpha_opaque_pixel_params(const AlphaOpaquePlan& ap, uint32_t
     return P;
 }
 
+// ---- the channel steps around a Convert ------------------------------------------------------------------------------------------
+// texconv runs the swizzle and masks of `channels` before its Convert (:2645-2694) and the colour key, invert Y and reconstruct Z
+// after it (:3134-3300); nothing enabled in either when channels == nullptr
+void split_channel_steps(const dxb200_channel_steps* channels, dxb200_channel_steps* swizzle, dxb200_channel_steps* later)
+{
+    *swizzle = { { 0, 1, 2, 3 }, 0, 0, 0, 0, 0, 0 };
+    *later = *swizzle;
+    if (!channels) return;
+    memcpy(swizzle->swizzle, channels->swizzle, 4); swizzle->zeroMask = channels->zeroMask; swizzle->oneMask = channels->oneMask;
+    later->colorKey = channels->colorKey; later->colorKeyValue = channels->colorKeyValue;
+    later->invertY = channels->invertY; later->reconstructZ = channels->reconstructZ;
+}
+
+// Without a Convert, out[i] takes the working image work[i] as it is: the same format and size (E_INVALIDARG, as a BC row pitch the
+// kernels cannot read), and pixels (E_POINTER)
+int32_t plan_unconverted(const dxb200_image* work, size_t n, const dxb200_image* out)
+{
+    for (size_t i = 0; i < n; ++i)
+    {
+        if (out[i].format != work[0].format || out[i].width != work[i].width || out[i].height != work[i].height || !bc_pitch_ok(out[i]))
+            return DXB_E_INVALIDARG;
+        if (!out[i].pixels) return DXB_E_POINTER;
+    }
+    return DXB_S_OK;
+}
+
+// The images levels_from only copies into dst (no step reads them, or only the channel steps, which check neither size nor
+// bounds): one format this library implements (E_NOT_SUPPORTED otherwise, as every other call answers, since its pitch is
+// unknown), non-NULL pixels (E_POINTER), a size of 1 to 2^32 - 1 in both directions and a BC row pitch of whole blocks
+// (E_INVALIDARG)
+int32_t plan_copy(const dxb200_image* src, size_t n)
+{
+    const uint32_t fmt = src[0].format;
+    if (!is_compressed(fmt) && !is_supported_pixel_format(fmt)) return DXB_E_NOT_SUPPORTED;
+    for (size_t i = 0; i < n; ++i)
+    {
+        if (src[i].format != fmt) return DXB_E_INVALIDARG;
+        if (!src[i].pixels) return DXB_E_POINTER;
+        if (!src[i].width || !src[i].height || src[i].width > 0xFFFFFFFFull || src[i].height > 0xFFFFFFFFull || !bc_pitch_ok(src[i]))
+            return DXB_E_INVALIDARG;
+    }
+    return DXB_S_OK;
+}
+
+// Without a Convert between them, the swizzle (fp->cp, when fp->channels) and the later steps (fp->pp) run as one launch: the step
+// word's flags say which steps run, each in texconv's order on the previous one's stored result
+void merge_channel_launches(FromPlan* fp)
+{
+    const uint32_t sw = fp->channels ? fp->cp.steps & (0xFFFFu | DXB_CH_SWIZZLE) : 0u;
+    fp->cp = fp->pp;
+    fp->cp.steps = (fp->pp.steps & ~0xFFFFu) | sw;
+    fp->channels = true; fp->post = false;
+}
+
 // ---- Decompress -> Resize -> swizzle -> Convert -> later channel steps -> mips -> coverage -> premultiply in one call --------------
 // (mipmaps_convert_from) texconv's path to an uncompressed target (Texconv/texconv.cpp:2316-3560).  Every check of the nine
 // separate calls before anything is uploaded, each with the HRESULT of the first that would fail: plan_front; the swizzle and
@@ -613,13 +668,8 @@ int32_t plan_mipmaps_convert_from(const dxb200_image* base, size_t items, const 
     if (!base || !items) return DXB_E_INVALIDARG;
     int32_t hr = plan_front(base, items, source, channels, fp);
     if (hr != DXB_S_OK) return hr;
-    dxb200_channel_steps swizzle = { { 0, 1, 2, 3 }, 0, 0, 0, 0, 0, 0 }, later = swizzle;        // nothing enabled
-    if (channels)
-    {
-        memcpy(swizzle.swizzle, channels->swizzle, 4); swizzle.zeroMask = channels->zeroMask; swizzle.oneMask = channels->oneMask;
-        later.colorKey = channels->colorKey; later.colorKeyValue = channels->colorKeyValue;
-        later.invertY = channels->invertY; later.reconstructZ = channels->reconstructZ;
-    }
+    dxb200_channel_steps swizzle, later;
+    split_channel_steps(channels, &swizzle, &later);
     fp->channels = channel_steps_word(swizzle) != 0;
     if (fp->channels && (hr = plan_channel_steps(fp->level0.data(), items, &swizzle, fp->level0.data(), &fp->cp)) != DXB_S_OK) return hr;
     if (!dst) return DXB_E_INVALIDARG;
@@ -633,30 +683,82 @@ int32_t plan_mipmaps_convert_from(const dxb200_image* base, size_t items, const 
         if ((hr = plan_convert(fp->level0.data(), items, dstFormat, convertFilter, out0.data(), &fp->cv)) != DXB_S_OK) return hr;
         fp->cv.threshold = threshold;
     }
-    else
-        for (size_t i = 0; i < items; ++i)
-        {
-            if (out0[i].format != dstFormat || out0[i].width != fp->level0[i].width || out0[i].height != fp->level0[i].height) return DXB_E_INVALIDARG;
-            if (!out0[i].pixels) return DXB_E_POINTER;
-        }
+    else if ((hr = plan_unconverted(fp->level0.data(), items, out0.data())) != DXB_S_OK)
+        return hr;
     // without a Convert the later steps read level 0 as the front steps leave it (the base when none runs) and write dst's level 0
     fp->post = channel_steps_word(later) != 0;
     if (fp->post && (hr = plan_channel_steps(fp->convert ? out0.data() : fp->level0.data(), items, &later, out0.data(), &fp->pp)) != DXB_S_OK)
         return hr;
-    if (!fp->convert && fp->post)
-    {
-        // one launch: the step word's flags say which steps run, each in texconv's order on the previous one's stored result
-        const uint32_t sw = fp->channels ? fp->cp.steps & (0xFFFFu | DXB_CH_SWIZZLE) : 0u;
-        fp->cp = fp->pp;
-        fp->cp.steps = (fp->pp.steps & ~0xFFFFu) | sw;
-        fp->channels = true; fp->post = false;
-    }
+    if (!fp->convert && fp->post) merge_channel_launches(fp);
     // without a Convert, GenerateMipMaps meets a chain whose level 0 is that image: its pixels and format are checked there
     for (size_t i = 0; i < items && levels && !fp->convert; ++i) chain[i * levels] = fp->level0[i];
     if ((hr = plan_chain_steps(items, levels, filter, steps, &fp->chain)) != DXB_S_OK) return hr;
     for (size_t i = 0; i < items && levels; ++i) chain[i * levels] = dst[i * levels];
     fp->chain.compressed = false;
     return alphaAllOpaque ? plan_alpha_opaque(dst, items * levels, alphaAllOpaque, ap) : DXB_S_OK;
+}
+
+// ---- texconv on items that keep their own levels (levels_from): Decompress -> [Resize] -> swizzle -> Convert -> later channel steps
+// -> premultiply -> Compress -> IsAlphaAllOpaque, each over the items * levels images as one array ---------------------------------
+// texconv keeps the input's chain when -m is not given (Texconv/texconv.cpp:2270) and makes none for -m 1, so neither the strip
+// (:3325) nor GenerateMipMaps (:3419) runs.  The call's own rules come first: levels == 0, a Resize with levels > 1 (texconv's Resize
+// drops the chain) and alphaReference > 0 (-keepcoverage regenerates the chain, :3325) are E_INVALIDARG.  Then every check of the
+// separate calls in their order, each on the format and size the images have at that point: plan_front on all the images (a BC base
+// is decompressed whatever the source); the swizzle and masks in place; Convert into dst for an uncompressed dstFormat other than the
+// working format (texconv's test, :3098), else dst must be the working images (plan_unconverted); the later channel steps;
+// premultiply (plan_chain_steps with generate off); Compress into dst for a BC dstFormat; IsAlphaAllOpaque of dst.  A BC base whose
+// dstFormat is its own format, with no channel step, no premultiply and no Resize, passes through (texconv :3621): its Decompress is
+// checked, as texconv makes it before it decides, but does not run; dst takes the base's bytes.  When the base is copied into dst
+// (no front step, no Convert, no Compress), plan_copy checks it last.
+int32_t plan_levels_from(const dxb200_image* base, size_t items, size_t levels, const dxb200_chain_source* source,
+                         const dxb200_channel_steps* channels, uint32_t dstFormat, uint32_t convertFilter, uint32_t compressFlags,
+                         float threshold, const dxb200_chain_steps* steps, const dxb200_image* dst, const int32_t* alphaAllOpaque,
+                         FromPlan* fp, AlphaOpaquePlan* ap)
+{
+    ap->scan = ap->blocks = false; ap->format = 0;
+    if (!base || !items || !levels) return DXB_E_INVALIDARG;
+    const size_t n = items * levels;
+    const dxb200_chain_source keep = { 0, 0, 0, 0 };
+    const dxb200_chain_source* src = source ? source : &keep;
+    if (levels > 1 && ((src->width && src->width != base[0].width) || (src->height && src->height != base[0].height))) return DXB_E_INVALIDARG;
+    if (steps && steps->alphaReference > 0.0f) return DXB_E_INVALIDARG;
+    int32_t hr = plan_front(base, n, src, channels, fp);
+    if (hr != DXB_S_OK) return hr;
+    ChainPlan& cp = fp->chain;
+    cp.generate = false; cp.mode = 0;
+    dxb200_channel_steps swizzle, later;
+    split_channel_steps(channels, &swizzle, &later);
+    const bool pass = is_compressed(base[0].format) && dstFormat == base[0].format && !channel_steps_word(swizzle) && !channel_steps_word(later)
+                      && !(steps && steps->premultiply) && !fp->resize;
+    if (pass)
+    {
+        fp->decompress = false;
+        fp->decompressed.clear();
+        fp->level0.assign(base, base + n);
+    }
+    fp->channels = channel_steps_word(swizzle) != 0;
+    if (fp->channels && (hr = plan_channel_steps(fp->level0.data(), n, &swizzle, fp->level0.data(), &fp->cp)) != DXB_S_OK) return hr;
+    // a compressed output is compressed from the working images, so the later steps and premultiply run in place on them
+    cp.compressed = is_compressed(dstFormat) && !pass;
+    if (!cp.compressed && !dst) return DXB_E_INVALIDARG;
+    const dxb200_image* out = cp.compressed ? fp->level0.data() : dst;
+    fp->convert = !is_compressed(dstFormat) && fp->level0[0].format != dstFormat;
+    if (fp->convert)
+    {
+        if ((hr = plan_convert(fp->level0.data(), n, dstFormat, convertFilter, dst, &fp->cv)) != DXB_S_OK) return hr;
+        fp->cv.threshold = threshold;
+    }
+    else if (!cp.compressed && (hr = plan_unconverted(fp->level0.data(), n, out)) != DXB_S_OK)
+        return hr;
+    fp->post = channel_steps_word(later) != 0;
+    if (fp->post && (hr = plan_channel_steps(fp->convert ? out : fp->level0.data(), n, &later, out, &fp->pp)) != DXB_S_OK) return hr;
+    if (!fp->convert && fp->post) merge_channel_launches(fp);
+    cp.chain.assign(out, out + n);
+    if ((hr = plan_chain_steps(items, levels, 0, steps, &cp)) != DXB_S_OK) return hr;
+    if (cp.compressed && (hr = plan_compress(out, n, dstFormat, compressFlags, threshold, dst, &cp.compress)) != DXB_S_OK) return hr;
+    const bool copy = !fp->decompress && !fp->resize && !fp->convert && !cp.compressed;
+    if (copy && (hr = plan_copy(base, n)) != DXB_S_OK) return hr;
+    return alphaAllOpaque ? plan_alpha_opaque(dst, n, alphaAllOpaque, ap) : DXB_S_OK;
 }
 
 } // namespace

@@ -256,6 +256,41 @@ DXB200_API int32_t  dxb200_mipmaps_convert_from(const dxb200_image* base, size_t
                                                 const dxb200_channel_steps* channels, uint32_t dstFormat, uint32_t convertFilter,
                                                 float threshold, size_t levels, uint32_t filter, const dxb200_chain_steps* steps,
                                                 const dxb200_image* dst, int32_t* alphaAllOpaque);
+/* texconv on textures that keep their own mip levels (no -m on an input with mips, Texconv/texconv.cpp:2270, or -m 1) in one call:
+ * base[i * levels + l] = level l of item i as loaded (host), BC or uncompressed, every image of base[0]'s format; level sizes need
+ * not halve.  dst[i * levels + l] = the same level of the result, laid out as ScratchImage::Initialize2D(dstFormat, W, H, items,
+ * levels) would, each of its base's size (or the resized size when levels == 1).  source and channels mean what they mean for
+ * dxb200_mipmaps_convert_from, convertFilter is dxb200_convert's filter, compressFlags dxb200_compress's flags and threshold both
+ * calls' threshold.  Results are identical to this sequence of calls, each over all items * levels images as one array and each
+ * run only when it does something:
+ *   1. dxb200_decompress of a BC base, to source->decompressFormat (source == NULL or 0: the format
+ *      dxb200_mipmaps_compress_from_channels picks);
+ *   2. dxb200_resize to source->width x height with source->resizeFilter, only when levels == 1;
+ *   3. dxb200_apply_channel_steps with the swizzle and masks of channels;
+ *   4. dxb200_convert to dstFormat with convertFilter and threshold, for an uncompressed dstFormat other than the working format
+ *      (texconv :3098);
+ *   5. dxb200_apply_channel_steps with the colour key, invert Y and reconstruct Z of channels;
+ *   6. dxb200_premultiply_alpha, when steps->premultiply;
+ *   7. dxb200_compress into dst with compressFlags and threshold, for a BC dstFormat;
+ *   8. dxb200_is_alpha_all_opaque of dst, when alphaAllOpaque != NULL.
+ * A BC base whose dstFormat is exactly its own format (BC1_UNORM -> BC1_UNORM_SRGB re-encodes), with no channel step, no
+ * premultiply and no resize, passes through as texconv passes it (:3621): dst takes the base's blocks and no decompress or
+ * compress kernel runs (the Decompress is still checked, as texconv makes it first); an uncompressed base already in dstFormat
+ * with nothing enabled is copied the same way.  Every argument is checked before anything is uploaded.  levels == 0, a size in
+ * source that differs from the base's with levels > 1 (texconv's Resize drops the chain and regenerates it, which
+ * dxb200_mipmaps_convert_from and dxb200_mipmaps_compress_from_channels do) and steps->alphaReference > 0 (-keepcoverage also
+ * regenerates it) -> E_INVALIDARG, in that order; then a failing call returns the HRESULT of the first of the calls above that
+ * would fail, each checked on the format and size every image has at that point.  Without a Convert, an uncompressed dst (or a
+ * passed-through one) must have the working format and size, and a row pitch of whole blocks (E_INVALIDARG), and pixels
+ * (E_POINTER).  A base that is only copied into dst (no decompress, resize, Convert or Compress) is checked last: a format this
+ * library does not implement (R8G8B8A8_UINT, R16_UINT, ...) -> HRESULT_E_NOT_SUPPORTED, as every other call answers it; images of
+ * other formats, a zero or over-32-bit width or height, or a BC row pitch of part blocks -> E_INVALIDARG; NULL pixels -> E_POINTER.
+ * Steps 3 and 5 run as one launch when no Convert sits between them.  The base goes up once, every level of it;
+ * only dst comes down. */
+DXB200_API int32_t  dxb200_levels_from(const dxb200_image* base, size_t items, size_t levels, const dxb200_chain_source* source,
+                                       const dxb200_channel_steps* channels, uint32_t dstFormat, uint32_t convertFilter,
+                                       uint32_t compressFlags, float threshold, const dxb200_chain_steps* steps, const dxb200_image* dst,
+                                       int32_t* alphaAllOpaque);
 
 /* ScratchImage::IsAlphaAllOpaque (DirectXTexImage.cpp:800-852; IsAlphaAllOpaqueBC, DirectXTexCompress.cpp:539-621) of
  * `nimages` images of one format: *opaque = 1 when every texel inside every image has alpha >= 0.997 (uncompressed, as
