@@ -18,6 +18,7 @@ SYMBOLS = [
     "dxb200_is_alpha_all_opaque", "dxb200_is_alpha_all_opaque_device",
     "dxb200_apply_channel_steps", "dxb200_apply_channel_steps_device", "dxb200_mipmaps_compress_from_channels",
     "dxb200_mipmaps_convert_from", "dxb200_levels_from",
+    "dxb200_mipmaps_compress_from_channels_ex", "dxb200_mipmaps_convert_from_ex", "dxb200_levels_from_ex",
     "dxb200_dds_encode_header", "dxb200_dds_save_memory", "dxb200_dds_get_metadata", "dxb200_dds_load_memory",
 ]
 
@@ -48,6 +49,11 @@ class ChannelSteps(C.Structure):
     """dxb200_channel_steps: texconv's swizzle, colour key, invert-Y and reconstruct-Z steps."""
     _fields_ = [("swizzle", C.c_uint8 * 4), ("zeroMask", C.c_uint8), ("oneMask", C.c_uint8), ("colorKey", C.c_uint8),
                 ("invertY", C.c_uint8), ("reconstructZ", C.c_uint8), ("colorKeyValue", C.c_uint32)]
+
+
+class TexconvSteps(C.Structure):
+    """dxb200_texconv_steps: texconv's -alpha (demultiply) and -f BC3n / RXGB (bc3Layout 1 / 2) steps."""
+    _fields_ = [("demultiply", C.c_uint32), ("demultiplyFlags", C.c_uint32), ("bc3Layout", C.c_uint32)]
 
 
 STATUS_FN = C.CFUNCTYPE(C.c_int, C.c_size_t, C.c_size_t, C.c_void_p)      # dxb200_status_fn
@@ -97,6 +103,10 @@ def _load():
                                                 C.c_float, C.c_size_t, C.c_uint32, C.POINTER(ChainSteps), IP, C.POINTER(C.c_int32)]
     lib.dxb200_levels_from.argtypes = [IP, C.c_size_t, C.c_size_t, C.POINTER(ChainSource), C.POINTER(ChannelSteps), C.c_uint32, C.c_uint32,
                                        C.c_uint32, C.c_float, C.POINTER(ChainSteps), IP, C.POINTER(C.c_int32)]
+    TP = C.POINTER(TexconvSteps)
+    lib.dxb200_mipmaps_compress_from_channels_ex.argtypes = lib.dxb200_mipmaps_compress_from_channels.argtypes + [TP]
+    lib.dxb200_mipmaps_convert_from_ex.argtypes = lib.dxb200_mipmaps_convert_from.argtypes + [TP]
+    lib.dxb200_levels_from_ex.argtypes = lib.dxb200_levels_from.argtypes + [TP]
     lib.dxb200_apply_channel_steps.argtypes = [IP, C.c_size_t, C.POINTER(ChannelSteps), IP]
     lib.dxb200_apply_channel_steps_device.argtypes = [IP, C.c_size_t, C.POINTER(ChannelSteps), IP, C.c_void_p]
     lib.dxb200_is_alpha_all_opaque.argtypes = [IP, C.c_size_t, C.POINTER(C.c_int32)]
@@ -126,7 +136,7 @@ def _load():
     lib.dxb200_dds_load_memory.argtypes = [C.c_void_p, C.c_size_t, C.c_uint32, IP, C.c_size_t]
     for name in ("dxb200_dds_encode_header", "dxb200_dds_save_memory", "dxb200_dds_get_metadata", "dxb200_dds_load_memory"):
         getattr(lib, name).restype = C.c_int32
-    for name in ("dxb200_init", "dxb200_init_devices", "dxb200_initialized_devices", "dxb200_compress_ex", "dxb200_convert_ex", "dxb200_mipmaps_compress", "dxb200_mipmaps_compress_ex", "dxb200_mipmaps_compress_from", "dxb200_mipmaps_compress_from_ex", "dxb200_is_alpha_all_opaque", "dxb200_is_alpha_all_opaque_device", "dxb200_apply_channel_steps", "dxb200_apply_channel_steps_device", "dxb200_mipmaps_compress_from_channels", "dxb200_mipmaps_convert_from", "dxb200_levels_from", "dxb200_device_count", "dxb200_compute_pitch", "dxb200_calculate_mip_levels", "dxb200_compress",
+    for name in ("dxb200_init", "dxb200_init_devices", "dxb200_initialized_devices", "dxb200_compress_ex", "dxb200_convert_ex", "dxb200_mipmaps_compress", "dxb200_mipmaps_compress_ex", "dxb200_mipmaps_compress_from", "dxb200_mipmaps_compress_from_ex", "dxb200_is_alpha_all_opaque", "dxb200_is_alpha_all_opaque_device", "dxb200_apply_channel_steps", "dxb200_apply_channel_steps_device", "dxb200_mipmaps_compress_from_channels", "dxb200_mipmaps_convert_from", "dxb200_levels_from", "dxb200_mipmaps_compress_from_channels_ex", "dxb200_mipmaps_convert_from_ex", "dxb200_levels_from_ex", "dxb200_device_count", "dxb200_compute_pitch", "dxb200_calculate_mip_levels", "dxb200_compress",
                  "dxb200_compress_device", "dxb200_decompress", "dxb200_decompress_device", "dxb200_convert",
                  "dxb200_convert_device", "dxb200_generate_mipmaps", "dxb200_generate_mipmaps_device", "dxb200_resize", "dxb200_resize_device", "dxb200_premultiply_alpha", "dxb200_premultiply_alpha_device"):
         getattr(lib, name).restype = C.c_int32
@@ -276,23 +286,30 @@ def channel_steps(swizzle=(0, 1, 2, 3), zero_mask=0, one_mask=0, color_key=None,
                         1 if reconstruct_z else 0, 0 if color_key is None else color_key)
 
 
+def texconv_steps(demultiply=False, demultiply_flags=0, bc3_layout=0):
+    """the dxb200_texconv_steps of texconv's -alpha (demultiply, with demultiply_flags; REVERSE is implied) and -f BC3n / DXT5nm
+    (bc3_layout = 1) or RXGB (bc3_layout = 2)"""
+    return TexconvSteps(1 if demultiply else 0, demultiply_flags, bc3_layout)
+
+
 def mipmaps_compress_from_channels(bases, w, h, base_fmt, dst_fmt, source=None, channels=None, filter=0, levels=0, flags=0, steps=None,
-                                   row_pitch=0):
-    """mipmaps_compress_from_ex through dxb200_mipmaps_compress_from_channels with the ChannelSteps `channels` (None: none): (the
-    chains, IsAlphaAllOpaque of the output as a bool)"""
+                                   row_pitch=0, texconv=None):
+    """mipmaps_compress_from_ex through dxb200_mipmaps_compress_from_channels_ex with the ChannelSteps `channels` and the TexconvSteps
+    `texconv` (None: none): (the chains, IsAlphaAllOpaque of the output as a bool)"""
     args, outs = _from_args(bases, w, h, base_fmt, dst_fmt, source, filter, levels, flags, steps, row_pitch)
     opaque = C.c_int32(-1)
-    hr = lib.dxb200_mipmaps_compress_from_channels(*args[:3], C.byref(channels) if channels is not None else None, *args[3:], C.byref(opaque))
+    hr = lib.dxb200_mipmaps_compress_from_channels_ex(*args[:3], C.byref(channels) if channels is not None else None, *args[3:], C.byref(opaque),
+                                                      C.byref(texconv) if texconv is not None else None)
     if hr != 0:
-        raise DxTexError(hr, "dxb200_mipmaps_compress_from_channels")
+        raise DxTexError(hr, "dxb200_mipmaps_compress_from_channels_ex")
     return outs, opaque.value == 1
 
 
 def mipmaps_convert_from(bases, w, h, base_fmt, dst_fmt, source=None, channels=None, convert_filter=0, threshold=0.5, filter=0, levels=0,
-                         steps=None):
-    """dxb200_mipmaps_convert_from of an array of equally sized w x h host images of base_fmt (BC or not) into dst_fmt chains, with
-    the ChainSource `source`, the ChannelSteps `channels` and the ChainSteps `steps` (None: none): (one chain per image, laid out as
-    texture_layout(dst_fmt, W, H, 1, levels), IsAlphaAllOpaque of the output as a bool)"""
+                         steps=None, texconv=None):
+    """dxb200_mipmaps_convert_from_ex of an array of equally sized w x h host images of base_fmt (BC or not) into dst_fmt chains,
+    with the ChainSource `source`, the ChannelSteps `channels`, the ChainSteps `steps` and the TexconvSteps `texconv` (None: none):
+    (one chain per image, laid out as texture_layout(dst_fmt, W, H, 1, levels), IsAlphaAllOpaque of the output as a bool)"""
     bases = [np.ascontiguousarray(a).view(np.uint8).reshape(-1) for a in bases]
     cw, ch = (source.width, source.height) if source is not None and source.width else (w, h)
     levels = levels or F.count_mips(cw, ch)
@@ -301,19 +318,20 @@ def mipmaps_convert_from(bases, w, h, base_fmt, dst_fmt, source=None, channels=N
     s = images([make_image(_np_ptr(a), w, h, base_fmt) for a in bases])
     d = images([Image(lw, lh, dst_fmt, r, sp, _np_ptr(o) + off) for o in outs for (off, lw, lh, r, sp) in olayout])
     opaque = C.c_int32(-1)
-    hr = lib.dxb200_mipmaps_convert_from(s, len(bases), C.byref(source) if source is not None else None,
-                                         C.byref(channels) if channels is not None else None, dst_fmt, convert_filter, threshold, levels,
-                                         filter, C.byref(steps) if steps is not None else None, d, C.byref(opaque))
+    hr = lib.dxb200_mipmaps_convert_from_ex(s, len(bases), C.byref(source) if source is not None else None,
+                                            C.byref(channels) if channels is not None else None, dst_fmt, convert_filter, threshold, levels,
+                                            filter, C.byref(steps) if steps is not None else None, d, C.byref(opaque),
+                                            C.byref(texconv) if texconv is not None else None)
     if hr != 0:
-        raise DxTexError(hr, "dxb200_mipmaps_convert_from")
+        raise DxTexError(hr, "dxb200_mipmaps_convert_from_ex")
     return outs, opaque.value == 1
 
 
 def levels_from(bases, sizes, base_fmt, dst_fmt, source=None, channels=None, convert_filter=0, compress_flags=0, threshold=0.5,
-                steps=None):
-    """dxb200_levels_from of items that keep their own levels: bases[i][l] = level l of item i (host, tight, of base_fmt, BC or
-    not), (w, h) = sizes[l] for every item; the ChainSource `source`, the ChannelSteps `channels` and the ChainSteps `steps`
-    (None: none).  Returns (outs[i][l] = that level in dst_fmt, tight; IsAlphaAllOpaque of the output as a bool)."""
+                steps=None, texconv=None):
+    """dxb200_levels_from_ex of items that keep their own levels: bases[i][l] = level l of item i (host, tight, of base_fmt, BC or
+    not), (w, h) = sizes[l] for every item; the ChainSource `source`, the ChannelSteps `channels`, the ChainSteps `steps` and the
+    TexconvSteps `texconv` (None: none).  Returns (outs[i][l] = that level in dst_fmt, tight; IsAlphaAllOpaque of the output as a bool)."""
     levels = len(sizes)
     osizes = [(source.width, source.height)] if levels == 1 and source is not None and source.width else list(sizes)
     bases = [[np.ascontiguousarray(a).view(np.uint8).reshape(-1) for a in item] for item in bases]
@@ -321,11 +339,12 @@ def levels_from(bases, sizes, base_fmt, dst_fmt, source=None, channels=None, con
     s = images([make_image(_np_ptr(a), w, h, base_fmt) for item in bases for a, (w, h) in zip(item, sizes)])
     d = images([make_image(_np_ptr(o), w, h, dst_fmt) for item in outs for o, (w, h) in zip(item, osizes)])
     opaque = C.c_int32(-1)
-    hr = lib.dxb200_levels_from(s, len(bases), levels, C.byref(source) if source is not None else None,
-                                C.byref(channels) if channels is not None else None, dst_fmt, convert_filter, compress_flags, threshold,
-                                C.byref(steps) if steps is not None else None, d, C.byref(opaque))
+    hr = lib.dxb200_levels_from_ex(s, len(bases), levels, C.byref(source) if source is not None else None,
+                                   C.byref(channels) if channels is not None else None, dst_fmt, convert_filter, compress_flags, threshold,
+                                   C.byref(steps) if steps is not None else None, d, C.byref(opaque),
+                                   C.byref(texconv) if texconv is not None else None)
     if hr != 0:
-        raise DxTexError(hr, "dxb200_levels_from")
+        raise DxTexError(hr, "dxb200_levels_from_ex")
     return outs, opaque.value == 1
 
 

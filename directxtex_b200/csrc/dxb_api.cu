@@ -675,8 +675,8 @@ struct ResultWords
     bool all_zero() const { return std::all_of(w, w + n, [](uint32_t v) { return v == 0; }); }
 };
 
-// ---- [Decompress] -> [Resize] -> [channel steps] -> [Convert] -> [channel steps] -> GenerateMipMaps -> [coverage] -> [premultiply]
-// -> [Compress], chunk by chunk ---------------------------------------------------------------------------------------------------
+// ---- [Decompress] -> [demultiply] -> [Resize] -> [channel steps] -> [Convert] -> [channel steps] -> GenerateMipMaps -> [coverage]
+// -> [premultiply] -> [BC3 layout] -> [Compress], chunk by chunk --------------------------------------------------------------------
 // texconv runs GenerateMipMaps and then Compress on the result (Texconv/texconv.cpp; SURVEY 3.5), after Decompress (:2316-2480) for
 // a BC input and Resize (:2576-2643) for a new size; with the host-pointer calls every intermediate travels device -> host ->
 // device.  Here each item's base goes up once, every step runs in device memory and only the packed blocks come back: 4 B/texel
@@ -695,7 +695,9 @@ struct ResultWords
 // Convert steps run on all of them, and no mip or coverage launch runs.  Each step is one launch per chunk over all its levels:
 // the kernels take mixed-size batches through the job tables.  That keeps a premultiply or a Convert off its vector kernel, which
 // needs equal jobs, yet per-level launches measured no faster (DESIGN.md §4).  A BC base that passes through is copied into dst like an
-// uncompressed one, row of blocks by row of blocks.
+// uncompressed one, row of blocks by row of blocks.  texconv's -alpha (fp.demultiply) is one premultiply launch per chunk in place on
+// the images Decompress wrote (or on the uploaded base), before Resize; its BC3n / RXGB layout (cp.layout) is one channel-steps launch
+// per chunk over every level of the chunk's chains, in place, before Compress.  Neither has a plane of its own.
 int32_t run_chains(const dxb200_image* base, size_t items, size_t levels, uint32_t filter, const FromPlan& fp, const dxb200_image* dst,
                    const AlphaOpaquePlan& scan, const ResultWords* words)
 {
@@ -730,6 +732,9 @@ int32_t run_chains(const dxb200_image* base, size_t items, size_t levels, uint32
                     // the image the front steps write and the channel steps (the swizzle, with a Convert) run on
                     const dxb200_image* first = pre ? dev[pc - 1].data() : fp.convert && !front ? src : level.data();
                     if (fp.decompress) h2 = launch_decompress(fp.dp, src, mid ? decompressed : first, m, st);
+                    // -alpha, in place on what Decompress wrote, else on the base as it went up (a device copy)
+                    const dxb200_image* loaded = fp.decompress ? (mid ? decompressed : first) : up ? level.data() : src;
+                    if (h2 == DXB_S_OK && fp.demultiply) h2 = launch_pmalpha(fp.dm, loaded, loaded, m, st);
                     if (h2 == DXB_S_OK && fp.resize) h2 = launch_resize(mid ? decompressed : src, first, m, fp.resizeFilter, fp.resizeMode, st);
                     for (size_t k = 0; k < m && h2 == DXB_S_OK && !up && !front && !fp.convert; ++k)
                     {
@@ -752,6 +757,7 @@ int32_t run_chains(const dxb200_image* base, size_t items, size_t levels, uint32
                         for (size_t it = 0; it < cnt && cp.generate; ++it) level[it] = chains[it * levels + l];
                         h2 = launch_pmalpha(cp.pm, level.data(), level.data(), m, st);
                     }
+                    if (h2 == DXB_S_OK && cp.layout) h2 = launch_channel_steps(cp.lp, chains, chains, cnt * levels, st);
                     if (h2 == DXB_S_OK && cp.compressed) h2 = launch_compress(cp.compress, chains, out, cnt * levels, st);
                     if (h2 == DXB_S_OK && words)
                     {
@@ -1010,14 +1016,15 @@ int32_t dxb200_generate_mipmaps(const dxb200_image* chain, size_t items, size_t 
 // chains in device memory; dxb200_mipmaps_compress_from adds Decompress and Resize in front of the mips.
 // dxb200_mipmaps_compress_from_ex adds texconv's "set alpha mode" test of the output (:3738-3766): IsAlphaAllOpaque of the blocks,
 // scanned where they were made.  dxb200_mipmaps_compress_from_channels adds texconv's channel steps after Resize (:2645-3300).
-int32_t dxb200_mipmaps_compress_from_channels(const dxb200_image* base, size_t items, const dxb200_chain_source* source,
-                                              const dxb200_channel_steps* channels, size_t levels, uint32_t filter, const dxb200_chain_steps* steps,
-                                              uint32_t dstFormat, uint32_t flags, float threshold, float alphaWeight, const dxb200_image* dst,
-                                              int32_t* alphaAllOpaque)
+// dxb200_mipmaps_compress_from_channels_ex adds texconv's -alpha and BC3n / RXGB steps (dxb200_texconv_steps).
+int32_t dxb200_mipmaps_compress_from_channels_ex(const dxb200_image* base, size_t items, const dxb200_chain_source* source,
+                                                 const dxb200_channel_steps* channels, size_t levels, uint32_t filter, const dxb200_chain_steps* steps,
+                                                 uint32_t dstFormat, uint32_t flags, float threshold, float alphaWeight, const dxb200_image* dst,
+                                                 int32_t* alphaAllOpaque, const dxb200_texconv_steps* ts)
 {
     (void)alphaWeight;
     FromPlan fp;
-    int32_t hr = plan_mipmaps_compress_channels(base, items, source, channels, levels, filter, steps, dstFormat, flags, threshold, dst, &fp);
+    int32_t hr = plan_mipmaps_compress_channels(base, items, source, channels, levels, filter, steps, dstFormat, flags, threshold, dst, &fp, ts);
     if (hr != DXB_S_OK) return hr;
     AlphaOpaquePlan ap = {};
     if (alphaAllOpaque && (hr = plan_alpha_opaque(dst, items * levels, alphaAllOpaque, &ap)) != DXB_S_OK) return hr;
@@ -1026,6 +1033,15 @@ int32_t dxb200_mipmaps_compress_from_channels(const dxb200_image* base, size_t i
     hr = run_chains(base, items, levels, filter, fp, dst, ap, ap.scan ? &words : nullptr);
     if (hr == DXB_S_OK && alphaAllOpaque) *alphaAllOpaque = (!ap.scan || words.all_zero()) ? 1 : 0;
     return hr;
+}
+
+int32_t dxb200_mipmaps_compress_from_channels(const dxb200_image* base, size_t items, const dxb200_chain_source* source,
+                                              const dxb200_channel_steps* channels, size_t levels, uint32_t filter, const dxb200_chain_steps* steps,
+                                              uint32_t dstFormat, uint32_t flags, float threshold, float alphaWeight, const dxb200_image* dst,
+                                              int32_t* alphaAllOpaque)
+{
+    return dxb200_mipmaps_compress_from_channels_ex(base, items, source, channels, levels, filter, steps, dstFormat, flags, threshold, alphaWeight,
+                                                    dst, alphaAllOpaque, nullptr);
 }
 
 int32_t dxb200_mipmaps_compress_from_ex(const dxb200_image* base, size_t items, const dxb200_chain_source* source, size_t levels, uint32_t filter,
@@ -1056,14 +1072,15 @@ int32_t dxb200_mipmaps_compress(const dxb200_image* base, size_t items, size_t l
 }
 
 // ---- texconv's path to an uncompressed target in one call: the chain never leaves HBM until it is done (run_chains) ------------
-int32_t dxb200_mipmaps_convert_from(const dxb200_image* base, size_t items, const dxb200_chain_source* source, const dxb200_channel_steps* channels,
-                                    uint32_t dstFormat, uint32_t convertFilter, float threshold, size_t levels, uint32_t filter,
-                                    const dxb200_chain_steps* steps, const dxb200_image* dst, int32_t* alphaAllOpaque)
+int32_t dxb200_mipmaps_convert_from_ex(const dxb200_image* base, size_t items, const dxb200_chain_source* source,
+                                       const dxb200_channel_steps* channels, uint32_t dstFormat, uint32_t convertFilter, float threshold,
+                                       size_t levels, uint32_t filter, const dxb200_chain_steps* steps, const dxb200_image* dst,
+                                       int32_t* alphaAllOpaque, const dxb200_texconv_steps* ts)
 {
     FromPlan fp;
     AlphaOpaquePlan ap;
     int32_t hr = plan_mipmaps_convert_from(base, items, source, channels, dstFormat, convertFilter, threshold, levels, filter, steps, dst,
-                                           alphaAllOpaque, &fp, &ap);
+                                           alphaAllOpaque, &fp, &ap, ts);
     if (hr != DXB_S_OK) return hr;
     ResultWords words;
     if (ap.scan && (hr = words.alloc(items)) != DXB_S_OK) return hr;
@@ -1072,21 +1089,38 @@ int32_t dxb200_mipmaps_convert_from(const dxb200_image* base, size_t items, cons
     return hr;
 }
 
+int32_t dxb200_mipmaps_convert_from(const dxb200_image* base, size_t items, const dxb200_chain_source* source, const dxb200_channel_steps* channels,
+                                    uint32_t dstFormat, uint32_t convertFilter, float threshold, size_t levels, uint32_t filter,
+                                    const dxb200_chain_steps* steps, const dxb200_image* dst, int32_t* alphaAllOpaque)
+{
+    return dxb200_mipmaps_convert_from_ex(base, items, source, channels, dstFormat, convertFilter, threshold, levels, filter, steps, dst,
+                                          alphaAllOpaque, nullptr);
+}
+
 // ---- texconv on items that keep their own levels: every level stays in device memory until it is done (run_chains) -------------
-int32_t dxb200_levels_from(const dxb200_image* base, size_t items, size_t levels, const dxb200_chain_source* source,
-                           const dxb200_channel_steps* channels, uint32_t dstFormat, uint32_t convertFilter, uint32_t compressFlags,
-                           float threshold, const dxb200_chain_steps* steps, const dxb200_image* dst, int32_t* alphaAllOpaque)
+int32_t dxb200_levels_from_ex(const dxb200_image* base, size_t items, size_t levels, const dxb200_chain_source* source,
+                              const dxb200_channel_steps* channels, uint32_t dstFormat, uint32_t convertFilter, uint32_t compressFlags,
+                              float threshold, const dxb200_chain_steps* steps, const dxb200_image* dst, int32_t* alphaAllOpaque,
+                              const dxb200_texconv_steps* ts)
 {
     FromPlan fp;
     AlphaOpaquePlan ap;
     int32_t hr = plan_levels_from(base, items, levels, source, channels, dstFormat, convertFilter, compressFlags, threshold, steps, dst,
-                                  alphaAllOpaque, &fp, &ap);
+                                  alphaAllOpaque, &fp, &ap, ts);
     if (hr != DXB_S_OK) return hr;
     ResultWords words;
     if (ap.scan && (hr = words.alloc(items)) != DXB_S_OK) return hr;
     hr = run_chains(base, items, levels, 0, fp, dst, ap, ap.scan ? &words : nullptr);
     if (hr == DXB_S_OK && alphaAllOpaque) *alphaAllOpaque = (!ap.scan || words.all_zero()) ? 1 : 0;
     return hr;
+}
+
+int32_t dxb200_levels_from(const dxb200_image* base, size_t items, size_t levels, const dxb200_chain_source* source,
+                           const dxb200_channel_steps* channels, uint32_t dstFormat, uint32_t convertFilter, uint32_t compressFlags,
+                           float threshold, const dxb200_chain_steps* steps, const dxb200_image* dst, int32_t* alphaAllOpaque)
+{
+    return dxb200_levels_from_ex(base, items, levels, source, channels, dstFormat, convertFilter, compressFlags, threshold, steps, dst,
+                                 alphaAllOpaque, nullptr);
 }
 
 int32_t dxb200_premultiply_alpha_device(const dxb200_image* src, size_t nimages, uint32_t flags, const dxb200_image* dst, void* stream)

@@ -350,12 +350,37 @@ struct ChainPlan
     bool generate = true; uint32_t mode;
     bool coverage; float ref;
     bool premultiply; dxb_convert_params pm;
+    bool layout; dxb_convert_params lp;         // texconv's BC3n / RXGB layout, after premultiply
     bool compressed; CompressPlan compress;
 };
 
-// GenerateMipMaps (when cp->generate), then the optional coverage and premultiply steps of `steps`, on cp->chain, with the HRESULT
-// of the first of those calls that would fail
-int32_t plan_chain_steps(size_t items, size_t levels, uint32_t filter, const dxb200_chain_steps* steps, ChainPlan* cp)
+// ---- texconv's -alpha and BC3n / RXGB steps (dxb200_texconv_steps) --------------------------------------------------------------
+// The _ex calls' own rules, checked before any other: a layout other than 1 or 2, or a layout into anything but BC3_UNORM (texconv
+// asserts it, :3556) or from a call with no BC target, is E_INVALIDARG.
+int32_t check_texconv_steps(const dxb200_texconv_steps* ts, uint32_t dstFormat, bool bcTarget)
+{
+    if (!ts) return DXB_S_OK;
+    if (ts->bc3Layout > 2) return DXB_E_INVALIDARG;
+    if (ts->bc3Layout && (!bcTarget || dstFormat != DXB_FMT_BC3_UNORM)) return DXB_E_INVALIDARG;
+    return DXB_S_OK;
+}
+
+uint32_t bc3_layout(const dxb200_texconv_steps* ts) { return ts ? ts->bc3Layout : 0u; }
+
+// The layout as TransformImage channel steps: DXT5nm is XMVectorPermute<4,1,5,0>(p, g_XMIdentityR0) = (1, y, 0, x), RXGB is
+// XMVectorSwizzle<3,1,2,0> = (a, g, b, r) (Texconv/texconv.cpp:3566-3595)
+dxb200_channel_steps bc3_layout_steps(uint32_t layout)
+{
+    dxb200_channel_steps s = { { 3, 1, 2, 0 }, 0, 0, 0, 0, 0, 0 };
+    if (layout == 1) { s.swizzle[0] = 0; s.zeroMask = 0x4; s.oneMask = 0x1; }
+    return s;
+}
+
+int32_t plan_channel_steps(const dxb200_image* src, size_t n, const dxb200_channel_steps* steps, const dxb200_image* dst, dxb_convert_params* P);
+
+// GenerateMipMaps (when cp->generate), then the optional coverage and premultiply steps of `steps` and the BC3 layout, on cp->chain,
+// with the HRESULT of the first of those calls that would fail
+int32_t plan_chain_steps(size_t items, size_t levels, uint32_t filter, const dxb200_chain_steps* steps, ChainPlan* cp, uint32_t layout = 0)
 {
     const dxb200_image* chain = cp->chain.data();
     int32_t hr = DXB_S_OK;
@@ -365,13 +390,16 @@ int32_t plan_chain_steps(size_t items, size_t levels, uint32_t filter, const dxb
     if (cp->coverage && (hr = plan_alpha_coverage(chain, items * levels, chain)) != DXB_S_OK) return hr;
     cp->premultiply = steps && steps->premultiply;
     if (cp->premultiply && (hr = plan_pmalpha(chain, items * levels, steps->pmalphaFlags, chain, &cp->pm)) != DXB_S_OK) return hr;
+    cp->layout = layout != 0;
+    const dxb200_channel_steps ls = bc3_layout_steps(layout);
+    if (cp->layout && (hr = plan_channel_steps(chain, items * levels, &ls, chain, &cp->lp)) != DXB_S_OK) return hr;
     return DXB_S_OK;
 }
 
-// Every check of the four steps before anything is uploaded, each with the HRESULT the reference's four calls would return at
-// the first step that fails; steps == nullptr (or no step enabled) = GenerateMipMaps + Compress.
+// Every check of the four steps (and the BC3 layout before Compress) before anything is uploaded, each with the HRESULT the
+// reference's calls would return at the first step that fails; steps == nullptr (or no step enabled) = GenerateMipMaps + Compress.
 int32_t plan_mipmaps_compress(const dxb200_image* base, size_t items, size_t levels, uint32_t filter, const dxb200_chain_steps* steps,
-                              uint32_t dstFormat, uint32_t flags, float threshold, const dxb200_image* dst, ChainPlan* cp)
+                              uint32_t dstFormat, uint32_t flags, float threshold, const dxb200_image* dst, ChainPlan* cp, uint32_t layout = 0)
 {
     if (!base || !dst || !items || !levels) return DXB_E_INVALIDARG;
     std::vector<dxb200_image>& chain = cp->chain;
@@ -393,7 +421,7 @@ int32_t plan_mipmaps_compress(const dxb200_image* base, size_t items, size_t lev
         }
         chain[i * levels].rowPitch = base[i].rowPitch; chain[i * levels].slicePitch = base[i].slicePitch;
     }
-    const int32_t hr = plan_chain_steps(items, levels, filter, steps, cp);
+    const int32_t hr = plan_chain_steps(items, levels, filter, steps, cp, layout);
     if (hr != DXB_S_OK) return hr;
     cp->compressed = true;
     return plan_compress(chain.data(), items * levels, dstFormat, flags, threshold, dst, &cp->compress);
@@ -439,15 +467,18 @@ int32_t plan_channel_steps(const dxb200_image* src, size_t n, const dxb200_chann
     return DXB_S_OK;
 }
 
-// The format texconv decompresses a BC base to when channel steps follow (:2393-2447): BC4 and BC5 hold one and two channels, so a
-// step that reads or writes another channel needs R8G8B8A8 (UNORM or SNORM as the BC format); otherwise DefaultDecompress.
-uint32_t channel_decompress_format(uint32_t bcFormat, const dxb200_channel_steps* s)
+// The format texconv decompresses a BC base to when channel steps or a BC3 layout follow (:2393-2447): BC4 and BC5 hold one and two
+// channels, so a step that reads or writes another channel, or a layout (dxt5nm || dxt5rxgb), needs R8G8B8A8 (UNORM or SNORM as the
+// BC format); otherwise DefaultDecompress.
+uint32_t channel_decompress_format(uint32_t bcFormat, const dxb200_channel_steps* s, uint32_t layout = 0)
 {
     const uint32_t def = dxb_default_decompress(bcFormat);
     const bool bc4 = bcFormat == DXB_FMT_BC4_UNORM || bcFormat == DXB_FMT_BC4_SNORM, bc5 = bcFormat == DXB_FMT_BC5_UNORM || bcFormat == DXB_FMT_BC5_SNORM;
-    if (!s || !channel_steps_word(*s) || (!bc4 && !bc5)) return def;
-    bool wide = s->reconstructZ || (bc4 && s->invertY);
-    for (uint32_t c = bc4 ? 1u : 2u; c < 4; ++c) wide |= s->swizzle[c] != c || ((s->zeroMask | s->oneMask) >> c & 1u);
+    const bool ch = s && channel_steps_word(*s);
+    if ((!ch && !layout) || (!bc4 && !bc5)) return def;
+    bool wide = layout != 0;
+    if (ch) wide |= s->reconstructZ || (bc4 && s->invertY);
+    for (uint32_t c = bc4 ? 1u : 2u; c < 4 && ch; ++c) wide |= s->swizzle[c] != c || ((s->zeroMask | s->oneMask) >> c & 1u);
     if (!wide) return def;
     return (bcFormat == DXB_FMT_BC4_SNORM || bcFormat == DXB_FMT_BC5_SNORM) ? DXB_FMT_R8G8B8A8_SNORM : DXB_FMT_R8G8B8A8_UNORM;
 }
@@ -461,8 +492,9 @@ uint32_t channel_decompress_format(uint32_t bcFormat, const dxb200_channel_steps
 // chain in the target format and the later steps (post) run in place there.
 struct FromPlan
 {
-    bool decompress, resize, channels, convert, post;
+    bool decompress, demultiply, resize, channels, convert, post;
     dxb_compress_params dp;                     // the Decompress
+    dxb_convert_params dm;                      // -alpha: PremultiplyAlpha(REVERSE) of what the Decompress leaves, in place
     std::vector<dxb200_image> decompressed;
     uint32_t resizeFilter, resizeMode;          // the Resize
     std::vector<dxb200_image> level0;
@@ -486,17 +518,17 @@ std::vector<dxb200_image> plan_images(const dxb200_image* base, size_t n, uint32
     return out;
 }
 
-// Decompress (a BC base, when source != nullptr) and Resize (when the source's size differs) of the base, with the HRESULT of the
-// first that would fail; fp->level0 = the images they leave.  With channel steps and no decompress format, a BC4 / BC5 base
-// decompresses to channel_decompress_format.
-int32_t plan_front(const dxb200_image* base, size_t items, const dxb200_chain_source* source, const dxb200_channel_steps* channels, FromPlan* fp)
+// Decompress (a BC base, when source != nullptr), -alpha's demultiply (when ts->demultiply) and Resize (when the source's size
+// differs) of the base, with the HRESULT of the first that would fail; fp->level0 = the images they leave.  With no decompress format,
+// a BC4 / BC5 base decompresses to channel_decompress_format of the channel steps and the BC3 layout.
+int32_t plan_front(const dxb200_image* base, size_t items, const dxb200_chain_source* source, const dxb200_channel_steps* channels, FromPlan* fp,
+                   const dxb200_texconv_steps* ts = nullptr)
 {
-    fp->decompress = fp->resize = fp->channels = fp->convert = fp->post = false;
+    fp->decompress = fp->demultiply = fp->resize = fp->channels = fp->convert = fp->post = false;
     fp->resizeFilter = fp->resizeMode = 0;
     fp->decompressed.clear();
     fp->level0.clear();
     if (source && (!source->width) != (!source->height)) return DXB_E_INVALIDARG;
-    const bool ch = channels && channel_steps_word(*channels);
     const size_t w = source && source->width ? source->width : base[0].width, h = source && source->height ? source->height : base[0].height;
     fp->decompress = source && is_compressed(base[0].format);
     fp->resize = (w != base[0].width || h != base[0].height);
@@ -504,12 +536,15 @@ int32_t plan_front(const dxb200_image* base, size_t items, const dxb200_chain_so
     int32_t hr = DXB_S_OK;
     if (fp->decompress)
     {
-        const uint32_t fmt = source->decompressFormat ? source->decompressFormat : ch ? channel_decompress_format(base[0].format, channels)
-                                                                                      : dxb_default_decompress(base[0].format);
+        const uint32_t fmt = source->decompressFormat ? source->decompressFormat : channel_decompress_format(base[0].format, channels, bc3_layout(ts));
         fp->decompressed = plan_images(base, items, fmt, 0, 0);
         if ((hr = plan_decompress(base, items, fmt, fp->decompressed.data(), &fp->dp)) != DXB_S_OK) return hr;
         fp->level0 = fp->decompressed;
     }
+    // texconv's -alpha (:2483-2531); REVERSE is implied
+    fp->demultiply = ts && ts->demultiply;
+    if (fp->demultiply && (hr = plan_pmalpha(fp->level0.data(), items, 0x2u | ts->demultiplyFlags, fp->level0.data(), &fp->dm)) != DXB_S_OK)
+        return hr;
     if (fp->resize)
     {
         const std::vector<dxb200_image> resized = plan_images(base, items, fp->level0[0].format, w, h);
@@ -520,27 +555,29 @@ int32_t plan_front(const dxb200_image* base, size_t items, const dxb200_chain_so
     return DXB_S_OK;
 }
 
-// Every check of Decompress, Resize, the channel steps and the four steps of plan_mipmaps_compress before anything is uploaded, each
-// with the HRESULT of the first of the separate calls that would fail.  source == nullptr, or a source that changes nothing, and
-// channels == nullptr, or no channel step enabled = plan_mipmaps_compress.
+// Every check of Decompress, -alpha's demultiply, Resize, the channel steps and the steps of plan_mipmaps_compress before anything is
+// uploaded, each with the HRESULT of the first of the separate calls that would fail; check_texconv_steps comes before all of them.
+// source == nullptr, or a source that changes nothing, channels == nullptr, or no channel step enabled, and ts == nullptr, or all
+// zeros = plan_mipmaps_compress.
 int32_t plan_mipmaps_compress_channels(const dxb200_image* base, size_t items, const dxb200_chain_source* source, const dxb200_channel_steps* channels,
                                        size_t levels, uint32_t filter, const dxb200_chain_steps* steps, uint32_t dstFormat, uint32_t flags,
-                                       float threshold, const dxb200_image* dst, FromPlan* fp)
+                                       float threshold, const dxb200_image* dst, FromPlan* fp, const dxb200_texconv_steps* ts = nullptr)
 {
-    fp->decompress = fp->resize = fp->channels = fp->convert = fp->post = false;
+    fp->decompress = fp->demultiply = fp->resize = fp->channels = fp->convert = fp->post = false;
     fp->resizeFilter = fp->resizeMode = 0;
     fp->decompressed.clear();
+    int32_t hr = check_texconv_steps(ts, dstFormat, true);
+    if (hr != DXB_S_OK) return hr;
     const bool ch = channels && channel_steps_word(*channels);
-    if ((!source && !ch) || !base || !items)
+    if ((!source && !ch && !(ts && ts->demultiply)) || !base || !items)
     {
         fp->level0.clear();
-        return plan_mipmaps_compress(base, items, levels, filter, steps, dstFormat, flags, threshold, dst, &fp->chain);
+        return plan_mipmaps_compress(base, items, levels, filter, steps, dstFormat, flags, threshold, dst, &fp->chain, bc3_layout(ts));
     }
-    int32_t hr = plan_front(base, items, source, channels, fp);
-    if (hr != DXB_S_OK) return hr;
+    if ((hr = plan_front(base, items, source, channels, fp, ts)) != DXB_S_OK) return hr;
     if (ch && (hr = plan_channel_steps(fp->level0.data(), items, channels, fp->level0.data(), &fp->cp)) != DXB_S_OK) return hr;
     fp->channels = ch;
-    return plan_mipmaps_compress(fp->level0.data(), items, levels, filter, steps, dstFormat, flags, threshold, dst, &fp->chain);
+    return plan_mipmaps_compress(fp->level0.data(), items, levels, filter, steps, dstFormat, flags, threshold, dst, &fp->chain, bc3_layout(ts));
 }
 
 int32_t plan_mipmaps_compress_from(const dxb200_image* base, size_t items, const dxb200_chain_source* source, size_t levels, uint32_t filter,
@@ -662,12 +699,13 @@ void merge_channel_launches(FromPlan* fp)
 int32_t plan_mipmaps_convert_from(const dxb200_image* base, size_t items, const dxb200_chain_source* source, const dxb200_channel_steps* channels,
                                   uint32_t dstFormat, uint32_t convertFilter, float threshold, size_t levels, uint32_t filter,
                                   const dxb200_chain_steps* steps, const dxb200_image* dst, const int32_t* alphaAllOpaque, FromPlan* fp,
-                                  AlphaOpaquePlan* ap)
+                                  AlphaOpaquePlan* ap, const dxb200_texconv_steps* ts = nullptr)
 {
     ap->scan = ap->blocks = false; ap->format = 0;
-    if (!base || !items) return DXB_E_INVALIDARG;
-    int32_t hr = plan_front(base, items, source, channels, fp);
+    int32_t hr = check_texconv_steps(ts, dstFormat, false);
     if (hr != DXB_S_OK) return hr;
+    if (!base || !items) return DXB_E_INVALIDARG;
+    if ((hr = plan_front(base, items, source, channels, fp, ts)) != DXB_S_OK) return hr;
     dxb200_channel_steps swizzle, later;
     split_channel_steps(channels, &swizzle, &later);
     fp->channels = channel_steps_word(swizzle) != 0;
@@ -713,23 +751,24 @@ int32_t plan_mipmaps_convert_from(const dxb200_image* base, size_t items, const 
 int32_t plan_levels_from(const dxb200_image* base, size_t items, size_t levels, const dxb200_chain_source* source,
                          const dxb200_channel_steps* channels, uint32_t dstFormat, uint32_t convertFilter, uint32_t compressFlags,
                          float threshold, const dxb200_chain_steps* steps, const dxb200_image* dst, const int32_t* alphaAllOpaque,
-                         FromPlan* fp, AlphaOpaquePlan* ap)
+                         FromPlan* fp, AlphaOpaquePlan* ap, const dxb200_texconv_steps* ts = nullptr)
 {
     ap->scan = ap->blocks = false; ap->format = 0;
+    int32_t hr = check_texconv_steps(ts, dstFormat, true);
+    if (hr != DXB_S_OK) return hr;
     if (!base || !items || !levels) return DXB_E_INVALIDARG;
     const size_t n = items * levels;
     const dxb200_chain_source keep = { 0, 0, 0, 0 };
     const dxb200_chain_source* src = source ? source : &keep;
     if (levels > 1 && ((src->width && src->width != base[0].width) || (src->height && src->height != base[0].height))) return DXB_E_INVALIDARG;
     if (steps && steps->alphaReference > 0.0f) return DXB_E_INVALIDARG;
-    int32_t hr = plan_front(base, n, src, channels, fp);
-    if (hr != DXB_S_OK) return hr;
+    if ((hr = plan_front(base, n, src, channels, fp, ts)) != DXB_S_OK) return hr;
     ChainPlan& cp = fp->chain;
     cp.generate = false; cp.mode = 0;
     dxb200_channel_steps swizzle, later;
     split_channel_steps(channels, &swizzle, &later);
     const bool pass = is_compressed(base[0].format) && dstFormat == base[0].format && !channel_steps_word(swizzle) && !channel_steps_word(later)
-                      && !(steps && steps->premultiply) && !fp->resize;
+                      && !(steps && steps->premultiply) && !fp->resize && !fp->demultiply && !bc3_layout(ts);
     if (pass)
     {
         fp->decompress = false;
@@ -754,7 +793,7 @@ int32_t plan_levels_from(const dxb200_image* base, size_t items, size_t levels, 
     if (fp->post && (hr = plan_channel_steps(fp->convert ? out : fp->level0.data(), n, &later, out, &fp->pp)) != DXB_S_OK) return hr;
     if (!fp->convert && fp->post) merge_channel_launches(fp);
     cp.chain.assign(out, out + n);
-    if ((hr = plan_chain_steps(items, levels, 0, steps, &cp)) != DXB_S_OK) return hr;
+    if ((hr = plan_chain_steps(items, levels, 0, steps, &cp, bc3_layout(ts))) != DXB_S_OK) return hr;
     if (cp.compressed && (hr = plan_compress(out, n, dstFormat, compressFlags, threshold, dst, &cp.compress)) != DXB_S_OK) return hr;
     const bool copy = !fp->decompress && !fp->resize && !fp->convert && !cp.compressed;
     if (copy && (hr = plan_copy(base, n)) != DXB_S_OK) return hr;

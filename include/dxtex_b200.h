@@ -292,6 +292,47 @@ DXB200_API int32_t  dxb200_levels_from(const dxb200_image* base, size_t items, s
                                        uint32_t compressFlags, float threshold, const dxb200_chain_steps* steps, const dxb200_image* dst,
                                        int32_t* alphaAllOpaque);
 
+/* texconv steps that dxb200_chain_source / dxb200_channel_steps / dxb200_chain_steps do not hold */
+typedef struct dxb200_texconv_steps
+{
+    uint32_t demultiply;       /* nonzero: -alpha: PremultiplyAlpha(TEX_PMALPHA_REVERSE | demultiplyFlags) after Decompress, before Resize */
+    uint32_t demultiplyFlags;  /* TEX_PMALPHA_FLAGS (texconv passes its -srgb / -srgbi / -srgbo bits); REVERSE is implied */
+    uint32_t bc3Layout;        /* 0 none; 1 DXT5nm / BC3n: (1, y, 0, x); 2 RXGB: (a, g, b, r); after premultiply, before Compress */
+} dxb200_texconv_steps;
+/* dxb200_mipmaps_compress_from_channels, dxb200_mipmaps_convert_from and dxb200_levels_from with texconv's -alpha
+ * (Texconv/texconv.cpp:2483-2531) and -f BC3n / DXT5nm / RXGB (:452-456, 1510-1518, 3553-3617) steps.  ts == NULL, or all zeros, is
+ * exactly the call without _ex (those calls are these with NULL).  The steps run in this order, each only when it does something:
+ *   Decompress -> demultiply -> Resize -> swizzle / masks -> [Convert] -> colour key / invert Y / reconstruct Z -> GenerateMipMaps
+ *   -> coverage -> premultiply -> BC3 layout -> Compress -> IsAlphaAllOpaque,
+ * with results identical to the separate calls in that order:
+ *   demultiply = dxb200_premultiply_alpha(0x2 REVERSE | ts->demultiplyFlags) of the working images: level 0 of every item for a
+ *     generated chain, every level as loaded for dxb200_levels_from_ex;
+ *   BC3 layout = dxb200_apply_channel_steps of every image of the chain, in the chain's format, with swizzle { 0, 1, 2, 0 },
+ *     zeroMask 0x4 and oneMask 0x1 (DXT5nm) or swizzle { 3, 1, 2, 0 } (RXGB).  Save the RXGB result with DDS_FLAGS_FORCE_DXT5_RXGB.
+ * With a layout and no decompress format, a BC4 or BC5 base decompresses to R8G8B8A8_UNORM (R8G8B8A8_SNORM for the SNORM twins), as
+ * texconv picks it (:2404-2447).  texconv runs -alpha only on an image whose format has alpha and is not A8_UNORM and whose alpha
+ * mode is premultiplied; the caller mirrors that guard.  Here a demultiply on a working format without alpha is PremultiplyAlpha's
+ * HRESULT_E_NOT_SUPPORTED.  Every argument is checked before anything is uploaded: first ts's own rules, each E_INVALIDARG
+ * (bc3Layout > 2; a layout with a dstFormat other than BC3_UNORM, as texconv asserts at :3556; any layout on
+ * dxb200_mipmaps_convert_from_ex, which has no BC target), then the rules of the call without _ex, then the HRESULT of the first
+ * separate call above that would fail, each checked on the format and size the image has at that point.  dxb200_levels_from_ex
+ * passes no BC chain through when a demultiply or a layout runs (texconv drops the original image after both, :2529, :3616).
+ * Neither step adds a staged image: one premultiply launch per chunk for the demultiply and one channel-steps launch per chunk for
+ * the layout, both in place. */
+DXB200_API int32_t  dxb200_mipmaps_compress_from_channels_ex(const dxb200_image* base, size_t items, const dxb200_chain_source* source,
+                                                             const dxb200_channel_steps* channels, size_t levels, uint32_t filter,
+                                                             const dxb200_chain_steps* steps, uint32_t dstFormat, uint32_t flags,
+                                                             float threshold, float alphaWeight, const dxb200_image* dst,
+                                                             int32_t* alphaAllOpaque, const dxb200_texconv_steps* ts);
+DXB200_API int32_t  dxb200_mipmaps_convert_from_ex(const dxb200_image* base, size_t items, const dxb200_chain_source* source,
+                                                   const dxb200_channel_steps* channels, uint32_t dstFormat, uint32_t convertFilter,
+                                                   float threshold, size_t levels, uint32_t filter, const dxb200_chain_steps* steps,
+                                                   const dxb200_image* dst, int32_t* alphaAllOpaque, const dxb200_texconv_steps* ts);
+DXB200_API int32_t  dxb200_levels_from_ex(const dxb200_image* base, size_t items, size_t levels, const dxb200_chain_source* source,
+                                          const dxb200_channel_steps* channels, uint32_t dstFormat, uint32_t convertFilter,
+                                          uint32_t compressFlags, float threshold, const dxb200_chain_steps* steps, const dxb200_image* dst,
+                                          int32_t* alphaAllOpaque, const dxb200_texconv_steps* ts);
+
 /* ScratchImage::IsAlphaAllOpaque (DirectXTexImage.cpp:800-852; IsAlphaAllOpaqueBC, DirectXTexCompress.cpp:539-621) of
  * `nimages` images of one format: *opaque = 1 when every texel inside every image has alpha >= 0.997 (uncompressed, as
  * LoadScanline reads it) or >= 0.99 (decoded BC1 / BC2 / BC3 / BC7 blocks; the padding texels of partial blocks do not count),
