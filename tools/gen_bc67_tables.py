@@ -49,25 +49,67 @@ _h1w = lambda s, i: 0x00307654 if (p2[s] >> i) & 1 else 0x00043210
 h1sel = [_h1w(s, 2 * k) | (_h1w(s, 2 * k + 1) << 32) for s in range(64) for k in range(8)]
 # BC7 block layout per mode (D3DX_BC7 mode table, BC6HBC7.cpp:1106-1124; bit order of D3DX_BC7::Decode, :2566-2780): mode (unary),
 # partition, rotation, index selector, then R of every endpoint, G, B, A, p-bits, colour indices, alpha indices.
-# (colour bits, alpha bits, p-bit type 0 none / 1 per endpoint / 2 per subset, subsets, partition bits, rotation bits, selector bits)
-BC7_MODES = [(4, 0, 1, 3, 4, 0, 0), (6, 0, 2, 2, 6, 0, 0), (5, 0, 0, 3, 6, 0, 0), (7, 0, 1, 2, 6, 0, 0),
-             (5, 6, 0, 1, 0, 2, 1), (7, 8, 0, 1, 0, 2, 0), (7, 7, 1, 1, 0, 0, 0), (5, 5, 1, 2, 6, 0, 0)]
-pack_mode, pack_ep = [], []
-for mode, (cb, ab, pt, ns, partb, rotb, imb) in enumerate(BC7_MODES):
+# (colour bits, alpha bits, p-bit type 0 none / 1 per endpoint / 2 per subset, subsets, partition bits, rotation bits, selector bits,
+#  colour index bits, alpha index bits)
+BC7_MODES = [(4, 0, 1, 3, 4, 0, 0, 3, 0), (6, 0, 2, 2, 6, 0, 0, 3, 0), (5, 0, 0, 3, 6, 0, 0, 2, 0), (7, 0, 1, 2, 6, 0, 0, 2, 0),
+             (5, 6, 0, 1, 0, 2, 1, 2, 3), (7, 8, 0, 1, 0, 2, 0, 2, 2), (7, 7, 1, 1, 0, 0, 0, 4, 0), (5, 5, 1, 2, 6, 0, 0, 2, 0)]
+# Stage 4 of the encoder (dxb_bc7.cuh) reads one layout word per (mode, index selector) and one field word per (mode, lane).
+# dxb_bc7_lay[m | sel << 3] (sel = the index selector, only ever 1 in mode 4; other modes repeat their sel = 0 word):
+#   bits 0-2 colour index bits, 3-5 alpha index bits (0: no alpha index set), 6-7 subsets, 8 alpha searched with the colour set,
+#   9-15 first index bit - w (w = 32 in mode 4, whose first index set crosses bit 64, else 64), 16 w == 32, 17 the first index set is
+#   the alpha set, 18-20 bits of the first index set, 21-23 bits of the second set (0: none), 24-30 first bit of the second set - 64 (1: none),
+#   32-39 the header's constant bits (mode in unary, index selector), 40-43 the shift of the partition or rotation field (mode + 1).
+lay = []
+for key in range(16):
+    mode, sel = key & 7, key >> 3
+    sel = sel if mode == 4 else 0
+    cb, ab, pt, ns, partb, rotb, imb, ibc, iba = BC7_MODES[mode]
+    if mode == 4:
+        ibc, iba = (3, 2) if sel else (2, 3)
     hdrb = mode + 1 + partb + rotb + imb
-    epb = ns * 2 * (3 * cb + ab)
     npb = 2 * ns if pt == 1 else (ns if pt == 2 else 0)
-    pack_mode.append((hdrb + epb + npb) | ((hdrb + epb) << 8) | (partb << 16) | (rotb << 19) | (imb << 21) | (npb << 24))
+    first = hdrb + ns * 2 * (3 * cb + ab) + npb
+    ib1, ib2 = (2, 3) if mode == 4 else (ibc, iba)
+    second = first + 16 * ib1 - ns
+    w = 32 if mode == 4 else 64
+    # every index set but mode 4's first one lies in bits 64..127, mode 4's first one in bits 32..95
+    assert w < first and first + 16 * ib1 - ns <= w + 64 and (ib2 == 0 or (second > 64 and second + 16 * ib2 - 1 == 128))
+    assert ib2 == 0 or first + 16 * ib1 - ns == second
+    hdr = (1 << mode) | (sel << (mode + 1 + partb + rotb))
+    lay.append(ibc | (iba << 3) | (ns << 6) | ((1 if mode in (6, 7) else 0) << 8) | ((first - w) << 9) | ((1 if w == 32 else 0) << 16) |
+               ((1 if (mode == 4 and sel) else 0) << 17) | (ib1 << 18) | (ib2 << 21) | (((second - 64) if ib2 else 1) << 24) |
+               (hdr << 32) | ((mode + 1) << 40))
+# dxb_bc7_lay_ep[16 m + l]: the endpoint fields l (bits 0-31) and l + 16 (bits 32-63) of mode m (field f = channel * 2 * subsets +
+# endpoint, endpoint = 2 * subset + 0 / 1; every field lies in bits 0..98).  Per field: bits 0-6 position p, 7-8 subset, 12-14 the
+# byte of the subset's endpoint pair (endpoint * 4 + channel: a byte-permute selector that moves it to the top byte), 16-22 120 - p,
+# 26-31 32 - width (32: no such field).
+# dxb_bc7_lay_pb[16 m + l]: position (63..97) of the p-bit that lane l deposits, 0 for none: per endpoint (p-bit type 1) lane l
+# holds the R field of endpoint l; per subset (type 2) lane 2 s holds the R field of subset s's first endpoint.  The p-bit is
+# the bit of that R byte just below its field.
+lay_ep, lay_pb = [], []
+for mode, (cb, ab, pt, ns, partb, rotb, imb, ibc, iba) in enumerate(BC7_MODES):
+    hdrb = mode + 1 + partb + rotb + imb
     per = 2 * ns
-    for fi in range(32):
-        if fi >= 4 * per:
-            pack_ep.append(0)
-            continue
-        c, e = fi // per, fi % per
-        nb = ab if c == 3 else cb
-        pos = hdrb + (3 * per * cb + e * ab if c == 3 else (c * per + e) * cb)
-        assert pos < 128 and nb < 16
-        pack_ep.append(pos | (nb << 7) | (c << 11) | ((e >> 1) << 13) | ((e & 1) << 15))
+    pbs = hdrb + ns * 2 * (3 * cb + ab)
+    for l in range(16):
+        words = []
+        for fi in (l, l + 16):
+            if fi >= 4 * per or (fi >= 3 * per and ab == 0):
+                words.append(32 << 26)
+                continue
+            c, e = fi // per, fi % per
+            nb = ab if c == 3 else cb
+            pos = hdrb + (3 * per * cb + e * ab if c == 3 else (c * per + e) * cb)
+            assert pos + nb <= 99 and 8 - nb <= pos
+            words.append(pos | ((e >> 1) << 7) | ((((e & 1) << 2) | c) << 12) | ((120 - pos) << 16) | ((32 - nb) << 26))
+        lay_ep.append(words[0] | (words[1] << 32))
+        q = 0
+        if pt == 1 and l < per:
+            q = pbs + l
+        elif pt == 2 and l < per and l % 2 == 0:
+            q = pbs + l // 2
+        assert q == 0 or 63 <= q <= 97
+        lay_pb.append(q)
 def arr(name, ctype, vals, fmt, per=8):
     out = [f'DXB_TABLE {ctype} {name}[{len(vals)}] = {{']
     for k in range(0, len(vals), per):
@@ -83,10 +125,9 @@ hdr = '''// dxb_bc67_tables.h — GENERATED by tools/gen_bc67_tables.py; do not 
 //   dxb_bc7_afrag[t*128 + lane*4 + r]  tensor-core A fragments of the shape/pixel membership matrix (dxb_bc7.cuh stage 1)
 //   dxb_bc7_h1sel[8s + k]  words of pixels 2k (bits 0-31) and 2k + 1 (bits 32-63) of shape s: 0x00043210 subset 0, 0x00307654 subset 1
 //                          (axis selector + projection bias of the stage-1 shape ranking, dxb_bc7.cuh)
-//   dxb_bc7_pack_mode[m]   BC7 mode m: bits 0-6 first index bit, 8-14 first p-bit, 16-18 partition bits, 19-20 rotation bits,
-//                          21 index-selector bits, 24-26 p-bit count                         (block packer, dxb_bc7.cuh stage 4)
-//   dxb_bc7_pack_ep[32m + f]  endpoint field f of mode m (f = channel * 2 * subsets + 2 * subset + endpoint): bits 0-6 position,
-//                          7-10 width (0 = no such field), 11-12 channel, 13-14 subset, 15 endpoint
+//   dxb_bc7_lay[m | sel << 3]  BC7 mode m, index selector sel: index bits, subsets, index-field windows, header pieces
+//   dxb_bc7_lay_ep[16m + l], dxb_bc7_lay_pb[16m + l]  endpoint fields l and l + 16 and the p-bit that lane l of mode m packs
+//                          (block packer, dxb_bc7.cuh stage 4; bit layouts in tools/gen_bc67_tables.py)
 // Subset 0's anchor is always pixel 0.
 #pragma once
 #include <stdint.h>
@@ -106,8 +147,9 @@ body = '\n\n'.join([
     arr('dxb_anchor3b', 'uint8_t', a3b, '%2d', 16),
     arr('dxb_bc7_afrag', 'uint32_t', afrag, '0x%08X', 4),
     arr('dxb_bc7_h1sel', 'uint64_t', h1sel, '0x%016XULL', 4),
-    arr('dxb_bc7_pack_mode', 'uint32_t', pack_mode, '0x%08X'),
-    arr('dxb_bc7_pack_ep', 'uint16_t', pack_ep, '0x%04X'),
+    arr('dxb_bc7_lay', 'uint64_t', lay, '0x%016XULL', 4),
+    arr('dxb_bc7_lay_ep', 'uint64_t', lay_ep, '0x%016XULL', 4),
+    arr('dxb_bc7_lay_pb', 'uint8_t', lay_pb, '%2d', 16),
 ])
 out = os.path.join(os.path.dirname(__file__), '..', 'directxtex_b200', 'csrc', 'dxb_bc67_tables.h')
 open(out, 'w').write(hdr + '\n' + body + '\n')

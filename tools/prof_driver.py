@@ -1,5 +1,9 @@
 #!/usr/bin/env python
-"""Times each hot-path kernel with CUDA events on device-resident data (two warm-up calls, then `reps` calls).  Usage: python tools/prof_driver.py [bc7|bc6h|bc15|bc3|dec|rows|rowscubic|rowslinear|rowshalf|all] [reps]"""
+"""Times each hot-path kernel with CUDA events on device-resident data (two warm-up calls, then `reps` calls).  Usage: python tools/prof_driver.py [bc7|bc7classes|bc6h|bc15|bc3|dec|rows|rowscubic|rowslinear|rowshalf|all] [reps]
+
+bc7classes: BC7 of a batch of 8 x 4096^2 RGBA32F images per LDR content class of synth, each image tiled from one 1024^2 image of
+that class, so that the batch runs on k_compress_bc7_tma.  The encoder's stages cost what the blocks' mode mix makes them cost,
+so a change to one stage is timed per class."""
 import ctypes as C
 import os
 import sys
@@ -56,6 +60,21 @@ if what in ("bc7", "all"):
     s = capi.images([capi.Image(w, h, 2, *F.compute_pitch(2, w, h), d_in.data_ptr())])
     d = capi.images([capi.Image(w, h, 98, *F.compute_pitch(98, w, h), d_out.data_ptr())])
     timed("bc7 4096^2 rgba32f", lambda: capi.lib.dxb200_compress_device(s, 1, 98, 0, 0.5, 1.0, d, st), w * h)
+
+if what == "bc7classes":
+    w = h = 4096
+    n = 8
+    d_out = torch.zeros(n * F.compute_pitch(98, w, h)[1], dtype=torch.uint8, device="cuda")
+    row, sl = F.compute_pitch(98, w, h)
+    d = capi.images([capi.Image(w, h, 98, row, sl, d_out.data_ptr() + i * sl) for i in range(n)])
+    srow, ssl = F.compute_pitch(2, w, h)
+    d_in = torch.zeros(n * ssl, dtype=torch.uint8, device="cuda")
+    s = capi.images([capi.Image(w, h, 2, srow, ssl, d_in.data_ptr() + i * ssl) for i in range(n)])     # constant stride: TMA-eligible
+    for kind in synth.LDR_CLASSES:
+        d_in.view(n, ssl)[:] = dev(np.tile(synth.content_ldr(kind, 1024, 1024, 5), (4, 4, 1)))
+        before = capi.kernel_launch_count("k_compress_bc7_tma")
+        timed("bc7 %-12s 8x4096^2" % kind, lambda: capi.lib.dxb200_compress_device(s, n, 98, 0, 0.5, 1.0, d, st), n * w * h)
+        assert capi.kernel_launch_count("k_compress_bc7_tma") > before, "the batch did not run k_compress_bc7_tma"
 
 if what in ("bc6h", "all"):
     w = h = 2048
