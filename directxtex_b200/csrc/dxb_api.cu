@@ -365,10 +365,6 @@ int32_t launch_compress(const CompressPlan& plan, const dxb200_image* src, const
 }
 
 // ---- host staging -------------------------------------------------------------------------------------
-// How one image of a staged item travels: its host pixels go up before the launch, its device result comes back after the
-// launch, or its bytes are only reserved in device memory (the levels of a chain that is compressed where it is built).
-enum class Copy : uint8_t { Up, Down, None };
-
 // One array of images of a staged call: item i owns images [i * per, (i + 1) * per) of `host`; image 0 of an item travels as
 // `first`, the others as `rest` (a mip chain uploads level 0 and makes the others).
 struct Plane { const dxb200_image* host; size_t per; Copy first, rest; };
@@ -676,100 +672,100 @@ struct ResultWords
 };
 
 // ---- [Decompress] -> [demultiply] -> [Resize] -> [channel steps] -> [Convert] -> [channel steps] -> GenerateMipMaps -> [coverage]
-// -> [premultiply] -> [BC3 layout] -> [Compress], chunk by chunk --------------------------------------------------------------------
-// texconv runs GenerateMipMaps and then Compress on the result (Texconv/texconv.cpp; SURVEY 3.5), after Decompress (:2316-2480) for
-// a BC input and Resize (:2576-2643) for a new size; with the host-pointer calls every intermediate travels device -> host ->
-// device.  Here each item's base goes up once, every step runs in device memory and only the packed blocks come back: 4 B/texel
-// up + 1.33 B/texel down for BC3 from RGBA8 instead of 4 + 5.33 + 5.33 + 1.33.  Chunks of whole items are pipelined over the
-// lane's NSLOT (stream, buffer) slots.  A chunk holds, per item and in plane order: the base as the caller laid it out (when a
-// device step reads it), the decompressed image (only when a resize follows), the pre-Convert level 0 (when a front step writes
-// it and a Convert follows), the chain (level 0 uploaded when no front step writes it and the output is compressed) and the blocks.
-// With no front step that is exactly the chain and the blocks.  Channel steps (fp.channels) run in place on every item's level 0
-// after the front steps or the upload, one launch per chunk and no plane of their own.  For an uncompressed output (mipmaps_
-// convert_from) the chain is the caller's dst, at its pitches, and every level comes back; the Convert writes its level 0 and the
-// later channel steps (fp.post) run in place there.  When no step writes that level 0 (no front step, no Convert), the uploaded
-// base is copied into it device to device.  With a scan (words != nullptr: one result word per item, see
-// dxb200_mipmaps_compress_from_ex) one more plane holds the items' words; they are cleared, set by one scan launch over all the
-// chunk's output after its last step, and come back with it.  Items that keep their own levels (cp.generate == false, levels_from)
-// stage the same planes with every level where the others hold level 0: every level of the base goes up, the front, channel and
-// Convert steps run on all of them, and no mip or coverage launch runs.  Each step is one launch per chunk over all its levels:
-// the kernels take mixed-size batches through the job tables.  That keeps a premultiply or a Convert off its vector kernel, which
-// needs equal jobs, yet per-level launches measured no faster (DESIGN.md §4).  A BC base that passes through is copied into dst like an
-// uncompressed one, row of blocks by row of blocks.  texconv's -alpha (fp.demultiply) is one premultiply launch per chunk in place on
-// the images Decompress wrote (or on the uploaded base), before Resize; its BC3n / RXGB layout (cp.layout) is one channel-steps launch
-// per chunk over every level of the chunk's chains, in place, before Compress.  Neither has a plane of its own.
-int32_t run_chains(const dxb200_image* base, size_t items, size_t levels, uint32_t filter, const FromPlan& fp, const dxb200_image* dst,
-                   const AlphaOpaquePlan& scan, const ResultWords* words)
+// -> [premultiply] -> [BC3 layout] -> [Compress] -> [IsAlphaAllOpaque], chunk by chunk --------------------------------------------
+// texconv runs each step as a separate call, so with the host-pointer calls every intermediate travels device -> host -> device.
+// Here each item's base goes up once, the steps of fp.chunk run in device memory and only the results come back: 4 B/texel up +
+// 1.33 B/texel down for BC3 from RGBA8 instead of 4 + 5.33 + 5.33 + 1.33.  Chunks of whole items are pipelined over the lane's
+// NSLOT (stream, buffer) slots.  Each step is one launch per chunk over all the images it covers: the kernels take mixed-size
+// batches through the job tables.  That keeps a Convert or a premultiply of kept levels off its vector kernel, which needs equal
+// jobs, yet per-level launches measured no faster (DESIGN.md §4); a generated chain's premultiply is one launch per level, whose
+// images are equal as the separate calls' are, so it takes the same kernel they do.  When no step writes the chain's level 0 (no
+// front step, no Convert), the uploaded base is copied into it device to device, at the chain's pitch; a BC base that passes
+// through is copied the same way, row of blocks by row of blocks.  *alphaAllOpaque (when given) = the answer of the scan, or of
+// its plan when nothing has to be scanned.
+int32_t run_chains(const dxb200_image* base, size_t items, size_t levels, const FromPlan& fp, const AlphaOpaquePlan& scan,
+                   const dxb200_image* dst, int32_t* alphaAllOpaque)
 {
     const ChainPlan& cp = fp.chain;
-    const bool front = fp.decompress || fp.resize, mid = fp.decompress && fp.resize, pre = front && fp.convert;
-    const bool up = !front && cp.compressed;                   // the chain's level 0 is uploaded; otherwise the base is
-    const size_t per = cp.generate ? 1 : levels;               // images per item that the steps in front of the mips act on
-    const Copy chainUp = up ? Copy::Up : Copy::None;
-    const std::vector<dxb200_image> wimg = words ? words->images() : std::vector<dxb200_image>();
-    return run_sharded(items, [&](size_t i) { return cp.chain[i * levels].slicePitch; },
+    const ChunkPlan& ck = fp.chunk;
+    ResultWords words;
+    int32_t hr = scan.scan ? words.alloc(items) : DXB_S_OK;
+    if (hr != DXB_S_OK) return hr;
+    const std::vector<dxb200_image> wimg = words.images();
+    const dxb200_image* host[PLANE_ROLES] = { base, fp.decompressed.data(), fp.level0.data(), cp.chain.data(), dst, wimg.data() };
+    size_t at[PLANE_ROLES] = {};                                // the plane of each staged role
+    for (size_t p = 0; p < ck.planes.size(); ++p) at[(size_t)ck.planes[p].role] = p;
+    hr = run_sharded(items, [&](size_t i) { return ck.weight[i]; },
         [&](size_t lo, size_t hi)
         {
             std::vector<Plane> planes;
-            if (!up) planes.push_back({ base + lo * per, per, Copy::Up, Copy::Up });
-            if (mid) planes.push_back({ fp.decompressed.data() + lo * per, per, Copy::None, Copy::None });
-            if (pre) planes.push_back({ fp.level0.data() + lo * per, per, Copy::None, Copy::None });
-            const size_t pc = planes.size();                    // the chains' plane, then the blocks' and the words'
-            if (cp.compressed) planes.push_back({ cp.chain.data() + lo * levels, levels, chainUp, cp.generate ? Copy::None : chainUp });
-            planes.push_back({ dst + lo * levels, levels, Copy::Down, Copy::Down });
-            if (words) planes.push_back({ wimg.data() + lo, 1, Copy::Down, Copy::Down });
+            for (const ChunkPlane& p : ck.planes) planes.push_back({ host[(size_t)p.role] + lo * p.per, p.per, p.first, p.rest });
             return run_staged(planes.data(), planes.size(), hi - lo, ITEM_CHUNK,
                 [&](const std::vector<dxb200_image>* dev, size_t cnt, cudaStream_t st)
                 {
-                    const dxb200_image* src = up ? nullptr : dev[0].data();
-                    const dxb200_image* decompressed = mid ? dev[1].data() : nullptr;
-                    const dxb200_image* chains = dev[pc].data();
-                    const dxb200_image* out = dev[cp.compressed ? pc + 1 : pc].data();
-                    int32_t h2 = DXB_S_OK;
-                    const size_t m = cnt * per;
+                    const size_t m = cnt * ck.per, all = cnt * levels;
                     std::vector<dxb200_image> level(m);
-                    for (size_t k = 0; k < m; ++k) level[k] = chains[k / per * levels + k % per];
-                    // the image the front steps write and the channel steps (the swizzle, with a Convert) run on
-                    const dxb200_image* first = pre ? dev[pc - 1].data() : fp.convert && !front ? src : level.data();
-                    if (fp.decompress) h2 = launch_decompress(fp.dp, src, mid ? decompressed : first, m, st);
-                    // -alpha, in place on what Decompress wrote, else on the base as it went up (a device copy)
-                    const dxb200_image* loaded = fp.decompress ? (mid ? decompressed : first) : up ? level.data() : src;
-                    if (h2 == DXB_S_OK && fp.demultiply) h2 = launch_pmalpha(fp.dm, loaded, loaded, m, st);
-                    if (h2 == DXB_S_OK && fp.resize) h2 = launch_resize(mid ? decompressed : src, first, m, fp.resizeFilter, fp.resizeMode, st);
-                    for (size_t k = 0; k < m && h2 == DXB_S_OK && !up && !front && !fp.convert; ++k)
+                    // the images of a plane a step covers; the Front of a plane of whole chains is gathered into `level`
+                    const auto images = [&](PlaneRole r, StepCover c) -> const dxb200_image*
                     {
-                        // the planned formats are implemented ones, so compute_pitch succeeds; rows of pixels or of blocks
-                        size_t row = 0, slice = 0;
-                        (void)compute_pitch(level[k].format, level[k].width, level[k].height, &row, &slice);
-                        const size_t rows = is_compressed(level[k].format) ? std::max<size_t>(1, (level[k].height + 3) / 4) : level[k].height;
-                        h2 = cuda_hr(cudaMemcpy2DAsync(level[k].pixels, level[k].rowPitch, src[k].pixels, src[k].rowPitch, row, rows,
-                                                       cudaMemcpyDeviceToDevice, st), "base -> level 0");
-                    }
-                    if (h2 == DXB_S_OK && fp.channels) h2 = launch_channel_steps(fp.cp, first, first, m, st);
-                    if (h2 == DXB_S_OK && fp.convert) h2 = launch_convert(fp.cv, first, level.data(), m, st);
-                    if (h2 == DXB_S_OK && fp.post) h2 = launch_channel_steps(fp.pp, level.data(), level.data(), m, st);
-                    if (h2 == DXB_S_OK && cp.generate) h2 = launch_mips(chains, cnt, levels, filter, cp.mode, st);
-                    if (h2 == DXB_S_OK && cp.coverage) h2 = launch_coverage(chains, chains, cnt, levels, cp.ref, st);
-                    // a generated chain premultiplies one launch per level: the chunk's images of a level are equal, as the separate
-                    // calls' images are, so they take the same premultiply kernel; kept levels already sit in `level`, one launch
-                    for (size_t l = 0; l < levels / per && h2 == DXB_S_OK && cp.premultiply; ++l)
+                        const std::vector<dxb200_image>& d = dev[at[(size_t)r]];
+                        if (c != StepCover::Front || ck.planes[at[(size_t)r]].per == ck.per) return d.data();
+                        for (size_t k = 0; k < m; ++k) level[k] = d[k / ck.per * levels + k % ck.per];
+                        return level.data();
+                    };
+                    int32_t h2 = DXB_S_OK;
+                    for (size_t i = 0; i < ck.steps.size() && h2 == DXB_S_OK; ++i)
                     {
-                        for (size_t it = 0; it < cnt && cp.generate; ++it) level[it] = chains[it * levels + l];
-                        h2 = launch_pmalpha(cp.pm, level.data(), level.data(), m, st);
-                    }
-                    if (h2 == DXB_S_OK && cp.layout) h2 = launch_channel_steps(cp.lp, chains, chains, cnt * levels, st);
-                    if (h2 == DXB_S_OK && cp.compressed) h2 = launch_compress(cp.compress, chains, out, cnt * levels, st);
-                    if (h2 == DXB_S_OK && words)
-                    {
-                        const std::vector<dxb200_image>& w = dev[planes.size() - 1];
-                        std::vector<dxb200_image> jobWords(cnt * levels);      // every level of an item sets the item's word
-                        for (size_t i = 0; i < jobWords.size(); ++i) jobWords[i] = w[i / levels];
-                        h2 = clear_words(w, st);
-                        if (h2 == DXB_S_OK) h2 = launch_alpha_opaque(scan, out, jobWords.data(), jobWords.size(), st);
+                        const ChunkStep& s = ck.steps[i];
+                        const dxb200_image* in = images(s.src, s.cover);
+                        const dxb200_image* out = images(s.dst, s.cover);
+                        const size_t n = s.cover == StepCover::Front ? m : all;
+                        switch (s.kind)
+                        {
+                        case StepKind::Decompress: h2 = launch_decompress(fp.dp, in, out, n, st); break;
+                        case StepKind::Demultiply: h2 = launch_pmalpha(fp.dm, in, out, n, st); break;
+                        case StepKind::Resize: h2 = launch_resize(in, out, n, fp.resizeFilter, fp.resizeMode, st); break;
+                        case StepKind::BaseCopy:
+                            for (size_t k = 0; k < n && h2 == DXB_S_OK; ++k)
+                            {
+                                // the planned formats are implemented ones, so compute_pitch succeeds; rows of pixels or of blocks
+                                size_t row = 0, slice = 0;
+                                (void)compute_pitch(out[k].format, out[k].width, out[k].height, &row, &slice);
+                                const size_t rows = is_compressed(out[k].format) ? std::max<size_t>(1, (out[k].height + 3) / 4) : out[k].height;
+                                h2 = cuda_hr(cudaMemcpy2DAsync(out[k].pixels, out[k].rowPitch, in[k].pixels, in[k].rowPitch, row, rows,
+                                                               cudaMemcpyDeviceToDevice, st), "base -> level 0");
+                            }
+                            break;
+                        case StepKind::Channels: h2 = launch_channel_steps(fp.cp, in, out, n, st); break;
+                        case StepKind::Convert: h2 = launch_convert(fp.cv, in, out, n, st); break;
+                        case StepKind::Post: h2 = launch_channel_steps(fp.pp, in, out, n, st); break;
+                        case StepKind::Mips: h2 = launch_mips(in, cnt, levels, ck.filter, cp.mode, st); break;
+                        case StepKind::Coverage: h2 = launch_coverage(in, out, cnt, levels, cp.ref, st); break;
+                        case StepKind::Premultiply:
+                            if (s.cover != StepCover::PerLevel) { h2 = launch_pmalpha(cp.pm, in, out, n, st); break; }
+                            for (size_t l = 0; l < levels && h2 == DXB_S_OK; ++l)
+                            {
+                                for (size_t it = 0; it < cnt; ++it) level[it] = in[it * levels + l];
+                                h2 = launch_pmalpha(cp.pm, level.data(), level.data(), cnt, st);
+                            }
+                            break;
+                        case StepKind::Layout: h2 = launch_channel_steps(cp.lp, in, out, n, st); break;
+                        case StepKind::Compress: h2 = launch_compress(cp.compress, in, out, n, st); break;
+                        case StepKind::Scan:
+                        {
+                            std::vector<dxb200_image> jobWords(n);      // every level of an item sets the item's word
+                            for (size_t k = 0; k < n; ++k) jobWords[k] = out[k / levels];
+                            h2 = clear_words(dev[at[(size_t)PlaneRole::Words]], st);
+                            if (h2 == DXB_S_OK) h2 = launch_alpha_opaque(scan, in, jobWords.data(), n, st);
+                            break;
+                        }
+                        }
                     }
                     return h2;
                 });
         });
+    if (hr == DXB_S_OK && alphaAllOpaque) *alphaAllOpaque = words.all_zero() ? 1 : 0;
+    return hr;
 }
 
 } // namespace
@@ -1024,15 +1020,10 @@ int32_t dxb200_mipmaps_compress_from_channels_ex(const dxb200_image* base, size_
 {
     (void)alphaWeight;
     FromPlan fp;
-    int32_t hr = plan_mipmaps_compress_channels(base, items, source, channels, levels, filter, steps, dstFormat, flags, threshold, dst, &fp, ts);
-    if (hr != DXB_S_OK) return hr;
-    AlphaOpaquePlan ap = {};
-    if (alphaAllOpaque && (hr = plan_alpha_opaque(dst, items * levels, alphaAllOpaque, &ap)) != DXB_S_OK) return hr;
-    ResultWords words;
-    if (ap.scan && (hr = words.alloc(items)) != DXB_S_OK) return hr;
-    hr = run_chains(base, items, levels, filter, fp, dst, ap, ap.scan ? &words : nullptr);
-    if (hr == DXB_S_OK && alphaAllOpaque) *alphaAllOpaque = (!ap.scan || words.all_zero()) ? 1 : 0;
-    return hr;
+    AlphaOpaquePlan ap;
+    const int32_t hr = plan_mipmaps_compress_channels(base, items, source, channels, levels, filter, steps, dstFormat, flags, threshold, dst,
+                                                      &fp, ts, alphaAllOpaque, &ap);
+    return hr != DXB_S_OK ? hr : run_chains(base, items, levels, fp, ap, dst, alphaAllOpaque);
 }
 
 int32_t dxb200_mipmaps_compress_from_channels(const dxb200_image* base, size_t items, const dxb200_chain_source* source,
@@ -1079,14 +1070,9 @@ int32_t dxb200_mipmaps_convert_from_ex(const dxb200_image* base, size_t items, c
 {
     FromPlan fp;
     AlphaOpaquePlan ap;
-    int32_t hr = plan_mipmaps_convert_from(base, items, source, channels, dstFormat, convertFilter, threshold, levels, filter, steps, dst,
-                                           alphaAllOpaque, &fp, &ap, ts);
-    if (hr != DXB_S_OK) return hr;
-    ResultWords words;
-    if (ap.scan && (hr = words.alloc(items)) != DXB_S_OK) return hr;
-    hr = run_chains(base, items, levels, filter, fp, dst, ap, ap.scan ? &words : nullptr);
-    if (hr == DXB_S_OK && alphaAllOpaque) *alphaAllOpaque = (!ap.scan || words.all_zero()) ? 1 : 0;
-    return hr;
+    const int32_t hr = plan_mipmaps_convert_from(base, items, source, channels, dstFormat, convertFilter, threshold, levels, filter, steps, dst,
+                                                 alphaAllOpaque, &fp, &ap, ts);
+    return hr != DXB_S_OK ? hr : run_chains(base, items, levels, fp, ap, dst, alphaAllOpaque);
 }
 
 int32_t dxb200_mipmaps_convert_from(const dxb200_image* base, size_t items, const dxb200_chain_source* source, const dxb200_channel_steps* channels,
@@ -1105,14 +1091,9 @@ int32_t dxb200_levels_from_ex(const dxb200_image* base, size_t items, size_t lev
 {
     FromPlan fp;
     AlphaOpaquePlan ap;
-    int32_t hr = plan_levels_from(base, items, levels, source, channels, dstFormat, convertFilter, compressFlags, threshold, steps, dst,
-                                  alphaAllOpaque, &fp, &ap, ts);
-    if (hr != DXB_S_OK) return hr;
-    ResultWords words;
-    if (ap.scan && (hr = words.alloc(items)) != DXB_S_OK) return hr;
-    hr = run_chains(base, items, levels, 0, fp, dst, ap, ap.scan ? &words : nullptr);
-    if (hr == DXB_S_OK && alphaAllOpaque) *alphaAllOpaque = (!ap.scan || words.all_zero()) ? 1 : 0;
-    return hr;
+    const int32_t hr = plan_levels_from(base, items, levels, source, channels, dstFormat, convertFilter, compressFlags, threshold, steps, dst,
+                                        alphaAllOpaque, &fp, &ap, ts);
+    return hr != DXB_S_OK ? hr : run_chains(base, items, levels, fp, ap, dst, alphaAllOpaque);
 }
 
 int32_t dxb200_levels_from(const dxb200_image* base, size_t items, size_t levels, const dxb200_chain_source* source,

@@ -483,13 +483,87 @@ uint32_t channel_decompress_format(uint32_t bcFormat, const dxb200_channel_steps
     return (bcFormat == DXB_FMT_BC4_SNORM || bcFormat == DXB_FMT_BC5_SNORM) ? DXB_FMT_R8G8B8A8_SNORM : DXB_FMT_R8G8B8A8_UNORM;
 }
 
+// ---- IsAlphaAllOpaque (DirectXTexImage.cpp:800-852; IsAlphaAllOpaqueBC, DirectXTexCompress.cpp:539-621) ---------------------
+// The reference's answer comes without a device when scan == false: a format without alpha is opaque, nothing is read.  Otherwise
+// every texel of every image has to be scanned: BC1 / BC2 / BC3 / BC7 blocks on k_decompress (blocks), any other implemented
+// format with alpha on k_convert.  Images of one call share one format; a null pixel pointer is E_POINTER whatever the format.
+struct AlphaOpaquePlan { bool scan, blocks; uint32_t format; };
+
+int32_t plan_alpha_opaque(const dxb200_image* images, size_t n, const int32_t* opaque, AlphaOpaquePlan* ap)
+{
+    ap->scan = ap->blocks = false; ap->format = 0;
+    if (!images || !opaque || !n) return DXB_E_INVALIDARG;
+    const uint32_t fmt = images[0].format;
+    for (size_t i = 0; i < n; ++i)
+    {
+        if (images[i].format != fmt) return DXB_E_INVALIDARG;
+        if (!images[i].pixels) return DXB_E_POINTER;
+    }
+    if (!dxb_has_alpha(fmt)) return DXB_S_OK;                                            // :805-806, no pixel is read
+    const bool blocks = is_compressed(fmt);
+    if (blocks ? !dxb_alpha_scan_blocks(fmt) : !is_supported_pixel_format(fmt)) return DXB_E_NOT_SUPPORTED;
+    for (size_t i = 0; i < n; ++i)
+    {
+        const dxb200_image& im = images[i];
+        if (!im.width || !im.height || im.width > 0xFFFFFFFFull || im.height > 0xFFFFFFFFull) return DXB_E_INVALIDARG;
+        if (!bc_pitch_ok(im)) return DXB_E_INVALIDARG;                                  // the rules of Decompress
+    }
+    ap->scan = true; ap->blocks = blocks; ap->format = fmt;
+    return DXB_S_OK;
+}
+
+// the parameters of the scan's launch over `units` work units of `njobs` jobs (dxb_alpha_opaque.h)
+dxb_compress_params alpha_opaque_block_params(const AlphaOpaquePlan& ap, uint32_t units, uint32_t njobs)
+{
+    dxb_compress_params P; memset(&P, 0, sizeof(P));
+    P.srcFormat = ap.format; P.dstFormat = DXB_SCAN_ALPHA_OPAQUE; P.inF = dxb_convert_flags(ap.format);
+    P.totalUnits = units; P.njobs = njobs;
+    return P;
+}
+dxb_convert_params alpha_opaque_pixel_params(const AlphaOpaquePlan& ap, uint32_t units, uint32_t njobs)
+{
+    dxb_convert_params P; memset(&P, 0, sizeof(P));
+    P.srcFormat = ap.format; P.dstFormat = DXB_SCAN_ALPHA_OPAQUE; P.inF = dxb_convert_flags(ap.format);
+    P.totalUnits = units; P.njobs = njobs;
+    return P;
+}
+
+// ---- what one chunk of a one-call pipeline stages and runs (run_chains) ------------------------------------------------------------
+// How one image of a staged item travels: its host pixels go up before the launch, its device result comes back after the
+// launch, or its bytes are only reserved in device memory (the levels of a chain that is compressed where it is built).
+enum class Copy : uint8_t { Up, Down, None };
+
+// The images a chunk can stage per item, one plane each: the caller's base, the decompressed image, level 0 in front of a Convert,
+// the chain, the caller's dst and the alpha scan's result word
+enum class PlaneRole : uint8_t { Base, Decompressed, Level0, Chain, Dst, Words };
+constexpr size_t PLANE_ROLES = 6;
+
+struct ChunkPlane { PlaneRole role; size_t per; Copy first, rest; };      // per = images per item; image 0 of an item travels as first
+
+// One kind per launch site of run_chains: Channels = the channel steps (with a Convert: the swizzle), Post = those after the Convert
+enum class StepKind : uint8_t { Decompress, Demultiply, Resize, BaseCopy, Channels, Convert, Post, Mips, Coverage, Premultiply, Layout,
+                                Compress, Scan };
+
+// The images of a plane a step covers: Front = the items' level 0 (every level when the items keep their levels), All = every
+// image, PerLevel = level l of every item, one launch per level
+enum class StepCover : uint8_t { Front, All, PerLevel };
+
+struct ChunkStep { StepKind kind; PlaneRole src, dst; StepCover cover; };
+
+struct ChunkPlan
+{
+    std::vector<ChunkPlane> planes;             // in the order the chunk's buffer holds them
+    std::vector<ChunkStep> steps;               // in texconv's order
+    size_t per;                                 // images per item a Front step covers: 1, or every level when the items keep theirs
+    uint32_t filter;                            // GenerateMipMaps' filter
+    std::vector<size_t> weight;                 // the bytes of each item's level 0 in the chain: the share of the items per device
+};
+
 // ---- Decompress -> Resize -> [channel steps] -> [Convert] -> [channel steps] -> mips ... [Compress] in one call ----------------
 // The per-item device images: base[i] (the caller's, BC or not, at its pitch), decompressed[i] (the base's size in the decompress
 // format at compute_pitch; in the buffer only when a resize follows, else it is level0[i]), level0[i] (what the front steps leave,
 // W x H at compute_pitch; the base when no front step runs), the chain and, for a compressed output, the blocks.  Images the device
-// makes carry base[i].pixels only for validation.  Without a Convert, level0[i] is level 0 of the chain: the channel steps run in
-// place on it.  With a Convert (mipmaps_convert_from), the swizzle runs in place on level0[i], the Convert writes level 0 of the
-// chain in the target format and the later steps (post) run in place there.
+// makes carry base[i].pixels only for validation.  Which of them a chunk stages and which steps read and write them: chunk.
 struct FromPlan
 {
     bool decompress, demultiply, resize, channels, convert, post;
@@ -502,7 +576,57 @@ struct FromPlan
     dxb_convert_params cv;                      // the Convert
     dxb_convert_params pp;                      // colour key, invert Y and reconstruct Z after the Convert
     ChainPlan chain;
+    ChunkPlan chunk;                            // plan_chunk's, once every check has passed
 };
+
+// The planners' last step: IsAlphaAllOpaque of dst (when alphaAllOpaque != nullptr), then the planes and steps of a chunk.  A
+// front step (Decompress or Resize) leaves level 0 in the chain (L: the chain's plane, or dst's for an uncompressed output), or in
+// level 0 in front of a Convert; without one, the base goes up where a step reads it, else the chain's level 0 does (up).
+int32_t plan_chunk(const dxb200_image* dst, size_t items, size_t levels, uint32_t filter, const int32_t* alphaAllOpaque, FromPlan* fp,
+                   AlphaOpaquePlan* ap)
+{
+    if (alphaAllOpaque)
+        if (const int32_t hr = plan_alpha_opaque(dst, items * levels, alphaAllOpaque, ap)) return hr;
+    const ChainPlan& cp = fp->chain;
+    ChunkPlan& ck = fp->chunk;
+    using R = PlaneRole;
+    using S = StepKind;
+    const bool front = fp->decompress || fp->resize, mid = fp->decompress && fp->resize, pre = front && fp->convert;
+    const bool up = !front && cp.compressed;
+    const R L = cp.compressed ? R::Chain : R::Dst;
+    const R W = pre ? R::Level0 : fp->convert && !front ? R::Base : L;        // what the front steps write, the channel steps run on
+    const R D = mid ? R::Decompressed : W;                                      // what the Decompress writes
+    const R DM = fp->decompress ? D : up ? L : R::Base;                         // what the demultiply runs on
+    const Copy chainUp = up ? Copy::Up : Copy::None;
+    ck.per = cp.generate ? 1 : levels;
+    ck.filter = filter;
+    ck.planes.clear();
+    if (!up) ck.planes.push_back({ R::Base, ck.per, Copy::Up, Copy::Up });
+    if (mid) ck.planes.push_back({ R::Decompressed, ck.per, Copy::None, Copy::None });
+    if (pre) ck.planes.push_back({ R::Level0, ck.per, Copy::None, Copy::None });
+    if (cp.compressed) ck.planes.push_back({ R::Chain, levels, chainUp, cp.generate ? Copy::None : chainUp });
+    ck.planes.push_back({ R::Dst, levels, Copy::Down, Copy::Down });
+    if (ap->scan) ck.planes.push_back({ R::Words, 1, Copy::Down, Copy::Down });
+    ck.steps.clear();
+    const auto step = [&](bool on, S kind, R src, R dst, StepCover cover) { if (on) ck.steps.push_back({ kind, src, dst, cover }); };
+    const StepCover F = StepCover::Front, A = StepCover::All;
+    step(fp->decompress, S::Decompress, R::Base, D, F);
+    step(fp->demultiply, S::Demultiply, DM, DM, F);
+    step(fp->resize, S::Resize, mid ? R::Decompressed : R::Base, W, F);
+    step(!up && !front && !fp->convert, S::BaseCopy, R::Base, L, F);
+    step(fp->channels, S::Channels, W, W, F);
+    step(fp->convert, S::Convert, W, L, F);
+    step(fp->post, S::Post, L, L, F);
+    step(cp.generate, S::Mips, L, L, A);
+    step(cp.coverage, S::Coverage, L, L, A);
+    step(cp.premultiply, S::Premultiply, L, L, cp.generate ? StepCover::PerLevel : F);
+    step(cp.layout, S::Layout, L, L, A);
+    step(cp.compressed, S::Compress, R::Chain, R::Dst, A);
+    step(ap->scan, S::Scan, R::Dst, R::Words, A);
+    ck.weight.resize(items);
+    for (size_t i = 0; i < items; ++i) ck.weight[i] = cp.chain[i * levels].slicePitch;
+    return DXB_S_OK;
+}
 
 // image i of `n` of format fmt, w x h, at compute_pitch, with the pixels of base[i]
 std::vector<dxb200_image> plan_images(const dxb200_image* base, size_t n, uint32_t fmt, size_t w, size_t h)
@@ -556,28 +680,36 @@ int32_t plan_front(const dxb200_image* base, size_t items, const dxb200_chain_so
 }
 
 // Every check of Decompress, -alpha's demultiply, Resize, the channel steps and the steps of plan_mipmaps_compress before anything is
-// uploaded, each with the HRESULT of the first of the separate calls that would fail; check_texconv_steps comes before all of them.
-// source == nullptr, or a source that changes nothing, channels == nullptr, or no channel step enabled, and ts == nullptr, or all
-// zeros = plan_mipmaps_compress.
+// uploaded, each with the HRESULT of the first of the separate calls that would fail; check_texconv_steps comes before all of them,
+// IsAlphaAllOpaque of dst (when alphaAllOpaque != nullptr) after them.  source == nullptr, or a source that changes nothing,
+// channels == nullptr, or no channel step enabled, and ts == nullptr, or all zeros = plan_mipmaps_compress.
 int32_t plan_mipmaps_compress_channels(const dxb200_image* base, size_t items, const dxb200_chain_source* source, const dxb200_channel_steps* channels,
                                        size_t levels, uint32_t filter, const dxb200_chain_steps* steps, uint32_t dstFormat, uint32_t flags,
-                                       float threshold, const dxb200_image* dst, FromPlan* fp, const dxb200_texconv_steps* ts = nullptr)
+                                       float threshold, const dxb200_image* dst, FromPlan* fp, const dxb200_texconv_steps* ts = nullptr,
+                                       const int32_t* alphaAllOpaque = nullptr, AlphaOpaquePlan* ap = nullptr)
 {
+    AlphaOpaquePlan none;
+    if (!ap) ap = &none;
+    ap->scan = ap->blocks = false; ap->format = 0;
     fp->decompress = fp->demultiply = fp->resize = fp->channels = fp->convert = fp->post = false;
     fp->resizeFilter = fp->resizeMode = 0;
     fp->decompressed.clear();
     int32_t hr = check_texconv_steps(ts, dstFormat, true);
     if (hr != DXB_S_OK) return hr;
     const bool ch = channels && channel_steps_word(*channels);
+    const dxb200_image* level0 = base;
     if ((!source && !ch && !(ts && ts->demultiply)) || !base || !items)
-    {
         fp->level0.clear();
-        return plan_mipmaps_compress(base, items, levels, filter, steps, dstFormat, flags, threshold, dst, &fp->chain, bc3_layout(ts));
+    else
+    {
+        if ((hr = plan_front(base, items, source, channels, fp, ts)) != DXB_S_OK) return hr;
+        if (ch && (hr = plan_channel_steps(fp->level0.data(), items, channels, fp->level0.data(), &fp->cp)) != DXB_S_OK) return hr;
+        fp->channels = ch;
+        level0 = fp->level0.data();
     }
-    if ((hr = plan_front(base, items, source, channels, fp, ts)) != DXB_S_OK) return hr;
-    if (ch && (hr = plan_channel_steps(fp->level0.data(), items, channels, fp->level0.data(), &fp->cp)) != DXB_S_OK) return hr;
-    fp->channels = ch;
-    return plan_mipmaps_compress(fp->level0.data(), items, levels, filter, steps, dstFormat, flags, threshold, dst, &fp->chain, bc3_layout(ts));
+    if ((hr = plan_mipmaps_compress(level0, items, levels, filter, steps, dstFormat, flags, threshold, dst, &fp->chain, bc3_layout(ts))) != DXB_S_OK)
+        return hr;
+    return plan_chunk(dst, items, levels, filter, alphaAllOpaque, fp, ap);
 }
 
 int32_t plan_mipmaps_compress_from(const dxb200_image* base, size_t items, const dxb200_chain_source* source, size_t levels, uint32_t filter,
@@ -585,51 +717,6 @@ int32_t plan_mipmaps_compress_from(const dxb200_image* base, size_t items, const
                                    FromPlan* fp)
 {
     return plan_mipmaps_compress_channels(base, items, source, nullptr, levels, filter, steps, dstFormat, flags, threshold, dst, fp);
-}
-
-// ---- IsAlphaAllOpaque (DirectXTexImage.cpp:800-852; IsAlphaAllOpaqueBC, DirectXTexCompress.cpp:539-621) ---------------------
-// The reference's answer comes without a device when scan == false: a format without alpha is opaque, nothing is read.  Otherwise
-// every texel of every image has to be scanned: BC1 / BC2 / BC3 / BC7 blocks on k_decompress (blocks), any other implemented
-// format with alpha on k_convert.  Images of one call share one format; a null pixel pointer is E_POINTER whatever the format.
-struct AlphaOpaquePlan { bool scan, blocks; uint32_t format; };
-
-int32_t plan_alpha_opaque(const dxb200_image* images, size_t n, const int32_t* opaque, AlphaOpaquePlan* ap)
-{
-    ap->scan = ap->blocks = false; ap->format = 0;
-    if (!images || !opaque || !n) return DXB_E_INVALIDARG;
-    const uint32_t fmt = images[0].format;
-    for (size_t i = 0; i < n; ++i)
-    {
-        if (images[i].format != fmt) return DXB_E_INVALIDARG;
-        if (!images[i].pixels) return DXB_E_POINTER;
-    }
-    if (!dxb_has_alpha(fmt)) return DXB_S_OK;                                            // :805-806, no pixel is read
-    const bool blocks = is_compressed(fmt);
-    if (blocks ? !dxb_alpha_scan_blocks(fmt) : !is_supported_pixel_format(fmt)) return DXB_E_NOT_SUPPORTED;
-    for (size_t i = 0; i < n; ++i)
-    {
-        const dxb200_image& im = images[i];
-        if (!im.width || !im.height || im.width > 0xFFFFFFFFull || im.height > 0xFFFFFFFFull) return DXB_E_INVALIDARG;
-        if (!bc_pitch_ok(im)) return DXB_E_INVALIDARG;                                  // the rules of Decompress
-    }
-    ap->scan = true; ap->blocks = blocks; ap->format = fmt;
-    return DXB_S_OK;
-}
-
-// the parameters of the scan's launch over `units` work units of `njobs` jobs (dxb_alpha_opaque.h)
-dxb_compress_params alpha_opaque_block_params(const AlphaOpaquePlan& ap, uint32_t units, uint32_t njobs)
-{
-    dxb_compress_params P; memset(&P, 0, sizeof(P));
-    P.srcFormat = ap.format; P.dstFormat = DXB_SCAN_ALPHA_OPAQUE; P.inF = dxb_convert_flags(ap.format);
-    P.totalUnits = units; P.njobs = njobs;
-    return P;
-}
-dxb_convert_params alpha_opaque_pixel_params(const AlphaOpaquePlan& ap, uint32_t units, uint32_t njobs)
-{
-    dxb_convert_params P; memset(&P, 0, sizeof(P));
-    P.srcFormat = ap.format; P.dstFormat = DXB_SCAN_ALPHA_OPAQUE; P.inF = dxb_convert_flags(ap.format);
-    P.totalUnits = units; P.njobs = njobs;
-    return P;
 }
 
 // ---- the channel steps around a Convert ------------------------------------------------------------------------------------------
@@ -733,7 +820,7 @@ int32_t plan_mipmaps_convert_from(const dxb200_image* base, size_t items, const 
     if ((hr = plan_chain_steps(items, levels, filter, steps, &fp->chain)) != DXB_S_OK) return hr;
     for (size_t i = 0; i < items && levels; ++i) chain[i * levels] = dst[i * levels];
     fp->chain.compressed = false;
-    return alphaAllOpaque ? plan_alpha_opaque(dst, items * levels, alphaAllOpaque, ap) : DXB_S_OK;
+    return plan_chunk(dst, items, levels, filter, alphaAllOpaque, fp, ap);
 }
 
 // ---- texconv on items that keep their own levels (levels_from): Decompress -> [Resize] -> swizzle -> Convert -> later channel steps
@@ -797,7 +884,7 @@ int32_t plan_levels_from(const dxb200_image* base, size_t items, size_t levels, 
     if (cp.compressed && (hr = plan_compress(out, n, dstFormat, compressFlags, threshold, dst, &cp.compress)) != DXB_S_OK) return hr;
     const bool copy = !fp->decompress && !fp->resize && !fp->convert && !cp.compressed;
     if (copy && (hr = plan_copy(base, n)) != DXB_S_OK) return hr;
-    return alphaAllOpaque ? plan_alpha_opaque(dst, n, alphaAllOpaque, ap) : DXB_S_OK;
+    return plan_chunk(dst, items, levels, 0, alphaAllOpaque, fp, ap);
 }
 
 } // namespace

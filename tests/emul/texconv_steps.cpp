@@ -1,7 +1,7 @@
 // tests/emul/texconv_steps.cpp — TEST INFRASTRUCTURE, never shipped: the planners of dxb200_mipmaps_compress_from_channels_ex,
 // dxb200_mipmaps_convert_from_ex and dxb200_levels_from_ex (dxb_plan.h) on the host, with the entry points' own signatures, so that
 // the CPU suite can hold their HRESULTs against the library's without a device.  Each also reports the plan a valid call would
-// stage.
+// stage, and emul_chunk_plan the planes and steps of its chunks.
 #include <cstdint>
 #include <cstddef>
 #include <cstring>
@@ -28,6 +28,21 @@ static void report(const FromPlan& fp, const AlphaOpaquePlan& ap, const dxb200_i
     out[16] = ap.scan;
 }
 
+// the chunk plan of the last valid call (run_chains' planes and steps), for emul_chunk_plan
+static ChunkPlan last;
+
+// out = { plane count, step count, per, filter, item 0's weight, then { role, per, first copy, rest copy } of every plane and
+// { kind, source role, destination role, cover } of every step }; returns the words written, at most cap
+extern "C" size_t emul_chunk_plan(uint64_t* out, size_t cap)
+{
+    std::vector<uint64_t> w = { last.planes.size(), last.steps.size(), last.per, last.filter, last.weight.empty() ? 0 : last.weight[0] };
+    for (const ChunkPlane& p : last.planes) w.insert(w.end(), { (uint64_t)p.role, p.per, (uint64_t)p.first, (uint64_t)p.rest });
+    for (const ChunkStep& s : last.steps) w.insert(w.end(), { (uint64_t)s.kind, (uint64_t)s.src, (uint64_t)s.dst, (uint64_t)s.cover });
+    const size_t n = std::min(w.size(), cap);
+    std::copy(w.begin(), w.begin() + n, out);
+    return n;
+}
+
 // out (may be NULL, NOUT words) filled on S_OK
 extern "C" int32_t emul_plan_compress_from_channels_ex(const dxb200_image* base, size_t items, const dxb200_chain_source* source,
                                                        const dxb200_channel_steps* channels, size_t levels, uint32_t filter,
@@ -37,10 +52,11 @@ extern "C" int32_t emul_plan_compress_from_channels_ex(const dxb200_image* base,
 {
     (void)alphaWeight;
     FromPlan fp;
-    AlphaOpaquePlan ap = {};
-    int32_t hr = plan_mipmaps_compress_channels(base, items, source, channels, levels, filter, steps, dstFormat, flags, threshold, dst, &fp, ts);
-    if (hr == DXB_S_OK && alphaAllOpaque) hr = plan_alpha_opaque(dst, items * levels, alphaAllOpaque, &ap);     // as the entry point
+    AlphaOpaquePlan ap;
+    const int32_t hr = plan_mipmaps_compress_channels(base, items, source, channels, levels, filter, steps, dstFormat, flags, threshold, dst,
+                                                      &fp, ts, alphaAllOpaque, &ap);
     if (hr == DXB_S_OK && out) report(fp, ap, base, out);
+    if (hr == DXB_S_OK) last = fp.chunk;
     return hr;
 }
 
@@ -54,6 +70,7 @@ extern "C" int32_t emul_plan_convert_from_ex(const dxb200_image* base, size_t it
     const int32_t hr = plan_mipmaps_convert_from(base, items, source, channels, dstFormat, convertFilter, threshold, levels, filter, steps, dst,
                                                  alphaAllOpaque, &fp, &ap, ts);
     if (hr == DXB_S_OK && out) report(fp, ap, base, out);
+    if (hr == DXB_S_OK) last = fp.chunk;
     return hr;
 }
 
@@ -67,5 +84,6 @@ extern "C" int32_t emul_plan_levels_from_ex(const dxb200_image* base, size_t ite
     const int32_t hr = plan_levels_from(base, items, levels, source, channels, dstFormat, convertFilter, compressFlags, threshold, steps, dst,
                                         alphaAllOpaque, &fp, &ap, ts);
     if (hr == DXB_S_OK && out) report(fp, ap, base, out);
+    if (hr == DXB_S_OK) last = fp.chunk;
     return hr;
 }
