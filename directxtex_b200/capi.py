@@ -18,7 +18,7 @@ SYMBOLS = [
     "dxb200_is_alpha_all_opaque", "dxb200_is_alpha_all_opaque_device",
     "dxb200_apply_channel_steps", "dxb200_apply_channel_steps_device", "dxb200_mipmaps_compress_from_channels",
     "dxb200_mipmaps_convert_from", "dxb200_levels_from",
-    "dxb200_mipmaps_compress_from_channels_ex", "dxb200_mipmaps_convert_from_ex", "dxb200_levels_from_ex",
+    "dxb200_mipmaps_compress_from_channels_ex", "dxb200_mipmaps_convert_from_ex", "dxb200_levels_from_ex", "dxb200_texconv_batch",
     "dxb200_dds_encode_header", "dxb200_dds_save_memory", "dxb200_dds_get_metadata", "dxb200_dds_load_memory",
 ]
 
@@ -54,6 +54,15 @@ class ChannelSteps(C.Structure):
 class TexconvSteps(C.Structure):
     """dxb200_texconv_steps: texconv's -alpha (demultiply) and -f BC3n / RXGB (bc3Layout 1 / 2) steps."""
     _fields_ = [("demultiply", C.c_uint32), ("demultiplyFlags", C.c_uint32), ("bc3Layout", C.c_uint32)]
+
+
+class TexconvJob(C.Structure):
+    """dxb200_texconv_job: one texture of dxb200_texconv_batch, the arguments of the call named by kind (0 =
+    dxb200_mipmaps_compress_from_channels_ex, 1 = dxb200_mipmaps_convert_from_ex, 2 = dxb200_levels_from_ex)."""
+    _fields_ = [("kind", C.c_uint32), ("base", C.POINTER(Image)), ("items", C.c_size_t), ("levels", C.c_size_t),
+                ("source", C.POINTER(ChainSource)), ("channels", C.POINTER(ChannelSteps)), ("filter", C.c_uint32),
+                ("steps", C.POINTER(ChainSteps)), ("ts", C.POINTER(TexconvSteps)), ("dstFormat", C.c_uint32), ("convertFilter", C.c_uint32),
+                ("compressFlags", C.c_uint32), ("threshold", C.c_float), ("dst", C.POINTER(Image)), ("alphaAllOpaque", C.POINTER(C.c_int32))]
 
 
 STATUS_FN = C.CFUNCTYPE(C.c_int, C.c_size_t, C.c_size_t, C.c_void_p)      # dxb200_status_fn
@@ -107,6 +116,8 @@ def _load():
     lib.dxb200_mipmaps_compress_from_channels_ex.argtypes = lib.dxb200_mipmaps_compress_from_channels.argtypes + [TP]
     lib.dxb200_mipmaps_convert_from_ex.argtypes = lib.dxb200_mipmaps_convert_from.argtypes + [TP]
     lib.dxb200_levels_from_ex.argtypes = lib.dxb200_levels_from.argtypes + [TP]
+    lib.dxb200_texconv_batch.argtypes = [C.POINTER(TexconvJob), C.c_size_t, C.POINTER(C.c_int32)]
+    lib.dxb200_texconv_batch.restype = C.c_int32
     lib.dxb200_apply_channel_steps.argtypes = [IP, C.c_size_t, C.POINTER(ChannelSteps), IP]
     lib.dxb200_apply_channel_steps_device.argtypes = [IP, C.c_size_t, C.POINTER(ChannelSteps), IP, C.c_void_p]
     lib.dxb200_is_alpha_all_opaque.argtypes = [IP, C.c_size_t, C.POINTER(C.c_int32)]
@@ -305,11 +316,13 @@ def mipmaps_compress_from_channels(bases, w, h, base_fmt, dst_fmt, source=None, 
     return outs, opaque.value == 1
 
 
-def mipmaps_convert_from(bases, w, h, base_fmt, dst_fmt, source=None, channels=None, convert_filter=0, threshold=0.5, filter=0, levels=0,
-                         steps=None, texconv=None):
-    """dxb200_mipmaps_convert_from_ex of an array of equally sized w x h host images of base_fmt (BC or not) into dst_fmt chains,
-    with the ChainSource `source`, the ChannelSteps `channels`, the ChainSteps `steps` and the TexconvSteps `texconv` (None: none):
-    (one chain per image, laid out as texture_layout(dst_fmt, W, H, 1, levels), IsAlphaAllOpaque of the output as a bool)"""
+def _ref(x):
+    return C.pointer(x) if x is not None else None
+
+
+def _convert_args(bases, w, h, base_fmt, dst_fmt, source=None, channels=None, convert_filter=0, threshold=0.5, filter=0, levels=0,
+                  steps=None, texconv=None):
+    """(the dxb200_texconv_job of mipmaps_convert_from's call, without alphaAllOpaque; the output arrays; what the job points to)"""
     bases = [np.ascontiguousarray(a).view(np.uint8).reshape(-1) for a in bases]
     cw, ch = (source.width, source.height) if source is not None and source.width else (w, h)
     levels = levels or F.count_mips(cw, ch)
@@ -317,14 +330,37 @@ def mipmaps_convert_from(bases, w, h, base_fmt, dst_fmt, source=None, channels=N
     outs = [np.zeros(total, np.uint8) for _ in bases]
     s = images([make_image(_np_ptr(a), w, h, base_fmt) for a in bases])
     d = images([Image(lw, lh, dst_fmt, r, sp, _np_ptr(o) + off) for o in outs for (off, lw, lh, r, sp) in olayout])
+    job = TexconvJob(1, s, len(bases), levels, _ref(source), _ref(channels), filter, _ref(steps), _ref(texconv), dst_fmt, convert_filter, 0,
+                     threshold, d, None)
+    return job, outs, (bases, s, d, source, channels, steps, texconv)
+
+
+def mipmaps_convert_from(bases, w, h, base_fmt, dst_fmt, source=None, channels=None, convert_filter=0, threshold=0.5, filter=0, levels=0,
+                         steps=None, texconv=None):
+    """dxb200_mipmaps_convert_from_ex of an array of equally sized w x h host images of base_fmt (BC or not) into dst_fmt chains,
+    with the ChainSource `source`, the ChannelSteps `channels`, the ChainSteps `steps` and the TexconvSteps `texconv` (None: none):
+    (one chain per image, laid out as texture_layout(dst_fmt, W, H, 1, levels), IsAlphaAllOpaque of the output as a bool)"""
+    j, outs, _keep = _convert_args(bases, w, h, base_fmt, dst_fmt, source, channels, convert_filter, threshold, filter, levels, steps, texconv)
     opaque = C.c_int32(-1)
-    hr = lib.dxb200_mipmaps_convert_from_ex(s, len(bases), C.byref(source) if source is not None else None,
-                                            C.byref(channels) if channels is not None else None, dst_fmt, convert_filter, threshold, levels,
-                                            filter, C.byref(steps) if steps is not None else None, d, C.byref(opaque),
-                                            C.byref(texconv) if texconv is not None else None)
+    hr = lib.dxb200_mipmaps_convert_from_ex(j.base, j.items, j.source, j.channels, j.dstFormat, j.convertFilter, j.threshold, j.levels,
+                                            j.filter, j.steps, j.dst, C.byref(opaque), j.ts)
     if hr != 0:
         raise DxTexError(hr, "dxb200_mipmaps_convert_from_ex")
     return outs, opaque.value == 1
+
+
+def _levels_args(bases, sizes, base_fmt, dst_fmt, source=None, channels=None, convert_filter=0, compress_flags=0, threshold=0.5, steps=None,
+                 texconv=None):
+    """(the dxb200_texconv_job of levels_from's call, without alphaAllOpaque; the output arrays; what the job points to)"""
+    levels = len(sizes)
+    osizes = [(source.width, source.height)] if levels == 1 and source is not None and source.width else list(sizes)
+    bases = [[np.ascontiguousarray(a).view(np.uint8).reshape(-1) for a in item] for item in bases]
+    outs = [[np.zeros(F.compute_pitch(dst_fmt, w, h)[1], np.uint8) for (w, h) in osizes] for _ in bases]
+    s = images([make_image(_np_ptr(a), w, h, base_fmt) for item in bases for a, (w, h) in zip(item, sizes)])
+    d = images([make_image(_np_ptr(o), w, h, dst_fmt) for item in outs for o, (w, h) in zip(item, osizes)])
+    job = TexconvJob(2, s, len(bases), levels, _ref(source), _ref(channels), 0, _ref(steps), _ref(texconv), dst_fmt, convert_filter,
+                     compress_flags, threshold, d, None)
+    return job, outs, (bases, s, d, source, channels, steps, texconv)
 
 
 def levels_from(bases, sizes, base_fmt, dst_fmt, source=None, channels=None, convert_filter=0, compress_flags=0, threshold=0.5,
@@ -332,20 +368,39 @@ def levels_from(bases, sizes, base_fmt, dst_fmt, source=None, channels=None, con
     """dxb200_levels_from_ex of items that keep their own levels: bases[i][l] = level l of item i (host, tight, of base_fmt, BC or
     not), (w, h) = sizes[l] for every item; the ChainSource `source`, the ChannelSteps `channels`, the ChainSteps `steps` and the
     TexconvSteps `texconv` (None: none).  Returns (outs[i][l] = that level in dst_fmt, tight; IsAlphaAllOpaque of the output as a bool)."""
-    levels = len(sizes)
-    osizes = [(source.width, source.height)] if levels == 1 and source is not None and source.width else list(sizes)
-    bases = [[np.ascontiguousarray(a).view(np.uint8).reshape(-1) for a in item] for item in bases]
-    outs = [[np.zeros(F.compute_pitch(dst_fmt, w, h)[1], np.uint8) for (w, h) in osizes] for _ in bases]
-    s = images([make_image(_np_ptr(a), w, h, base_fmt) for item in bases for a, (w, h) in zip(item, sizes)])
-    d = images([make_image(_np_ptr(o), w, h, dst_fmt) for item in outs for o, (w, h) in zip(item, osizes)])
+    j, outs, _keep = _levels_args(bases, sizes, base_fmt, dst_fmt, source, channels, convert_filter, compress_flags, threshold, steps, texconv)
     opaque = C.c_int32(-1)
-    hr = lib.dxb200_levels_from_ex(s, len(bases), levels, C.byref(source) if source is not None else None,
-                                   C.byref(channels) if channels is not None else None, dst_fmt, convert_filter, compress_flags, threshold,
-                                   C.byref(steps) if steps is not None else None, d, C.byref(opaque),
-                                   C.byref(texconv) if texconv is not None else None)
+    hr = lib.dxb200_levels_from_ex(j.base, j.items, j.levels, j.source, j.channels, j.dstFormat, j.convertFilter, j.compressFlags,
+                                   j.threshold, j.steps, j.dst, C.byref(opaque), j.ts)
     if hr != 0:
         raise DxTexError(hr, "dxb200_levels_from_ex")
     return outs, opaque.value == 1
+
+
+def _compress_args(bases, w, h, base_fmt, dst_fmt, source=None, channels=None, filter=0, levels=0, flags=0, steps=None, row_pitch=0,
+                   texconv=None):
+    """(the dxb200_texconv_job of mipmaps_compress_from_channels' call, without alphaAllOpaque; the output arrays; what it points to)"""
+    args, outs = _from_args(bases, w, h, base_fmt, dst_fmt, source, filter, levels, flags, steps, row_pitch)
+    s, n, _, levels, filter, _, dst_fmt, flags, threshold, _, d = args
+    job = TexconvJob(0, s, n, levels, _ref(source), _ref(channels), filter, _ref(steps), _ref(texconv), dst_fmt, 0, flags, threshold, d, None)
+    return job, outs, (s, d, source, channels, steps, texconv)
+
+
+TEXCONV_KINDS = {"compress": _compress_args, "convert": _convert_args, "levels": _levels_args}
+
+
+def texconv_batch(jobs):
+    """dxb200_texconv_batch of a list of (kind, kwargs): kind "compress" takes mipmaps_compress_from_channels' arguments, "convert"
+    mipmaps_convert_from's and "levels" levels_from's.  Returns (the batch's HRESULT, [(HRESULT, outputs as the helper returns them,
+    IsAlphaAllOpaque as a bool) per job])."""
+    built = [TEXCONV_KINDS[kind](**kw) for kind, kw in jobs]
+    opaque = [C.c_int32(-1) for _ in built]
+    for (j, _, _), o in zip(built, opaque):
+        j.alphaAllOpaque = C.pointer(o)
+    table = (TexconvJob * len(built))(*[j for j, _, _ in built])
+    results = (C.c_int32 * len(built))()
+    hr = lib.dxb200_texconv_batch(table, len(built), results)
+    return F.hr_u32(hr), [(F.hr_u32(results[i]), built[i][1], opaque[i].value == 1) for i in range(len(built))]
 
 
 def apply_channel_steps(arrays, w, h, fmt, channels, row_pitch=0):

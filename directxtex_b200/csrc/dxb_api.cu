@@ -18,6 +18,7 @@
 #include <condition_variable>
 #include <memory>
 #include <thread>
+#include <functional>
 #include <unistd.h>
 #include <sys/syscall.h>
 #include <vector>
@@ -225,18 +226,7 @@ int32_t run_sharded(size_t n, WeightFn weight, Fn fn)
         hr = sc.enter(devs[0]);
         return hr != DXB_S_OK ? hr : fn(size_t(0), n);
     }
-    double total = 0;
-    for (size_t i = 0; i < n; ++i) total += (double)weight(i);
-    std::vector<size_t> cut(nd + 1, n);
-    cut[0] = 0;
-    {
-        double acc = 0; size_t d = 1;
-        for (size_t i = 0; i < n && d < nd; ++i)
-        {
-            acc += (double)weight(i);
-            while (d < nd && acc >= total * (double)d / (double)nd) cut[d++] = i + 1;
-        }
-    }
+    const std::vector<size_t> cut = shard_cuts(n, nd, weight);
     std::vector<int32_t> hrs(nd, DXB_S_OK);
     std::vector<std::string> errs(nd);
     auto work = [&](size_t d)
@@ -369,67 +359,79 @@ int32_t launch_compress(const CompressPlan& plan, const dxb200_image* src, const
 // `first`, the others as `rest` (a mip chain uploads level 0 and makes the others).
 struct Plane { const dxb200_image* host; size_t per; Copy first, rest; };
 
-// Stages items [0, n) of the planes through the calling thread's lane.  Whole items are grouped into chunks of at most `budget`
-// bytes of device memory (an item larger than that is a chunk by itself), and chunk c goes through slot c % NSLOT, so the H2D
-// copies, kernels and D2H copies of consecutive chunks overlap (fully when the caller's memory is pinned, see
-// dxb200_host_alloc).  In the slot's buffer the chunk's images lie plane after plane, each on a 256-byte boundary, so equal
-// images of one plane sit at a constant stride (the vector kernels' alignment checks and the BC7 TMA feed rely on both).
-// fn(dev, count, stream) enqueues the kernels: dev[p] is plane p's images of the chunk's `count` items, with device pointers.
-// prog (optional) is told before each chunk's upload the units[] of the items the chunk completes, and stops the call between
-// chunks (E_ABORT).  Every slot is synchronised before returning; the first error wins.
-template <typename Fn>
-int32_t run_staged(const Plane* planes, size_t nplanes, size_t n, size_t budget, Fn fn, Progress* prog = nullptr, const size_t* units = nullptr)
+// fn(dev, count, stream) of a staged segment: enqueues the kernels of one chunk; dev[p] is plane p's images of the chunk's `count`
+// items, with device pointers
+using StageFn = std::function<int32_t(const std::vector<dxb200_image>*, size_t, cudaStream_t)>;
+
+// items [0, n) of `nplanes` planes, staged with their own launch function
+struct Segment { const Plane* planes; size_t nplanes; size_t n; StageFn fn; };
+
+// Stages the items of every segment, in order, through the calling thread's lane.  Whole items of one segment are grouped into
+// chunks of at most `budget` bytes of device memory (an item larger than that is a chunk by itself; a chunk never spans two
+// segments), and chunk c of the call goes through slot c % NSLOT, so the H2D copies, kernels and D2H copies of consecutive chunks
+// overlap, from one segment to the next too (fully when the caller's memory is pinned, see dxb200_host_alloc).  In the slot's
+// buffer the chunk's images lie plane after plane, each on a 256-byte boundary, so equal images of one plane sit at a constant
+// stride (the vector kernels' alignment checks and the BC7 TMA feed rely on both).  prog (optional) is told before each chunk's
+// upload the units[] of the items the chunk completes (units counts the items of all segments in order), and stops the call
+// between chunks (E_ABORT).  Every slot is synchronised once, before returning; the first error wins.
+int32_t run_segments(const Segment* segs, size_t nsegs, size_t budget, Progress* prog = nullptr, const size_t* units = nullptr)
 {
     auto padded = [](const dxb200_image& im) { return (im.slicePitch + 255) & ~size_t(255); };
     Lane& L = *t_v.lane;
-    std::vector<std::vector<dxb200_image>> dev(nplanes);
-    size_t i = 0; int slot = 0;
+    int slot = 0;
     int32_t hr = DXB_S_OK;
-    while (i < n && hr == DXB_S_OK)
+    for (size_t sg = 0; sg < nsegs && hr == DXB_S_OK; units += units ? segs[sg].n : 0, ++sg)
     {
-        size_t bytes = 0, k = i;
-        while (k < n)
+        const Plane* planes = segs[sg].planes;
+        const size_t nplanes = segs[sg].nplanes, n = segs[sg].n;
+        std::vector<std::vector<dxb200_image>> dev(nplanes);
+        size_t i = 0;
+        while (i < n && hr == DXB_S_OK)
         {
-            size_t b = 0;
-            for (size_t p = 0; p < nplanes; ++p)
-                for (size_t m = k * planes[p].per; m < (k + 1) * planes[p].per; ++m) b += padded(planes[p].host[m]);
-            if (k > i && bytes + b > budget) break;
-            bytes += b; ++k;
-        }
-        cudaStream_t st = L.streams[slot];
-        hr = cuda_hr(cudaStreamSynchronize(st), "slot sync"); if (hr) break;
-        if (prog)
-        {
-            size_t add = 0;
-            for (size_t m = i; m < k; ++m) add += units[m];
-            if (!prog->report(add)) { hr = DXB_E_ABORT; break; }
-        }
-        hr = ensure_buffer(&L.buf[slot], &L.cap[slot], bytes); if (hr) break;
-        size_t off = 0;
-        for (size_t p = 0; p < nplanes && hr == DXB_S_OK; ++p)
-        {
-            const Plane& pl = planes[p];
-            const dxb200_image* host = pl.host + i * pl.per;
-            dev[p].assign(host, pl.host + k * pl.per);
-            for (size_t m = 0; m < dev[p].size() && hr == DXB_S_OK; ++m)
+            size_t bytes = 0, k = i;
+            while (k < n)
             {
-                dev[p][m].pixels = static_cast<uint8_t*>(L.buf[slot]) + off;
-                off += padded(dev[p][m]);
-                if ((m % pl.per ? pl.rest : pl.first) == Copy::Up)
-                    hr = cuda_hr(cudaMemcpyAsync(dev[p][m].pixels, host[m].pixels, host[m].slicePitch, cudaMemcpyHostToDevice, st), "H2D");
+                size_t b = 0;
+                for (size_t p = 0; p < nplanes; ++p)
+                    for (size_t m = k * planes[p].per; m < (k + 1) * planes[p].per; ++m) b += padded(planes[p].host[m]);
+                if (k > i && bytes + b > budget) break;
+                bytes += b; ++k;
             }
+            cudaStream_t st = L.streams[slot];
+            hr = cuda_hr(cudaStreamSynchronize(st), "slot sync"); if (hr) break;
+            if (prog)
+            {
+                size_t add = 0;
+                for (size_t m = i; m < k; ++m) add += units[m];
+                if (!prog->report(add)) { hr = DXB_E_ABORT; break; }
+            }
+            hr = ensure_buffer(&L.buf[slot], &L.cap[slot], bytes); if (hr) break;
+            size_t off = 0;
+            for (size_t p = 0; p < nplanes && hr == DXB_S_OK; ++p)
+            {
+                const Plane& pl = planes[p];
+                const dxb200_image* host = pl.host + i * pl.per;
+                dev[p].assign(host, pl.host + k * pl.per);
+                for (size_t m = 0; m < dev[p].size() && hr == DXB_S_OK; ++m)
+                {
+                    dev[p][m].pixels = static_cast<uint8_t*>(L.buf[slot]) + off;
+                    off += padded(dev[p][m]);
+                    if ((m % pl.per ? pl.rest : pl.first) == Copy::Up)
+                        hr = cuda_hr(cudaMemcpyAsync(dev[p][m].pixels, host[m].pixels, host[m].slicePitch, cudaMemcpyHostToDevice, st), "H2D");
+                }
+            }
+            if (hr) break;
+            hr = segs[sg].fn(dev.data(), k - i, st); if (hr) break;
+            for (size_t p = 0; p < nplanes && hr == DXB_S_OK; ++p)
+            {
+                const Plane& pl = planes[p];
+                const dxb200_image* host = pl.host + i * pl.per;
+                for (size_t m = 0; m < dev[p].size() && hr == DXB_S_OK; ++m)
+                    if ((m % pl.per ? pl.rest : pl.first) == Copy::Down)
+                        hr = cuda_hr(cudaMemcpyAsync(host[m].pixels, dev[p][m].pixels, host[m].slicePitch, cudaMemcpyDeviceToHost, st), "D2H");
+            }
+            i = k; slot = (slot + 1) % NSLOT;
         }
-        if (hr) break;
-        hr = fn(dev.data(), k - i, st); if (hr) break;
-        for (size_t p = 0; p < nplanes && hr == DXB_S_OK; ++p)
-        {
-            const Plane& pl = planes[p];
-            const dxb200_image* host = pl.host + i * pl.per;
-            for (size_t m = 0; m < dev[p].size() && hr == DXB_S_OK; ++m)
-                if ((m % pl.per ? pl.rest : pl.first) == Copy::Down)
-                    hr = cuda_hr(cudaMemcpyAsync(host[m].pixels, dev[p][m].pixels, host[m].slicePitch, cudaMemcpyDeviceToHost, st), "D2H");
-        }
-        i = k; slot = (slot + 1) % NSLOT;
     }
     for (int s = 0; s < NSLOT; ++s)
     {
@@ -437,6 +439,13 @@ int32_t run_staged(const Plane* planes, size_t nplanes, size_t n, size_t budget,
         if (hr == DXB_S_OK) hr = h2;
     }
     return hr;
+}
+
+// run_segments of one segment
+int32_t run_staged(const Plane* planes, size_t nplanes, size_t n, size_t budget, StageFn fn, Progress* prog = nullptr, const size_t* units = nullptr)
+{
+    const Segment seg = { planes, nplanes, n, std::move(fn) };
+    return run_segments(&seg, 1, budget, prog, units);
 }
 
 // Band calls cut host images into BANDS of whole work rows (4 pixel rows per block row on the BC side) of about BAND_BYTES.
@@ -671,6 +680,82 @@ struct ResultWords
     bool all_zero() const { return std::all_of(w, w + n, [](uint32_t v) { return v == 0; }); }
 };
 
+// The staged planes of items [lo, ...) of a chunk plan: host[r] = the host images of role r, ck.planes[p].per per item
+std::vector<Plane> chain_planes(const ChunkPlan& ck, const dxb200_image* const* host, size_t lo)
+{
+    std::vector<Plane> planes;
+    for (const ChunkPlane& p : ck.planes) planes.push_back({ host[(size_t)p.role] + lo * p.per, p.per, p.first, p.rest });
+    return planes;
+}
+
+// The launches of one chunk of `cnt` items of fp.chunk: dev[p] = plane p's device images
+int32_t run_chunk(const FromPlan& fp, const AlphaOpaquePlan& scan, size_t levels, const std::vector<dxb200_image>* dev, size_t cnt, cudaStream_t st)
+{
+    const ChainPlan& cp = fp.chain;
+    const ChunkPlan& ck = fp.chunk;
+    size_t at[PLANE_ROLES] = {};                                // the plane of each staged role
+    for (size_t p = 0; p < ck.planes.size(); ++p) at[(size_t)ck.planes[p].role] = p;
+    const size_t m = cnt * ck.per, all = cnt * levels;
+    std::vector<dxb200_image> level(m);
+    // the images of a plane a step covers; the Front of a plane of whole chains is gathered into `level`
+    const auto images = [&](PlaneRole r, StepCover c) -> const dxb200_image*
+    {
+        const std::vector<dxb200_image>& d = dev[at[(size_t)r]];
+        if (c != StepCover::Front || ck.planes[at[(size_t)r]].per == ck.per) return d.data();
+        for (size_t k = 0; k < m; ++k) level[k] = d[k / ck.per * levels + k % ck.per];
+        return level.data();
+    };
+    int32_t h2 = DXB_S_OK;
+    for (size_t i = 0; i < ck.steps.size() && h2 == DXB_S_OK; ++i)
+    {
+        const ChunkStep& s = ck.steps[i];
+        const dxb200_image* in = images(s.src, s.cover);
+        const dxb200_image* out = images(s.dst, s.cover);
+        const size_t n = s.cover == StepCover::Front ? m : all;
+        switch (s.kind)
+        {
+        case StepKind::Decompress: h2 = launch_decompress(fp.dp, in, out, n, st); break;
+        case StepKind::Demultiply: h2 = launch_pmalpha(fp.dm, in, out, n, st); break;
+        case StepKind::Resize: h2 = launch_resize(in, out, n, fp.resizeFilter, fp.resizeMode, st); break;
+        case StepKind::BaseCopy:
+            for (size_t k = 0; k < n && h2 == DXB_S_OK; ++k)
+            {
+                // the planned formats are implemented ones, so compute_pitch succeeds; rows of pixels or of blocks
+                size_t row = 0, slice = 0;
+                (void)compute_pitch(out[k].format, out[k].width, out[k].height, &row, &slice);
+                const size_t rows = is_compressed(out[k].format) ? std::max<size_t>(1, (out[k].height + 3) / 4) : out[k].height;
+                h2 = cuda_hr(cudaMemcpy2DAsync(out[k].pixels, out[k].rowPitch, in[k].pixels, in[k].rowPitch, row, rows,
+                                               cudaMemcpyDeviceToDevice, st), "base -> level 0");
+            }
+            break;
+        case StepKind::Channels: h2 = launch_channel_steps(fp.cp, in, out, n, st); break;
+        case StepKind::Convert: h2 = launch_convert(fp.cv, in, out, n, st); break;
+        case StepKind::Post: h2 = launch_channel_steps(fp.pp, in, out, n, st); break;
+        case StepKind::Mips: h2 = launch_mips(in, cnt, levels, ck.filter, cp.mode, st); break;
+        case StepKind::Coverage: h2 = launch_coverage(in, out, cnt, levels, cp.ref, st); break;
+        case StepKind::Premultiply:
+            if (s.cover != StepCover::PerLevel) { h2 = launch_pmalpha(cp.pm, in, out, n, st); break; }
+            for (size_t l = 0; l < levels && h2 == DXB_S_OK; ++l)
+            {
+                for (size_t it = 0; it < cnt; ++it) level[it] = in[it * levels + l];
+                h2 = launch_pmalpha(cp.pm, level.data(), level.data(), cnt, st);
+            }
+            break;
+        case StepKind::Layout: h2 = launch_channel_steps(cp.lp, in, out, n, st); break;
+        case StepKind::Compress: h2 = launch_compress(cp.compress, in, out, n, st); break;
+        case StepKind::Scan:
+        {
+            std::vector<dxb200_image> jobWords(n);      // every level of an item sets the item's word
+            for (size_t k = 0; k < n; ++k) jobWords[k] = out[k / levels];
+            h2 = clear_words(dev[at[(size_t)PlaneRole::Words]], st);
+            if (h2 == DXB_S_OK) h2 = launch_alpha_opaque(scan, in, jobWords.data(), n, st);
+            break;
+        }
+        }
+    }
+    return h2;
+}
+
 // ---- [Decompress] -> [demultiply] -> [Resize] -> [channel steps] -> [Convert] -> [channel steps] -> GenerateMipMaps -> [coverage]
 // -> [premultiply] -> [BC3 layout] -> [Compress] -> [IsAlphaAllOpaque], chunk by chunk --------------------------------------------
 // texconv runs each step as a separate call, so with the host-pointer calls every intermediate travels device -> host -> device.
@@ -686,86 +771,85 @@ struct ResultWords
 int32_t run_chains(const dxb200_image* base, size_t items, size_t levels, const FromPlan& fp, const AlphaOpaquePlan& scan,
                    const dxb200_image* dst, int32_t* alphaAllOpaque)
 {
-    const ChainPlan& cp = fp.chain;
     const ChunkPlan& ck = fp.chunk;
     ResultWords words;
     int32_t hr = scan.scan ? words.alloc(items) : DXB_S_OK;
     if (hr != DXB_S_OK) return hr;
     const std::vector<dxb200_image> wimg = words.images();
-    const dxb200_image* host[PLANE_ROLES] = { base, fp.decompressed.data(), fp.level0.data(), cp.chain.data(), dst, wimg.data() };
-    size_t at[PLANE_ROLES] = {};                                // the plane of each staged role
-    for (size_t p = 0; p < ck.planes.size(); ++p) at[(size_t)ck.planes[p].role] = p;
+    const dxb200_image* host[PLANE_ROLES] = { base, fp.decompressed.data(), fp.level0.data(), fp.chain.chain.data(), dst, wimg.data() };
     hr = run_sharded(items, [&](size_t i) { return ck.weight[i]; },
         [&](size_t lo, size_t hi)
         {
-            std::vector<Plane> planes;
-            for (const ChunkPlane& p : ck.planes) planes.push_back({ host[(size_t)p.role] + lo * p.per, p.per, p.first, p.rest });
+            const std::vector<Plane> planes = chain_planes(ck, host, lo);
             return run_staged(planes.data(), planes.size(), hi - lo, ITEM_CHUNK,
-                [&](const std::vector<dxb200_image>* dev, size_t cnt, cudaStream_t st)
-                {
-                    const size_t m = cnt * ck.per, all = cnt * levels;
-                    std::vector<dxb200_image> level(m);
-                    // the images of a plane a step covers; the Front of a plane of whole chains is gathered into `level`
-                    const auto images = [&](PlaneRole r, StepCover c) -> const dxb200_image*
-                    {
-                        const std::vector<dxb200_image>& d = dev[at[(size_t)r]];
-                        if (c != StepCover::Front || ck.planes[at[(size_t)r]].per == ck.per) return d.data();
-                        for (size_t k = 0; k < m; ++k) level[k] = d[k / ck.per * levels + k % ck.per];
-                        return level.data();
-                    };
-                    int32_t h2 = DXB_S_OK;
-                    for (size_t i = 0; i < ck.steps.size() && h2 == DXB_S_OK; ++i)
-                    {
-                        const ChunkStep& s = ck.steps[i];
-                        const dxb200_image* in = images(s.src, s.cover);
-                        const dxb200_image* out = images(s.dst, s.cover);
-                        const size_t n = s.cover == StepCover::Front ? m : all;
-                        switch (s.kind)
-                        {
-                        case StepKind::Decompress: h2 = launch_decompress(fp.dp, in, out, n, st); break;
-                        case StepKind::Demultiply: h2 = launch_pmalpha(fp.dm, in, out, n, st); break;
-                        case StepKind::Resize: h2 = launch_resize(in, out, n, fp.resizeFilter, fp.resizeMode, st); break;
-                        case StepKind::BaseCopy:
-                            for (size_t k = 0; k < n && h2 == DXB_S_OK; ++k)
-                            {
-                                // the planned formats are implemented ones, so compute_pitch succeeds; rows of pixels or of blocks
-                                size_t row = 0, slice = 0;
-                                (void)compute_pitch(out[k].format, out[k].width, out[k].height, &row, &slice);
-                                const size_t rows = is_compressed(out[k].format) ? std::max<size_t>(1, (out[k].height + 3) / 4) : out[k].height;
-                                h2 = cuda_hr(cudaMemcpy2DAsync(out[k].pixels, out[k].rowPitch, in[k].pixels, in[k].rowPitch, row, rows,
-                                                               cudaMemcpyDeviceToDevice, st), "base -> level 0");
-                            }
-                            break;
-                        case StepKind::Channels: h2 = launch_channel_steps(fp.cp, in, out, n, st); break;
-                        case StepKind::Convert: h2 = launch_convert(fp.cv, in, out, n, st); break;
-                        case StepKind::Post: h2 = launch_channel_steps(fp.pp, in, out, n, st); break;
-                        case StepKind::Mips: h2 = launch_mips(in, cnt, levels, ck.filter, cp.mode, st); break;
-                        case StepKind::Coverage: h2 = launch_coverage(in, out, cnt, levels, cp.ref, st); break;
-                        case StepKind::Premultiply:
-                            if (s.cover != StepCover::PerLevel) { h2 = launch_pmalpha(cp.pm, in, out, n, st); break; }
-                            for (size_t l = 0; l < levels && h2 == DXB_S_OK; ++l)
-                            {
-                                for (size_t it = 0; it < cnt; ++it) level[it] = in[it * levels + l];
-                                h2 = launch_pmalpha(cp.pm, level.data(), level.data(), cnt, st);
-                            }
-                            break;
-                        case StepKind::Layout: h2 = launch_channel_steps(cp.lp, in, out, n, st); break;
-                        case StepKind::Compress: h2 = launch_compress(cp.compress, in, out, n, st); break;
-                        case StepKind::Scan:
-                        {
-                            std::vector<dxb200_image> jobWords(n);      // every level of an item sets the item's word
-                            for (size_t k = 0; k < n; ++k) jobWords[k] = out[k / levels];
-                            h2 = clear_words(dev[at[(size_t)PlaneRole::Words]], st);
-                            if (h2 == DXB_S_OK) h2 = launch_alpha_opaque(scan, in, jobWords.data(), n, st);
-                            break;
-                        }
-                        }
-                    }
-                    return h2;
-                });
+                [&](const std::vector<dxb200_image>* dev, size_t cnt, cudaStream_t st) { return run_chunk(fp, scan, levels, dev, cnt, st); });
         });
     if (hr == DXB_S_OK && alphaAllOpaque) *alphaAllOpaque = words.all_zero() ? 1 : 0;
     return hr;
+}
+
+// dxb200_texconv_batch once every job is planned: group g's items are units bp.firstUnit[g] .. firstUnit[g + 1], split over the
+// devices by run_sharded; each device stages its units of every group as one segment per group, through one lane, with the launches
+// of the group's first job's plan (equal to every member's).  The alpha answer of a job is the AND of its items' words.
+int32_t run_batch(const dxb200_texconv_job* jobs, const BatchPlan& bp)
+{
+    const size_t ng = bp.groups.size(), units = bp.firstUnit.back();
+    bool scan = false;
+    for (const std::vector<size_t>& members : bp.groups) scan |= bp.ap[members[0]].scan;
+    ResultWords words;
+    int32_t hr = scan ? words.alloc(units) : DXB_S_OK;
+    if (hr != DXB_S_OK) return hr;
+    const std::vector<dxb200_image> wimg = words.images();
+    // the host images of every role of every group: its jobs' images in job order
+    std::vector<std::vector<dxb200_image>> roles(ng * PLANE_ROLES);
+    std::vector<const dxb200_image*> host(ng * PLANE_ROLES, nullptr);
+    for (size_t g = 0; g < ng; ++g)
+    {
+        for (size_t j : bp.groups[g])
+        {
+            const FromPlan& fp = bp.fp[j];
+            const size_t n = jobs[j].items * fp.chunk.per, all = jobs[j].items * jobs[j].levels;
+            std::vector<dxb200_image>* r = &roles[g * PLANE_ROLES];
+            r[(size_t)PlaneRole::Base].insert(r[(size_t)PlaneRole::Base].end(), jobs[j].base, jobs[j].base + n);
+            r[(size_t)PlaneRole::Decompressed].insert(r[(size_t)PlaneRole::Decompressed].end(), fp.decompressed.begin(), fp.decompressed.end());
+            r[(size_t)PlaneRole::Level0].insert(r[(size_t)PlaneRole::Level0].end(), fp.level0.begin(), fp.level0.end());
+            r[(size_t)PlaneRole::Chain].insert(r[(size_t)PlaneRole::Chain].end(), fp.chain.chain.begin(), fp.chain.chain.end());
+            r[(size_t)PlaneRole::Dst].insert(r[(size_t)PlaneRole::Dst].end(), jobs[j].dst, jobs[j].dst + all);
+        }
+        for (size_t r = 0; r < PLANE_ROLES; ++r) host[g * PLANE_ROLES + r] = roles[g * PLANE_ROLES + r].data();
+        if (scan) host[g * PLANE_ROLES + (size_t)PlaneRole::Words] = wimg.data() + bp.firstUnit[g];
+    }
+    hr = run_sharded(units, [&](size_t i) { return bp.weight[i]; },
+        [&](size_t lo, size_t hi)
+        {
+            std::vector<std::vector<Plane>> planes(ng);
+            std::vector<Segment> segs;
+            for (size_t g = 0; g < ng; ++g)
+            {
+                const size_t a = std::max(lo, bp.firstUnit[g]), b = std::min(hi, bp.firstUnit[g + 1]);
+                if (a >= b) continue;
+                const size_t j = bp.groups[g][0];
+                const FromPlan& fp = bp.fp[j];
+                const size_t levels = jobs[j].levels;
+                planes[g] = chain_planes(fp.chunk, &host[g * PLANE_ROLES], a - bp.firstUnit[g]);
+                segs.push_back({ planes[g].data(), planes[g].size(), b - a,
+                                 [&fp, &bp, j, levels](const std::vector<dxb200_image>* dev, size_t cnt, cudaStream_t st)
+                                 { return run_chunk(fp, bp.ap[j], levels, dev, cnt, st); } });
+            }
+            return run_segments(segs.data(), segs.size(), ITEM_CHUNK);
+        });
+    if (hr != DXB_S_OK) return hr;
+    for (size_t g = 0; g < ng; ++g)
+    {
+        size_t u = bp.firstUnit[g];
+        for (size_t j : bp.groups[g])
+        {
+            const bool opaque = !bp.ap[j].scan || std::all_of(words.w + u, words.w + u + jobs[j].items, [](uint32_t v) { return v == 0; });
+            if (jobs[j].alphaAllOpaque) *jobs[j].alphaAllOpaque = opaque ? 1 : 0;
+            u += jobs[j].items;
+        }
+    }
+    return DXB_S_OK;
 }
 
 } // namespace
@@ -1102,6 +1186,20 @@ int32_t dxb200_levels_from(const dxb200_image* base, size_t items, size_t levels
 {
     return dxb200_levels_from_ex(base, items, levels, source, channels, dstFormat, convertFilter, compressFlags, threshold, steps, dst,
                                  alphaAllOpaque, nullptr);
+}
+
+// ---- texconv over a list of textures: the jobs planned first, then every group's units sharded and staged (run_batch) ----------
+int32_t dxb200_texconv_batch(const dxb200_texconv_job* jobs, size_t njobs, int32_t* results)
+{
+    if (!jobs || !njobs) return DXB_E_INVALIDARG;
+    BatchPlan bp;
+    (void)plan_texconv_batch(jobs, njobs, &bp);          // each job's HRESULT is in bp.hr
+    if (!bp.groups.empty())
+        if (const int32_t hr = run_batch(jobs, bp))
+            for (size_t i = 0; i < njobs; ++i) if (bp.group[i] != SIZE_MAX) bp.hr[i] = hr;
+    if (results) std::copy(bp.hr.begin(), bp.hr.end(), results);
+    for (int32_t hr : bp.hr) if (hr != DXB_S_OK) return hr;
+    return DXB_S_OK;
 }
 
 int32_t dxb200_premultiply_alpha_device(const dxb200_image* src, size_t nimages, uint32_t flags, const dxb200_image* dst, void* stream)

@@ -887,4 +887,148 @@ int32_t plan_levels_from(const dxb200_image* base, size_t items, size_t levels, 
     return plan_chunk(dst, items, levels, 0, alphaAllOpaque, fp, ap);
 }
 
+// ---- how a host call splits its units over the devices (run_sharded) -------------------------------------------------------------
+// cut[d] .. cut[d + 1] = the contiguous units of device d, nd = min(devices, max(n, 1)): device d's range ends at the first unit
+// where the running weight reaches d / nd of the total
+template <typename WeightFn>
+std::vector<size_t> shard_cuts(size_t n, size_t devices, WeightFn weight)
+{
+    const size_t nd = std::min(devices, std::max<size_t>(n, 1));
+    std::vector<size_t> cut(nd + 1, n);
+    cut[0] = 0;
+    double total = 0;
+    for (size_t i = 0; i < n; ++i) total += (double)weight(i);
+    double acc = 0; size_t d = 1;
+    for (size_t i = 0; i < n && d < nd; ++i)
+    {
+        acc += (double)weight(i);
+        while (d < nd && acc >= total * (double)d / (double)nd) cut[d++] = i + 1;
+    }
+    return cut;
+}
+
+// ---- texconv over a list of textures (dxb200_texconv_batch) ----------------------------------------------------------------------
+// Job i planned by the planner of its kind, exactly as the single call plans it
+int32_t plan_texconv_job(const dxb200_texconv_job& j, FromPlan* fp, AlphaOpaquePlan* ap)
+{
+    switch (j.kind)
+    {
+    case 0:
+        return plan_mipmaps_compress_channels(j.base, j.items, j.source, j.channels, j.levels, j.filter, j.steps, j.dstFormat, j.compressFlags,
+                                              j.threshold, j.dst, fp, j.ts, j.alphaAllOpaque, ap);
+    case 1:
+        return plan_mipmaps_convert_from(j.base, j.items, j.source, j.channels, j.dstFormat, j.convertFilter, j.threshold, j.levels, j.filter,
+                                         j.steps, j.dst, j.alphaAllOpaque, fp, ap, j.ts);
+    case 2:
+        return plan_levels_from(j.base, j.items, j.levels, j.source, j.channels, j.dstFormat, j.convertFilter, j.compressFlags, j.threshold,
+                                j.steps, j.dst, j.alphaAllOpaque, fp, ap, j.ts);
+    default:
+        return DXB_E_INVALIDARG;
+    }
+}
+
+// the parameter records are all 4-byte fields and every planned record starts from a zeroed FromPlan, so equal records compare equal
+template <typename T>
+bool same_bytes(const T& a, const T& b) { return memcmp(&a, &b, sizeof(T)) == 0; }
+
+bool same_images(const dxb200_image* a, const dxb200_image* b, size_t n)
+{
+    for (size_t i = 0; i < n; ++i)
+        if (a[i].format != b[i].format || a[i].width != b[i].width || a[i].height != b[i].height) return false;
+    return true;
+}
+
+// The launches two valid jobs' chunks run are the same when their plans are equal apart from image pointers and row pitches
+bool same_plan(const dxb200_texconv_job& ja, const FromPlan& a, const AlphaOpaquePlan& sa, const dxb200_texconv_job& jb, const FromPlan& b,
+               const AlphaOpaquePlan& sb)
+{
+    const ChainPlan& ca = a.chain; const ChainPlan& cb = b.chain;
+    const ChunkPlan& ka = a.chunk; const ChunkPlan& kb = b.chunk;
+    if (ja.kind != jb.kind || ja.levels != jb.levels) return false;
+    if (a.decompress != b.decompress || a.demultiply != b.demultiply || a.resize != b.resize || a.channels != b.channels ||
+        a.convert != b.convert || a.post != b.post || a.resizeFilter != b.resizeFilter || a.resizeMode != b.resizeMode)
+        return false;
+    if (!same_bytes(a.dp, b.dp) || !same_bytes(a.dm, b.dm) || !same_bytes(a.cp, b.cp) || !same_bytes(a.cv, b.cv) || !same_bytes(a.pp, b.pp))
+        return false;
+    if (ca.generate != cb.generate || ca.mode != cb.mode || ca.coverage != cb.coverage || ca.ref != cb.ref || ca.premultiply != cb.premultiply ||
+        ca.layout != cb.layout || ca.compressed != cb.compressed || !same_bytes(ca.pm, cb.pm) || !same_bytes(ca.lp, cb.lp) ||
+        !same_bytes(ca.compress.P, cb.compress.P) || ca.compress.bc7 != cb.compress.bc7 || ca.compress.bc6h != cb.compress.bc6h)
+        return false;
+    if (ka.per != kb.per || ka.filter != kb.filter || ka.planes.size() != kb.planes.size() || ka.steps.size() != kb.steps.size()) return false;
+    for (size_t p = 0; p < ka.planes.size(); ++p)
+        if (ka.planes[p].role != kb.planes[p].role || ka.planes[p].per != kb.planes[p].per || ka.planes[p].first != kb.planes[p].first ||
+            ka.planes[p].rest != kb.planes[p].rest)
+            return false;
+    for (size_t s = 0; s < ka.steps.size(); ++s)
+        if (ka.steps[s].kind != kb.steps[s].kind || ka.steps[s].src != kb.steps[s].src || ka.steps[s].dst != kb.steps[s].dst ||
+            ka.steps[s].cover != kb.steps[s].cover)
+            return false;
+    return sa.scan == sb.scan && sa.blocks == sb.blocks && sa.format == sb.format;
+}
+
+// every item of a valid job has the formats and sizes of item `it` of job j: its base images (ck.per each) and its dst images
+bool item_shape_is(const dxb200_texconv_job& a, const ChunkPlan& ck, const dxb200_texconv_job& j, size_t it)
+{
+    for (size_t i = 0; i < a.items; ++i)
+        if (!same_images(a.base + i * ck.per, j.base + it * ck.per, ck.per) || !same_images(a.dst + i * a.levels, j.dst + it * j.levels, j.levels))
+            return false;
+    return true;
+}
+
+// The plan of a batch: every job's HRESULT and plan; the groups of valid jobs, in the order of their first job, each a list of
+// jobs in job order whose items run as the items of one call of that kind; the units, (group, item) in that order, with the bytes
+// each weighs when the units are split over the devices (the items' chunk weights); result = the lowest-index job's failure.
+struct BatchPlan
+{
+    std::vector<int32_t> hr;
+    std::vector<FromPlan> fp;
+    std::vector<AlphaOpaquePlan> ap;
+    std::vector<size_t> group;                  // of each job; SIZE_MAX for a job that failed its checks
+    std::vector<std::vector<size_t>> groups;
+    std::vector<size_t> firstUnit;              // of each group, and the total unit count last
+    std::vector<size_t> weight;                 // of each unit
+    int32_t result = DXB_S_OK;
+};
+
+int32_t plan_texconv_batch(const dxb200_texconv_job* jobs, size_t njobs, BatchPlan* bp)
+{
+    if (!jobs || !njobs) return DXB_E_INVALIDARG;
+    bp->hr.assign(njobs, DXB_S_OK);
+    bp->fp.assign(njobs, FromPlan());
+    bp->ap.assign(njobs, AlphaOpaquePlan());
+    bp->group.assign(njobs, SIZE_MAX);
+    bp->groups.clear(); bp->firstUnit.clear(); bp->weight.clear();
+    bp->result = DXB_S_OK;
+    for (size_t i = 0; i < njobs; ++i)
+    {
+        bp->hr[i] = plan_texconv_job(jobs[i], &bp->fp[i], &bp->ap[i]);
+        if (bp->hr[i] != DXB_S_OK)
+        {
+            if (bp->result == DXB_S_OK) bp->result = bp->hr[i];
+            continue;
+        }
+        const ChunkPlan& ck = bp->fp[i].chunk;
+        // a job whose items differ in shape runs as a group of its own
+        const bool uniform = item_shape_is(jobs[i], ck, jobs[i], 0);
+        size_t g = 0;
+        for (; uniform && g < bp->groups.size(); ++g)
+        {
+            const size_t j = bp->groups[g][0];
+            if (same_plan(jobs[j], bp->fp[j], bp->ap[j], jobs[i], bp->fp[i], bp->ap[i]) && item_shape_is(jobs[j], ck, jobs[j], 0) &&
+                item_shape_is(jobs[i], ck, jobs[j], 0))
+                break;
+        }
+        if (!uniform || g == bp->groups.size()) { g = bp->groups.size(); bp->groups.emplace_back(); }
+        bp->groups[g].push_back(i);
+        bp->group[i] = g;
+    }
+    for (const std::vector<size_t>& members : bp->groups)
+    {
+        bp->firstUnit.push_back(bp->weight.size());
+        for (size_t j : members) bp->weight.insert(bp->weight.end(), bp->fp[j].chunk.weight.begin(), bp->fp[j].chunk.weight.end());
+    }
+    bp->firstUnit.push_back(bp->weight.size());
+    return bp->result;
+}
+
 } // namespace

@@ -333,6 +333,33 @@ DXB200_API int32_t  dxb200_levels_from_ex(const dxb200_image* base, size_t items
                                           uint32_t compressFlags, float threshold, const dxb200_chain_steps* steps, const dxb200_image* dst,
                                           int32_t* alphaAllOpaque, const dxb200_texconv_steps* ts);
 
+/* One texture of dxb200_texconv_batch: the arguments of the one-call pipeline named by kind.
+ *   kind 0 = dxb200_mipmaps_compress_from_channels_ex (compressFlags is its flags; convertFilter is not used),
+ *   kind 1 = dxb200_mipmaps_convert_from_ex (compressFlags is not used),
+ *   kind 2 = dxb200_levels_from_ex (filter is not used).
+ * alphaWeight is not in the record: every one of those calls ignores it. */
+typedef struct dxb200_texconv_job
+{
+    uint32_t kind;
+    const dxb200_image* base; size_t items; size_t levels;
+    const dxb200_chain_source* source; const dxb200_channel_steps* channels;
+    uint32_t filter;            /* GenerateMipMaps' filter (kinds 0, 1) */
+    const dxb200_chain_steps* steps; const dxb200_texconv_steps* ts;
+    uint32_t dstFormat; uint32_t convertFilter; uint32_t compressFlags; float threshold;
+    const dxb200_image* dst; int32_t* alphaAllOpaque;
+} dxb200_texconv_job;
+/* texconv over a list of textures of any sizes and formats in one call (texconv -r over a folder).  Job i's dst bytes and
+ * *alphaAllOpaque are identical to what the call named by its kind writes with the same arguments.  Every job is planned, with that
+ * call's own checks, before anything is uploaded; results[i] (when results != NULL) receives job i's HRESULT.  A job that fails its
+ * checks does not run and its dst is not written; the other jobs still run.  The return value is S_OK or the HRESULT of the
+ * lowest-index job that failed.  A device-side failure is returned and written into results[] of every job that was to run; their
+ * dst is then undefined.  jobs == NULL or njobs == 0 -> E_INVALIDARG.  No job's dst may overlap another job's base or dst.
+ * Jobs whose plans are equal apart from image pointers and row pitches (same kind, steps, formats, sizes and level counts) run as one
+ * multi-item call would, their items in job order; the (job, item) units are split over the initialised devices in contiguous
+ * ranges of about equal bytes, as every host call shards its items, and each device stages its share of every group through one
+ * pipeline of chunks, so that one texture's upload overlaps the previous one's kernels. */
+DXB200_API int32_t  dxb200_texconv_batch(const dxb200_texconv_job* jobs, size_t njobs, int32_t* results);
+
 /* ScratchImage::IsAlphaAllOpaque (DirectXTexImage.cpp:800-852; IsAlphaAllOpaqueBC, DirectXTexCompress.cpp:539-621) of
  * `nimages` images of one format: *opaque = 1 when every texel inside every image has alpha >= 0.997 (uncompressed, as
  * LoadScanline reads it) or >= 0.99 (decoded BC1 / BC2 / BC3 / BC7 blocks; the padding texels of partial blocks do not count),
