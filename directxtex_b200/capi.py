@@ -19,6 +19,7 @@ SYMBOLS = [
     "dxb200_apply_channel_steps", "dxb200_apply_channel_steps_device", "dxb200_mipmaps_compress_from_channels",
     "dxb200_mipmaps_convert_from", "dxb200_levels_from",
     "dxb200_mipmaps_compress_from_channels_ex", "dxb200_mipmaps_convert_from_ex", "dxb200_levels_from_ex", "dxb200_texconv_batch",
+    "dxb200_texconv_batch_device",
     "dxb200_dds_encode_header", "dxb200_dds_save_memory", "dxb200_dds_get_metadata", "dxb200_dds_load_memory",
 ]
 
@@ -118,6 +119,8 @@ def _load():
     lib.dxb200_levels_from_ex.argtypes = lib.dxb200_levels_from.argtypes + [TP]
     lib.dxb200_texconv_batch.argtypes = [C.POINTER(TexconvJob), C.c_size_t, C.POINTER(C.c_int32)]
     lib.dxb200_texconv_batch.restype = C.c_int32
+    lib.dxb200_texconv_batch_device.argtypes = [C.POINTER(TexconvJob), C.c_size_t, C.POINTER(C.c_int32), C.c_void_p]
+    lib.dxb200_texconv_batch_device.restype = C.c_int32
     lib.dxb200_apply_channel_steps.argtypes = [IP, C.c_size_t, C.POINTER(ChannelSteps), IP]
     lib.dxb200_apply_channel_steps_device.argtypes = [IP, C.c_size_t, C.POINTER(ChannelSteps), IP, C.c_void_p]
     lib.dxb200_is_alpha_all_opaque.argtypes = [IP, C.c_size_t, C.POINTER(C.c_int32)]
@@ -401,6 +404,18 @@ def texconv_batch(jobs):
     results = (C.c_int32 * len(built))()
     hr = lib.dxb200_texconv_batch(table, len(built), results)
     return F.hr_u32(hr), [(F.hr_u32(results[i]), built[i][1], opaque[i].value == 1) for i in range(len(built))]
+
+
+def texconv_batch_device(jobs, stream=None):
+    """dxb200_texconv_batch_device of a list of TexconvJob records whose base and dst pixels are device memory of one device (for
+    example torch CUDA tensors' data_ptr()), on `stream`: a torch.cuda.Stream, a raw cudaStream_t handle, or None for the legacy
+    default stream.  Returns (the batch's HRESULT, [HRESULT per job]).  Without a job asking for the alpha answer the work is only
+    enqueued: synchronise the stream before reading dst."""
+    handle = getattr(stream, "cuda_stream", stream)
+    table = (TexconvJob * len(jobs))(*jobs)
+    results = (C.c_int32 * len(jobs))()
+    hr = lib.dxb200_texconv_batch_device(table, len(jobs), results, handle)
+    return F.hr_u32(hr), [F.hr_u32(r) for r in results]
 
 
 def apply_channel_steps(arrays, w, h, fmt, channels, row_pitch=0):

@@ -355,10 +355,6 @@ int32_t launch_compress(const CompressPlan& plan, const dxb200_image* src, const
 }
 
 // ---- host staging -------------------------------------------------------------------------------------
-// One array of images of a staged call: item i owns images [i * per, (i + 1) * per) of `host`; image 0 of an item travels as
-// `first`, the others as `rest` (a mip chain uploads level 0 and makes the others).
-struct Plane { const dxb200_image* host; size_t per; Copy first, rest; };
-
 // fn(dev, count, stream) of a staged segment: enqueues the kernels of one chunk; dev[p] is plane p's images of the chunk's `count`
 // items, with device pointers
 using StageFn = std::function<int32_t(const std::vector<dxb200_image>*, size_t, cudaStream_t)>;
@@ -367,16 +363,14 @@ using StageFn = std::function<int32_t(const std::vector<dxb200_image>*, size_t, 
 struct Segment { const Plane* planes; size_t nplanes; size_t n; StageFn fn; };
 
 // Stages the items of every segment, in order, through the calling thread's lane.  Whole items of one segment are grouped into
-// chunks of at most `budget` bytes of device memory (an item larger than that is a chunk by itself; a chunk never spans two
-// segments), and chunk c of the call goes through slot c % NSLOT, so the H2D copies, kernels and D2H copies of consecutive chunks
-// overlap, from one segment to the next too (fully when the caller's memory is pinned, see dxb200_host_alloc).  In the slot's
-// buffer the chunk's images lie plane after plane, each on a 256-byte boundary, so equal images of one plane sit at a constant
-// stride (the vector kernels' alignment checks and the BC7 TMA feed rely on both).  prog (optional) is told before each chunk's
-// upload the units[] of the items the chunk completes (units counts the items of all segments in order), and stops the call
-// between chunks (E_ABORT).  Every slot is synchronised once, before returning; the first error wins.
+// chunks of at most `budget` bytes of device memory (chunk_end; a chunk never spans two segments), and chunk c of the call goes
+// through slot c % NSLOT, so the H2D copies, kernels and D2H copies of consecutive chunks overlap, from one segment to the next too
+// (fully when the caller's memory is pinned, see dxb200_host_alloc).  In the slot's buffer the chunk's images lie as chunk_layout
+// lays them out.  prog (optional) is told before each chunk's upload the units[] of the items the chunk completes (units counts the
+// items of all segments in order), and stops the call between chunks (E_ABORT).  Every slot is synchronised once, before returning;
+// the first error wins.
 int32_t run_segments(const Segment* segs, size_t nsegs, size_t budget, Progress* prog = nullptr, const size_t* units = nullptr)
 {
-    auto padded = [](const dxb200_image& im) { return (im.slicePitch + 255) & ~size_t(255); };
     Lane& L = *t_v.lane;
     int slot = 0;
     int32_t hr = DXB_S_OK;
@@ -388,15 +382,7 @@ int32_t run_segments(const Segment* segs, size_t nsegs, size_t budget, Progress*
         size_t i = 0;
         while (i < n && hr == DXB_S_OK)
         {
-            size_t bytes = 0, k = i;
-            while (k < n)
-            {
-                size_t b = 0;
-                for (size_t p = 0; p < nplanes; ++p)
-                    for (size_t m = k * planes[p].per; m < (k + 1) * planes[p].per; ++m) b += padded(planes[p].host[m]);
-                if (k > i && bytes + b > budget) break;
-                bytes += b; ++k;
-            }
+            const size_t k = chunk_end(planes, nplanes, i, n, budget);
             cudaStream_t st = L.streams[slot];
             hr = cuda_hr(cudaStreamSynchronize(st), "slot sync"); if (hr) break;
             if (prog)
@@ -405,20 +391,15 @@ int32_t run_segments(const Segment* segs, size_t nsegs, size_t budget, Progress*
                 for (size_t m = i; m < k; ++m) add += units[m];
                 if (!prog->report(add)) { hr = DXB_E_ABORT; break; }
             }
-            hr = ensure_buffer(&L.buf[slot], &L.cap[slot], bytes); if (hr) break;
-            size_t off = 0;
+            hr = ensure_buffer(&L.buf[slot], &L.cap[slot], chunk_bytes(planes, nplanes, i, k)); if (hr) break;
+            chunk_layout(planes, nplanes, i, k, nullptr, static_cast<uint8_t*>(L.buf[slot]), dev.data());
             for (size_t p = 0; p < nplanes && hr == DXB_S_OK; ++p)
             {
                 const Plane& pl = planes[p];
                 const dxb200_image* host = pl.host + i * pl.per;
-                dev[p].assign(host, pl.host + k * pl.per);
                 for (size_t m = 0; m < dev[p].size() && hr == DXB_S_OK; ++m)
-                {
-                    dev[p][m].pixels = static_cast<uint8_t*>(L.buf[slot]) + off;
-                    off += padded(dev[p][m]);
                     if ((m % pl.per ? pl.rest : pl.first) == Copy::Up)
                         hr = cuda_hr(cudaMemcpyAsync(dev[p][m].pixels, host[m].pixels, host[m].slicePitch, cudaMemcpyHostToDevice, st), "H2D");
-                }
             }
             if (hr) break;
             hr = segs[sg].fn(dev.data(), k - i, st); if (hr) break;
@@ -680,14 +661,6 @@ struct ResultWords
     bool all_zero() const { return std::all_of(w, w + n, [](uint32_t v) { return v == 0; }); }
 };
 
-// The staged planes of items [lo, ...) of a chunk plan: host[r] = the host images of role r, ck.planes[p].per per item
-std::vector<Plane> chain_planes(const ChunkPlan& ck, const dxb200_image* const* host, size_t lo)
-{
-    std::vector<Plane> planes;
-    for (const ChunkPlane& p : ck.planes) planes.push_back({ host[(size_t)p.role] + lo * p.per, p.per, p.first, p.rest });
-    return planes;
-}
-
 // The launches of one chunk of `cnt` items of fp.chunk: dev[p] = plane p's device images
 int32_t run_chunk(const FromPlan& fp, const AlphaOpaquePlan& scan, size_t levels, const std::vector<dxb200_image>* dev, size_t cnt, cudaStream_t st)
 {
@@ -788,37 +761,68 @@ int32_t run_chains(const dxb200_image* base, size_t items, size_t levels, const 
     return hr;
 }
 
-// dxb200_texconv_batch once every job is planned: group g's items are units bp.firstUnit[g] .. firstUnit[g + 1], split over the
-// devices by run_sharded; each device stages its units of every group as one segment per group, through one lane, with the launches
-// of the group's first job's plan (equal to every member's).  The alpha answer of a job is the AND of its items' words.
-int32_t run_batch(const dxb200_texconv_job* jobs, const BatchPlan& bp)
+// The caller's images of every role of every group of a batch, its jobs' images in job order: host[g * PLANE_ROLES + r] = group g's
+// images of role r; the words of group g start at unit bp.firstUnit[g] of wimg.  roles holds the arrays host points into.
+void batch_roles(const dxb200_texconv_job* jobs, const BatchPlan& bp, const std::vector<dxb200_image>& wimg,
+                 std::vector<std::vector<dxb200_image>>* roles, std::vector<const dxb200_image*>* host)
 {
-    const size_t ng = bp.groups.size(), units = bp.firstUnit.back();
-    bool scan = false;
-    for (const std::vector<size_t>& members : bp.groups) scan |= bp.ap[members[0]].scan;
-    ResultWords words;
-    int32_t hr = scan ? words.alloc(units) : DXB_S_OK;
-    if (hr != DXB_S_OK) return hr;
-    const std::vector<dxb200_image> wimg = words.images();
-    // the host images of every role of every group: its jobs' images in job order
-    std::vector<std::vector<dxb200_image>> roles(ng * PLANE_ROLES);
-    std::vector<const dxb200_image*> host(ng * PLANE_ROLES, nullptr);
+    const size_t ng = bp.groups.size();
+    roles->assign(ng * PLANE_ROLES, std::vector<dxb200_image>());
+    host->assign(ng * PLANE_ROLES, nullptr);
     for (size_t g = 0; g < ng; ++g)
     {
+        std::vector<dxb200_image>* r = &(*roles)[g * PLANE_ROLES];
         for (size_t j : bp.groups[g])
         {
             const FromPlan& fp = bp.fp[j];
             const size_t n = jobs[j].items * fp.chunk.per, all = jobs[j].items * jobs[j].levels;
-            std::vector<dxb200_image>* r = &roles[g * PLANE_ROLES];
             r[(size_t)PlaneRole::Base].insert(r[(size_t)PlaneRole::Base].end(), jobs[j].base, jobs[j].base + n);
             r[(size_t)PlaneRole::Decompressed].insert(r[(size_t)PlaneRole::Decompressed].end(), fp.decompressed.begin(), fp.decompressed.end());
             r[(size_t)PlaneRole::Level0].insert(r[(size_t)PlaneRole::Level0].end(), fp.level0.begin(), fp.level0.end());
             r[(size_t)PlaneRole::Chain].insert(r[(size_t)PlaneRole::Chain].end(), fp.chain.chain.begin(), fp.chain.chain.end());
             r[(size_t)PlaneRole::Dst].insert(r[(size_t)PlaneRole::Dst].end(), jobs[j].dst, jobs[j].dst + all);
         }
-        for (size_t r = 0; r < PLANE_ROLES; ++r) host[g * PLANE_ROLES + r] = roles[g * PLANE_ROLES + r].data();
-        if (scan) host[g * PLANE_ROLES + (size_t)PlaneRole::Words] = wimg.data() + bp.firstUnit[g];
+        for (size_t k = 0; k < PLANE_ROLES; ++k) (*host)[g * PLANE_ROLES + k] = r[k].data();
+        if (!wimg.empty()) (*host)[g * PLANE_ROLES + (size_t)PlaneRole::Words] = wimg.data() + bp.firstUnit[g];
     }
+}
+
+// whether any group of a batch runs the alpha scan
+bool batch_scans(const BatchPlan& bp)
+{
+    bool scan = false;
+    for (const std::vector<size_t>& members : bp.groups) scan |= bp.ap[members[0]].scan;
+    return scan;
+}
+
+// *alphaAllOpaque of every job that ran: the AND of its items' words (1 when it has no scan)
+void batch_answers(const dxb200_texconv_job* jobs, const BatchPlan& bp, const ResultWords& words)
+{
+    for (size_t g = 0; g < bp.groups.size(); ++g)
+    {
+        size_t u = bp.firstUnit[g];
+        for (size_t j : bp.groups[g])
+        {
+            const bool opaque = !bp.ap[j].scan || std::all_of(words.w + u, words.w + u + jobs[j].items, [](uint32_t v) { return v == 0; });
+            if (jobs[j].alphaAllOpaque) *jobs[j].alphaAllOpaque = opaque ? 1 : 0;
+            u += jobs[j].items;
+        }
+    }
+}
+
+// dxb200_texconv_batch once every job is planned: group g's items are units bp.firstUnit[g] .. firstUnit[g + 1], split over the
+// devices by run_sharded; each device stages its units of every group as one segment per group, through one lane, with the launches
+// of the group's first job's plan (equal to every member's).  The alpha answer of a job is the AND of its items' words.
+int32_t run_batch(const dxb200_texconv_job* jobs, const BatchPlan& bp)
+{
+    const size_t ng = bp.groups.size(), units = bp.firstUnit.back();
+    ResultWords words;
+    int32_t hr = batch_scans(bp) ? words.alloc(units) : DXB_S_OK;
+    if (hr != DXB_S_OK) return hr;
+    const std::vector<dxb200_image> wimg = words.images();
+    std::vector<std::vector<dxb200_image>> roles;
+    std::vector<const dxb200_image*> host;
+    batch_roles(jobs, bp, wimg, &roles, &host);
     hr = run_sharded(units, [&](size_t i) { return bp.weight[i]; },
         [&](size_t lo, size_t hi)
         {
@@ -839,17 +843,99 @@ int32_t run_batch(const dxb200_texconv_job* jobs, const BatchPlan& bp)
             return run_segments(segs.data(), segs.size(), ITEM_CHUNK);
         });
     if (hr != DXB_S_OK) return hr;
-    for (size_t g = 0; g < ng; ++g)
+    batch_answers(jobs, bp, words);
+    return DXB_S_OK;
+}
+
+// A job of dxb200_texconv_batch_device may run when every base and dst image lies in device or managed memory of device `ord` and
+// every BC image's pixel pointer is a whole number of blocks from 0 (bc_pointers_ok): E_INVALIDARG otherwise, so that a wrong pointer
+// is refused before any launch instead of faulting a kernel
+int32_t device_job_ok(const dxb200_texconv_job& j, size_t per, int ord)
+{
+    const dxb200_image* sets[2] = { j.base, j.dst };
+    const size_t counts[2] = { j.items * per, j.items * j.levels };
+    for (int s = 0; s < 2; ++s)
     {
-        size_t u = bp.firstUnit[g];
-        for (size_t j : bp.groups[g])
+        if (!bc_pointers_ok(sets[s], counts[s])) return DXB_E_INVALIDARG;
+        for (size_t i = 0; i < counts[s]; ++i)
         {
-            const bool opaque = !bp.ap[j].scan || std::all_of(words.w + u, words.w + u + jobs[j].items, [](uint32_t v) { return v == 0; });
-            if (jobs[j].alphaAllOpaque) *jobs[j].alphaAllOpaque = opaque ? 1 : 0;
-            u += jobs[j].items;
+            cudaPointerAttributes a;
+            const cudaError_t e = cudaPointerGetAttributes(&a, sets[s][i].pixels);
+            (void)cudaGetLastError();
+            if (e != cudaSuccess || (a.type != cudaMemoryTypeDevice && a.type != cudaMemoryTypeManaged) || a.device != ord)
+                return DXB_E_INVALIDARG;
         }
     }
     return DXB_S_OK;
+}
+
+// One chunk of a _device batch: items [i, k) of group g, whose planes lie chunk_bytes(..., alias) bytes into scratch memory
+struct DeviceChunk { size_t g, i, k; };
+
+// dxb200_texconv_batch_device once every job is planned and checked: every group's units on the calling thread's device and
+// `stream`, in chunks cut as run_segments cuts them.  A chunk's aliased planes (device_aliases) are the caller's images; the others lie
+// in one scratch allocation, sized for the largest chunk and reused chunk after chunk (stream order makes that safe), as the slot
+// buffer lays them out, with their Copy::Up images copied in device to device.  Each chunk's result words are read back into pinned
+// memory behind its launches; only when a job asks for the alpha answer is the stream synchronised, at the end.
+int32_t run_batch_device(const dxb200_texconv_job* jobs, const BatchPlan& bp, cudaStream_t st)
+{
+    const size_t ng = bp.groups.size();
+    const bool scan = batch_scans(bp);
+    ResultWords words;
+    int32_t hr = scan ? words.alloc(bp.firstUnit.back()) : DXB_S_OK;
+    if (hr != DXB_S_OK) return hr;
+    const std::vector<dxb200_image> wimg = words.images();
+    std::vector<std::vector<dxb200_image>> roles;
+    std::vector<const dxb200_image*> host;
+    batch_roles(jobs, bp, wimg, &roles, &host);
+    std::vector<std::vector<Plane>> planes(ng);
+    std::vector<std::vector<bool>> alias(ng);
+    std::vector<DeviceChunk> chunks;
+    size_t scratch = 0;
+    for (size_t g = 0; g < ng; ++g)
+    {
+        const ChunkPlan& ck = bp.fp[bp.groups[g][0]].chunk;
+        planes[g] = chain_planes(ck, &host[g * PLANE_ROLES], 0);
+        alias[g] = device_aliases(ck);
+        const size_t n = bp.firstUnit[g + 1] - bp.firstUnit[g];
+        for (size_t i = 0, k; i < n; i = k)
+        {
+            k = chunk_end(planes[g].data(), planes[g].size(), i, n, ITEM_CHUNK);
+            chunks.push_back({ g, i, k });
+            scratch = std::max(scratch, chunk_bytes(planes[g].data(), planes[g].size(), i, k, &alias[g]));
+        }
+    }
+    uint8_t* buf = nullptr;
+    DXB_CUDA(cudaMallocAsync(reinterpret_cast<void**>(&buf), std::max<size_t>(scratch, 1), st));
+    std::vector<dxb200_image> dev[PLANE_ROLES];
+    for (size_t c = 0; c < chunks.size() && hr == DXB_S_OK; ++c)
+    {
+        const DeviceChunk& ch = chunks[c];
+        const std::vector<Plane>& pl = planes[ch.g];
+        chunk_layout(pl.data(), pl.size(), ch.i, ch.k, &alias[ch.g], buf, dev);
+        for (size_t p = 0; p < pl.size() && hr == DXB_S_OK; ++p)
+        {
+            const dxb200_image* src = pl[p].host + ch.i * pl[p].per;
+            for (size_t m = 0; m < dev[p].size() && hr == DXB_S_OK && !alias[ch.g][p]; ++m)
+                if ((m % pl[p].per ? pl[p].rest : pl[p].first) == Copy::Up)
+                    hr = cuda_hr(cudaMemcpyAsync(dev[p][m].pixels, src[m].pixels, src[m].slicePitch, cudaMemcpyDeviceToDevice, st), "copy in");
+        }
+        const size_t j = bp.groups[ch.g][0];
+        if (hr == DXB_S_OK) hr = run_chunk(bp.fp[j], bp.ap[j], jobs[j].levels, dev, ch.k - ch.i, st);
+        // the words of a chunk lie padded_bytes (256) apart in scratch, one per item, and go to consecutive host words
+        for (size_t p = 0; p < pl.size() && hr == DXB_S_OK; ++p)
+        {
+            if (bp.fp[j].chunk.planes[p].role != PlaneRole::Words) continue;
+            const std::vector<dxb200_image>& w = dev[p];
+            hr = cuda_hr(cudaMemcpy2DAsync(words.w + bp.firstUnit[ch.g] + ch.i, sizeof(uint32_t), w[0].pixels, padded_bytes(w[0]), sizeof(uint32_t),
+                                           w.size(), cudaMemcpyDeviceToHost, st), "alpha words");
+        }
+    }
+    const int32_t hf = cuda_hr(cudaFreeAsync(buf, st), "cudaFreeAsync(scratch)");
+    if (hr == DXB_S_OK) hr = hf;
+    if (hr == DXB_S_OK && scan) hr = cuda_hr(cudaStreamSynchronize(st), "alpha answer sync");       // the answer is a host value
+    if (hr == DXB_S_OK) batch_answers(jobs, bp, words);
+    return hr;
 }
 
 } // namespace
@@ -1196,6 +1282,28 @@ int32_t dxb200_texconv_batch(const dxb200_texconv_job* jobs, size_t njobs, int32
     (void)plan_texconv_batch(jobs, njobs, &bp);          // each job's HRESULT is in bp.hr
     if (!bp.groups.empty())
         if (const int32_t hr = run_batch(jobs, bp))
+            for (size_t i = 0; i < njobs; ++i) if (bp.group[i] != SIZE_MAX) bp.hr[i] = hr;
+    if (results) std::copy(bp.hr.begin(), bp.hr.end(), results);
+    for (int32_t hr : bp.hr) if (hr != DXB_S_OK) return hr;
+    return DXB_S_OK;
+}
+
+// ---- the same on textures in device memory, on the caller's stream (run_batch_device) -------------------------------------------
+int32_t dxb200_texconv_batch_device(const dxb200_texconv_job* jobs, size_t njobs, int32_t* results, void* stream)
+{
+    if (!jobs || !njobs) return DXB_E_INVALIDARG;
+    // the device is entered when the first job passes its planner, so that a batch of failing jobs needs none
+    DevScope scope;
+    bool entered = false;
+    int32_t hs = DXB_S_OK;
+    BatchPlan bp;
+    (void)plan_texconv_batch(jobs, njobs, &bp, [&](size_t i)
+    {
+        if (!entered) { entered = true; hs = scope.enter(jobs[0].base && jobs[0].items ? jobs[0].base[0].pixels : nullptr); }
+        return hs != DXB_S_OK ? hs : device_job_ok(jobs[i], bp.fp[i].chunk.per, scope.ord);
+    });
+    if (!bp.groups.empty())
+        if (const int32_t hr = run_batch_device(jobs, bp, static_cast<cudaStream_t>(stream)))
             for (size_t i = 0; i < njobs; ++i) if (bp.group[i] != SIZE_MAX) bp.hr[i] = hr;
     if (results) std::copy(bp.hr.begin(), bp.hr.end(), results);
     for (int32_t hr : bp.hr) if (hr != DXB_S_OK) return hr;

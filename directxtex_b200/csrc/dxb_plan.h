@@ -628,6 +628,75 @@ int32_t plan_chunk(const dxb200_image* dst, size_t items, size_t levels, uint32_
     return DXB_S_OK;
 }
 
+// ---- how a chunk's images lie in device memory (run_segments, run_batch_device) ----------------------------------------------------
+// One array of images of a staged call: item i owns images [i * per, (i + 1) * per) of `host`; image 0 of an item travels as
+// `first`, the others as `rest` (a mip chain uploads level 0 and makes the others).
+struct Plane { const dxb200_image* host; size_t per; Copy first, rest; };
+
+// The planes of items [lo, ...) of a chunk plan: host[r] = the caller's images of role r, ck.planes[p].per per item
+std::vector<Plane> chain_planes(const ChunkPlan& ck, const dxb200_image* const* host, size_t lo)
+{
+    std::vector<Plane> planes;
+    for (const ChunkPlane& p : ck.planes) planes.push_back({ host[(size_t)p.role] + lo * p.per, p.per, p.first, p.rest });
+    return planes;
+}
+
+// every image of a chunk starts on a 256-byte boundary
+size_t padded_bytes(const dxb200_image& im) { return (im.slicePitch + 255) & ~size_t(255); }
+
+// The device bytes of items [i, k) of the planes not aliased to the caller's images (alias == nullptr: of every plane)
+size_t chunk_bytes(const Plane* planes, size_t nplanes, size_t i, size_t k, const std::vector<bool>* alias = nullptr)
+{
+    size_t b = 0;
+    for (size_t p = 0; p < nplanes; ++p)
+        if (!alias || !(*alias)[p])
+            for (size_t m = i * planes[p].per; m < k * planes[p].per; ++m) b += padded_bytes(planes[p].host[m]);
+    return b;
+}
+
+// The end of the chunk that starts at item i of n: whole items while every plane's bytes fit `budget`; an item larger than that is
+// a chunk by itself.  Host staging and a _device call cut the same chunks, so they run the same launches.
+size_t chunk_end(const Plane* planes, size_t nplanes, size_t i, size_t n, size_t budget)
+{
+    size_t bytes = 0, k = i;
+    for (; k < n; ++k)
+    {
+        const size_t b = chunk_bytes(planes, nplanes, k, k + 1);
+        if (k > i && bytes + b > budget) break;
+        bytes += b;
+    }
+    return k;
+}
+
+// Items [i, k) of a chunk: dev[p] = plane p's images at their row pitches.  An aliased plane keeps the caller's pixels; every other
+// image takes the next 256-byte boundary of buf, plane after plane, so equal images of one plane lie at a constant stride (the vector
+// kernels' alignment checks and the BC7 TMA feed rely on both).  Takes chunk_bytes(planes, nplanes, i, k, alias) bytes of buf.
+void chunk_layout(const Plane* planes, size_t nplanes, size_t i, size_t k, const std::vector<bool>* alias, uint8_t* buf,
+                  std::vector<dxb200_image>* dev)
+{
+    size_t off = 0;
+    for (size_t p = 0; p < nplanes; ++p)
+    {
+        dev[p].assign(planes[p].host + i * planes[p].per, planes[p].host + k * planes[p].per);
+        if (alias && (*alias)[p]) continue;
+        for (dxb200_image& im : dev[p]) { im.pixels = buf + off; off += padded_bytes(im); }
+    }
+}
+
+// Where each plane of a chunk lives on a _device call (dxb200_texconv_batch_device): aliased[p] = plane p is the caller's images.
+// Dst is, since it is the output.  Base is when no step writes it (the demultiply and the swizzle in front of a Convert may run in
+// place on it): the caller's inputs are never written.  Every other plane lies in scratch memory, with its Copy::Up images copied in
+// device to device; only Words has Copy::Down images in scratch, which are read back.
+std::vector<bool> device_aliases(const ChunkPlan& ck)
+{
+    bool baseWritten = false;
+    for (const ChunkStep& s : ck.steps) baseWritten |= s.dst == PlaneRole::Base;
+    std::vector<bool> alias(ck.planes.size());
+    for (size_t p = 0; p < ck.planes.size(); ++p)
+        alias[p] = ck.planes[p].role == PlaneRole::Dst || (ck.planes[p].role == PlaneRole::Base && !baseWritten);
+    return alias;
+}
+
 // image i of `n` of format fmt, w x h, at compute_pitch, with the pixels of base[i]
 std::vector<dxb200_image> plan_images(const dxb200_image* base, size_t n, uint32_t fmt, size_t w, size_t h)
 {
@@ -990,7 +1059,9 @@ struct BatchPlan
     int32_t result = DXB_S_OK;
 };
 
-int32_t plan_texconv_batch(const dxb200_texconv_job* jobs, size_t njobs, BatchPlan* bp)
+// check(i) = the HRESULT of checks a caller adds to job i's once its planner has passed (the _device call's pointer checks)
+template <typename CheckFn>
+int32_t plan_texconv_batch(const dxb200_texconv_job* jobs, size_t njobs, BatchPlan* bp, CheckFn check)
 {
     if (!jobs || !njobs) return DXB_E_INVALIDARG;
     bp->hr.assign(njobs, DXB_S_OK);
@@ -1002,6 +1073,7 @@ int32_t plan_texconv_batch(const dxb200_texconv_job* jobs, size_t njobs, BatchPl
     for (size_t i = 0; i < njobs; ++i)
     {
         bp->hr[i] = plan_texconv_job(jobs[i], &bp->fp[i], &bp->ap[i]);
+        if (bp->hr[i] == DXB_S_OK) bp->hr[i] = check(i);
         if (bp->hr[i] != DXB_S_OK)
         {
             if (bp->result == DXB_S_OK) bp->result = bp->hr[i];
@@ -1029,6 +1101,11 @@ int32_t plan_texconv_batch(const dxb200_texconv_job* jobs, size_t njobs, BatchPl
     }
     bp->firstUnit.push_back(bp->weight.size());
     return bp->result;
+}
+
+int32_t plan_texconv_batch(const dxb200_texconv_job* jobs, size_t njobs, BatchPlan* bp)
+{
+    return plan_texconv_batch(jobs, njobs, bp, [](size_t) { return DXB_S_OK; });
 }
 
 } // namespace

@@ -359,6 +359,18 @@ typedef struct dxb200_texconv_job
  * ranges of about equal bytes, as every host call shards its items, and each device stages its share of every group through one
  * pipeline of chunks, so that one texture's upload overlaps the previous one's kernels. */
 DXB200_API int32_t  dxb200_texconv_batch(const dxb200_texconv_job* jobs, size_t njobs, int32_t* results);
+/* dxb200_texconv_batch on textures already in device memory: every base and dst pixel pointer of every job is device (or managed)
+ * memory of one device.  Job i's dst bytes, *alphaAllOpaque, results[i] and the return value are what dxb200_texconv_batch gives
+ * for the same jobs on host copies of the same images.  The call runs on the device that owns job 0's base pixels, on `stream`
+ * (NULL = the legacy default stream); it neither shards over devices nor uses the host calls' staging buffers, so calls on
+ * different streams do not wait for each other.  Base images are never written.  Once a job has passed its planner's checks,
+ * an image that is not device or managed memory of that device (pageable or pinned host memory, another device's memory), or a
+ * BC image whose pixel pointer is not a multiple of its block size, makes it E_INVALIDARG: it does not run and its dst is not
+ * written.  Scratch memory comes from the device's stream-ordered pool (cudaMallocAsync on `stream`).
+ * With no job asking for the alpha answer (alphaAllOpaque == NULL), the call only enqueues its work on `stream` and returns without
+ * synchronising: dst is complete when the stream's work up to the call is.  When a job asks, the answer is a host value, so the
+ * call synchronises `stream` before it returns, as dxb200_is_alpha_all_opaque_device does. */
+DXB200_API int32_t  dxb200_texconv_batch_device(const dxb200_texconv_job* jobs, size_t njobs, int32_t* results, void* stream);
 
 /* ScratchImage::IsAlphaAllOpaque (DirectXTexImage.cpp:800-852; IsAlphaAllOpaqueBC, DirectXTexCompress.cpp:539-621) of
  * `nimages` images of one format: *opaque = 1 when every texel inside every image has alpha >= 0.997 (uncompressed, as
